@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the CosyVoice2-0.5B hot path (LM decode -> CFM flow -> HiFT vocoder) on B200.
+"""Benchmark of the CosyVoice2-0.5B hot path (LM decode -> CFM flow -> HiFT vocoder) on H100.
 
 Metric (BASELINE.json): audio-sec/s, CosyVoice2-0.5B zero-shot batch-32, NFE=10 - synthetic data (random-init weights of
 the reference architecture, random token / prompt tensors of the Z10 shape, SURVEY.md §8d).  One *step* = one pass of
@@ -9,6 +9,7 @@ the whole pipeline over one batch of 32 ragged utterances per GPU.
   python bench.py --impl reference --steps 1 --warmup 0    # the reference's algorithm on the host CPU cores
   torchrun --nnodes=1 --nproc-per-node N bench.py --gpus N ...   (N > 1: one rank per GPU; primary = the same 32 requests
                                                                    sharded over the ranks, "weak" key = 32 requests per rank)
+  python bench.py --steps 3 --warmup 3 --dump-outputs DIR  # also write what the last timed step computed, DIR/<name>.npy
 
 Prints ONE JSON line on rank 0 (contract in the task statement): value = device-resident throughput, e2e = the same
 metric through the public API with host buffers (H2D of the request tensors, D2H of the waveforms inside the timed
@@ -35,11 +36,11 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured (MEASURED_PEAKS.json, sustained)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="H100 SXM data sheet (dense bf16, 700 W card), not a measured peak")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -192,6 +193,24 @@ def stage_roofline(stats, inputs, pk, nfe=10):
 
 
 # ================================================================================================ our arm (GPU)
+DUMP_MAX_FLOATS = 16 * 1024 * 1024       # 64 MB of float32 at most
+
+
+def dump_outputs(out_dir, wav, n):
+    """The arrays a caller of tts_batch_device receives from the last timed step: the waveform buffer (float32, the utterances
+    back to back) and the per-utterance sample counts.  A waveform larger than DUMP_MAX_FLOATS is replaced by a fixed, seeded
+    sample of its positions (wav_index.npy) so that two builds can still be compared value for value."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    w = wav[:sum(n)].float().cpu().numpy()
+    if w.size > DUMP_MAX_FLOATS:
+        idx = np.sort(np.random.default_rng(0).choice(w.size, DUMP_MAX_FLOATS, replace=False))
+        np.save(os.path.join(out_dir, "wav_index.npy"), idx.astype(np.float64))
+        w = w[idx]
+    np.save(os.path.join(out_dir, "wav.npy"), w.astype(np.float32))
+    np.save(os.path.join(out_dir, "wav_lens.npy"), np.asarray(n, dtype=np.float64))
+
+
 def run_ours(args):
     import torch
     rank, world, local = dist_env()
@@ -246,10 +265,11 @@ def run_ours(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0 = time.perf_counter()
         e0.record(model.stream)
-        audio_s, stats = 0.0, None
+        audio_s, stats, wav = 0.0, None, None
         for _ in range(args.steps):
-            _, n, stats = model.tts_batch_device(inputs_dev)
+            wav, n, stats = model.tts_batch_device(inputs_dev)
             audio_s += sum(n) / 24000.0
+        last = (wav, n)                                # what the last timed step computed (for --dump-outputs)
         e1.record(model.stream)
         barrier()
         dev_ms = e0.elapsed_time(e1)
@@ -285,12 +305,14 @@ def run_ours(args):
         dev_ms, e2e_ms, wall_ms = tt.tolist()
         audio_s, audio_e2e, launches, h2d_all = aa.tolist()
         return dict(value=audio_s / (dev_ms / 1000.0), e2e=audio_e2e / (e2e_ms / 1000.0), dev_ms=dev_ms, e2e_ms=e2e_ms, wall_ms=wall_ms,
-                    launches=int(launches), h2d=int(h2d_all), d2h=int(d2h), clocks=clocks, stats=stats, inputs=inputs)
+                    launches=int(launches), h2d=int(h2d_all), d2h=int(d2h), clocks=clocks, stats=stats, inputs=inputs, last=last)
 
     # ---- primary: the contract's split - the SAME `batch` utterances sharded over the ranks (strong scaling), LPT on expected tokens
     all_inputs = synth.batch32_zero_shot(batch)
     plan = shard_lpt([int(i["text"].shape[1] * TOKEN_RATIO) for i in all_inputs], world)
     strong = measure([all_inputs[i] for i in plan[rank]], [len(p) for p in plan], True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *strong["last"])
     # ---- one extra instrumented step (CUDA events around every GEMM / attention launch) for the per-family roofline
     model.ctx.profile(1)
     model.tts_batch_device([{k: v.to(dev) for k, v in i.items()} for i in strong["inputs"]])
@@ -306,18 +328,12 @@ def run_ours(args):
     pk = peaks()
     value, e2e_v, dev_ms = strong["value"], strong["e2e"], strong["dev_ms"]
     # dominant kernel family = the one with the largest share of device time (instrumented step)
-    fam_names = ["conv_gemm_tc (tcgen05 bf16)", "conv_gemm_simt (fp32 CUDA cores)", "attention (tcgen05 flash kernels; fp32-math CUDA-core kernel in fp32 mode)"]
+    fam_names = ["conv_gemm_tc (wgmma bf16)", "conv_gemm_simt (fp32 CUDA cores)", "attention (wgmma flash kernels; fp32-math CUDA-core kernel in fp32 mode)"]
     dom = max(range(3), key=lambda f: prof[f]["ms"])
     p = prof[dom]
     ach = p["flops"] / (p["ms"] / 1000.0) / 1e12 if p["ms"] > 0 else 0.0
     roof = {"bound": "tensor", "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"]}
-    traffic, traffic_note = None, "no ncu capture committed for this kernel"
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if dom == 0 and os.path.exists(tpath):            # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch from `ncu --set full`
-            tj = json.load(open(tpath))
-            traffic, traffic_note = tj["dram_bytes_per_launch"], tj["note"]
-            break
+    traffic, traffic_note = None, "DRAM traffic not measured"
     step_ms = dev_ms / args.steps
     roof.update({"traffic": traffic, "traffic_note": traffic_note, "kernel": fam_names[dom], "launches": p["launches"], "avg_launch_ms": p["ms"] / max(p["launches"], 1),
                  "share_of_step": p["ms"] / step_ms, "peak_source": pk["source"], "timed": "one extra instrumented step (not inside the `value` region)",
@@ -336,7 +352,7 @@ def run_ours(args):
                                    f"{per_gpu} per GPU), NFE=10, 40-60 text tokens -> 200-300 speech tokens, 75 prompt tokens / 150 prompt mel frames"
                                    + ("" if full else " [SMALL DEBUG MODEL]"),
                        "global_batch": batch, "per_gpu": per_gpu, "nfe": 10,
-                       "l2": "working set (1.3 GB weights + GBs of activations) exceeds the 126 MB L2",
+                       "l2": "working set (1.3 GB weights + GBs of activations) exceeds the 50 MB L2",
                        "parallelism": f"dp{n_gpus} (independent utterances, weights broadcast once over NCCL, waveform buffers gathered device-to-device on rank 0)",
                        "stage_ms_last_step_rank0": {k: stats[k] for k in ("lm_ms", "flow_ms", "hift_ms")}, "rtf": 1.0 / value},
             "e2e": {"value": e2e_v, "unit": "audio-sec/s", "h2d_bytes_per_step": strong["h2d"], "d2h_bytes_per_step": strong["d2h"]},
@@ -446,9 +462,13 @@ def main():
     ap.add_argument("--workspace-gb", type=float, default=40.0)
     ap.add_argument("--lm-chains", type=int, default=1)
     ap.add_argument("--opt", action="append", default=[], help="library option key=value (cvk_set_option), repeatable")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (batch32 workload)")
     ap.add_argument("--workload", default="batch32", choices=["batch32", "cv3-bistream"],
                     help="batch32 = the headline metric (BASELINE.json configs[2]); cv3-bistream = configs[3] (1 GPU)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "batch32"):
+        ap.error("--dump-outputs is implemented for the GPU batch32 workload only (--impl ours --workload batch32)")
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "cv3-bistream":

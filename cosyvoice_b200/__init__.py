@@ -1,2 +1,2 @@
-"""B200-native CosyVoice2 hot path: hand-written sm_100a kernels behind the C ABI of include/cvk.h."""
+"""H100-native CosyVoice2 hot path: hand-written sm_90a kernels behind the C ABI of include/cvk.h."""
 __version__ = "0.1"

@@ -2,7 +2,7 @@
 
 The reference serves one request per thread: every FastAPI / gRPC handler calls ``cosyvoice.inference_*`` itself and streams
 ``(tts_speech.numpy() * 2**15).astype(np.int16).tobytes()`` back (runtime/python/fastapi/server.py:40-43,
-runtime/python/grpc/server.py:62-64).  On a B200 a single utterance leaves the GPU launch-bound, while the batched pipeline
+runtime/python/grpc/server.py:62-64).  On a GPU of this class a single utterance leaves the GPU launch-bound, while the batched pipeline
 (``B200CosyVoice2Model.tts_batch``) is what the headline metric measures - so the step after the hot path is a queue that turns
 concurrent requests into ragged batches.  This module is that queue and nothing else: no HTTP / gRPC layer, no text
 normalisation, no tokenizer (those stay with the reference's frontend and server code, which call ``submit`` instead of

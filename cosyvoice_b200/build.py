@@ -1,4 +1,4 @@
-"""Build libcvk.so in-tree with nvcc for sm_100a (no torch, no cmake).  The .so travels to the GPU box."""
+"""Build libcvk.so in-tree with nvcc for sm_90a (H100; no torch, no cmake).  No GPU is needed to build."""
 import hashlib
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcvk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-DCVK_BUILD"]
 
 
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
         fail |= p.returncode != 0
     if fail:
         raise RuntimeError("nvcc failed")
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     open(stamp, "w").write(dig)
     return LIB

@@ -62,7 +62,7 @@ void prompt_feat_init(cvk_ctx* ctx);
 
 extern "C" {
 
-const char* cvk_version(void) { return "libcvk 0.1 (sm_100a)"; }
+const char* cvk_version(void) { return "libcvk 0.1 (sm_90a)"; }
 
 int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out) {
   if (!out) return CVK_ERR_INVALID;
@@ -73,7 +73,7 @@ int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out)
   if (cudaSetDevice(device) != cudaSuccess) return CVK_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return CVK_ERR_CUDA;
-  if (prop.major != 10) return CVK_ERR_CUDA;   // sm_100a only: the tcgen05/TMA kernels have no other code path
+  if (prop.major != 9) return CVK_ERR_CUDA;    // sm_90a only: the wgmma/TMA kernels have no other code path
   cvk_ctx* ctx = new cvk_ctx();
   ctx->device = device;
   ctx->precision = precision;
@@ -106,14 +106,9 @@ thread_local int cvk_in_capture = 0;
 int64_t cvk_launch_count(cvk_ctx* ctx) { return ctx ? ctx->launches.load() : 0; }
 double cvk_last_op_ms(cvk_ctx* ctx) { return ctx ? ctx->op_ms : 0.0; }
 int cvk_debug_read(cvk_ctx* ctx, long long* out, int n) {
-  if (ctx && ctx->tl && out && n == 4096) {   // LM-chain timeline
-    if (cudaMemcpy(out, ctx->tl, 4096 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return CVK_ERR_CUDA;
-    return CVK_OK;
-  }
-  if (!ctx || !ctx->dbg || !out || n > 1024) return CVK_ERR_INVALID;
+  if (!ctx || !ctx->tl || !out || n != 4096) return CVK_ERR_INVALID;   // the LM-chain timeline ("chain_timeline")
   cudaSetDevice(ctx->device);
-  if (cudaMemcpy(out, ctx->dbg, (size_t)n * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return CVK_ERR_CUDA;
-  cudaMemset(ctx->dbg, 0, 1024 * sizeof(long long));
+  if (cudaMemcpy(out, ctx->tl, 4096 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return CVK_ERR_CUDA;
   return CVK_OK;
 }
 
@@ -121,8 +116,6 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   CVK_API_BEGIN
   std::string k(key ? key : "");
   if (k == "use_tc") ctx->use_tc = value;
-  else if (k == "tc_bn256") ctx->tc_bn256 = value;
-  else if (k == "tc_pbn256") ctx->tc_pbn256 = value;
   else if (k == "tc_epi") ctx->tc_epi = value;
   else if (k == "tc_persist") ctx->tc_persist = value;
   else if (k == "op_out_bf16") ctx->op_out_bf16 = value;
@@ -133,7 +126,6 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   else if (k == "lm_fused") ctx->lm_fused = value;
   else if (k == "pdl") ctx->pdl = value;
   else if (k == "lm_mega") ctx->lm_mega = value;
-  else if (k == "attn_single_pass") ctx->attn_single_pass = value;
   else if (k == "enc_tc_attn") ctx->enc_tc_attn = value;
   else if (k == "hift_f16") ctx->hift_f16 = value;      // takes effect at the next cvk_finalize("hift" / "hift3")
   else if (k == "mega_coop") ctx->mega_coop = value;
@@ -143,13 +135,6 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
       CVK_CHECK_CUDA(cudaMemset(ctx->tl, 0, 4096 * sizeof(long long)));
     }
     if (!value) ctx->tl = nullptr;
-  }
-  else if (k == "debug_timeline") {
-    if (value && !ctx->dbg) {
-      ctx->dbg = ctx->dmalloc(1024 * sizeof(long long));
-      CVK_CHECK_CUDA(cudaMemset(ctx->dbg, 0, 1024 * sizeof(long long)));
-    }
-    if (!value) ctx->dbg = nullptr;
   }
   else throw CvkError(CVK_ERR_INVALID, "unknown option: " + k);
   CVK_API_END
@@ -274,7 +259,7 @@ int cvk_op_conv1d(cvk_ctx* ctx, const float* x, const int* lens, int B, int K, c
 
 // out[b, n] = sum_k x[b,k] w[n,k] (+bias) through the LM decode weight-streaming kernel (bf16 mode, rows <= 64)
 int cvk_op_linear_small(cvk_ctx* ctx, const float* x, int rows, int K, const float* w, const float* bias, int N, float* out, int iters,
-                        float* ms_out, long long* timeline_host, void* stream) {
+                        float* ms_out, void* stream) {
   CVK_API_BEGIN
   cudaStream_t st = (cudaStream_t)stream;
   CVK_REQUIRE(x && w && out && rows > 0 && rows <= 64 && ctx->precision == CVK_PREC_BF16, "cvk_op_linear_small: bf16 context, rows <= 64");
@@ -301,7 +286,6 @@ int cvk_op_linear_small(cvk_ctx* ctx, const float* x, int rows, int K, const flo
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   if (ms_out) *ms_out = iters > 0 ? ms / iters : 0.f;
-  if (timeline_host && ctx->dbg) CVK_CHECK_CUDA(cudaMemcpy(timeline_host, ctx->dbg, 1024 * sizeof(long long), cudaMemcpyDeviceToHost));
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   ctx->tiled.erase(W.w16);
   for (size_t i = owned_mark; i < ctx->owned.size(); ++i) cudaFree(ctx->owned[i]);

@@ -223,7 +223,7 @@ void relpos_attention_fwd(cvk_ctx* ctx, cudaStream_t st, const Mat& q, const Mat
     const size_t mark = ctx->arena.off;
     const int C = H * HD;
     Mat qu = arena_mat(ctx, DT_BF16, s.R, C), qv = arena_mat(ctx, DT_BF16, s.R, C);
-    add_pos_bias_kernel<<<148 * 8, 256, 0, st>>>(q.b16(), q.ld, bias_u, bias_v, s.R, C, qu.b16(), qv.b16(), qu.ld);
+    add_pos_bias_kernel<<<132 * 8, 256, 0, st>>>(q.b16(), q.ld, bias_u, bias_v, s.R, C, qu.b16(), qv.b16(), qu.ld);
     ctx->launches++;
     CVK_LAUNCH_CHECK();
     const int ldu = round_up(pos_rows, 64);

@@ -1,29 +1,20 @@
-// bf16 self-attention on tcgen05 tensor cores for the flow estimator (matcha transformer.py:243-316 via diffusers
-// Attention; flow/decoder.py:439-449): head_dim 64, ragged sequences, full or block-causal (chunk) masking.
-//
-// One CTA = 128 queries of one (sequence, head).  S = Q K^T and O += P V are tcgen05.mma with accumulators in TMEM
-// (S: three 64-column half-tile buffers, O: 64 columns); Q/K/V tiles arrive by TMA (SWIZZLE_128B) straight out of the fused QKV activation
-// matrix; V is consumed MN-major so no transpose is ever materialised; the mask is a predicate on (query, key) indices.
-// Softmax is two-pass (pass 1: row maxima from S tiles, pass 2: P = exp2(S - max) and O accumulation) so O is never
-// read-modify-written: exp throughput, not the tensor pipe, bounds this kernel, and the extra Q K^T costs ~1/4 of it.
-// Both passes are software-pipelined through multiple S buffers in TMEM (see the kernel comment).
-// Warps 0-7: softmax (two threads per query row, 32 keys of every 64-key half tile each; TMEM lane == row), warp 8: TMA
-// producer, warp 9: MMA issuer.
-// Two CTAs are co-resident per SM (TMEM 2 x 256 columns, smem 2 x 98 KB): 16 softmax warps per SM hide the TMEM-load and
-// exp latencies (ncu on the first version, which only fitted one CTA per SM: 33 % issue utilisation, long-scoreboard bound).
+// bf16 self-attention on Hopper tensor cores (wgmma) for the flow estimator (matcha transformer.py:243-316 via diffusers
+// Attention; flow/decoder.py:439-449): head_dim 64, ragged sequences, full or block-causal (chunk) masking, and the conformer
+// relative-position attention of the encoder.
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int AT_BQ = 128, AT_BK = 64, AT_HD = 64;    // 128 queries x 64-key half tiles
-constexpr int AT_KVST = 3;                             // K/V stages (one half tile each)
-constexpr int AT_THREADS = 320;   // warps 0-7 softmax (2 threads per query row: key halves), warp 8 TMA, warp 9 MMA
+constexpr int AT_BQ = 128, AT_BK = 64, AT_HD = 64;    // 128 queries x 64-key tiles
+constexpr int AT_KVST = 3;                             // K/V stages (one key tile each)
+constexpr int AT_THREADS = 384;   // warp 0: TMA producer; warpgroups 1-2: 64 queries each (MMA + softmax)
 constexpr uint32_t Q_BYTES = AT_BQ * AT_HD * 2;        // 16 KB
 constexpr uint32_t K_BYTES = AT_BK * AT_HD * 2;        // 8 KB
 constexpr uint32_t V_BYTES = AT_BK * AT_HD * 2;        // 8 KB
-constexpr uint32_t P_BYTES = 2 * AT_BQ * AT_BK * 2;    // 32 KB: two 128x64 SW128 P buffers
 constexpr uint32_t KV_STAGE = K_BYTES + V_BYTES;       // 16 KB
-constexpr uint32_t AT_SMEM = Q_BYTES + AT_KVST * KV_STAGE + P_BYTES + 1024;   // 97 KB: two CTAs per SM
+
+constexpr uint32_t AT_SMEM = Q_BYTES + AT_KVST * KV_STAGE + 1024;   // 65 KB
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -44,7 +35,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       : "=r"(ok)
       : "r"(bar), "r"(parity)
       : "memory");
-  if (ok) return;            // fast path without clock reads: the wait sits on the single MMA-issuing thread's instruction stream
+  if (ok) return;            // fast path without clock reads
   const long long t0 = clock64();
   for (;;) {
     asm volatile(
@@ -65,62 +56,38 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// SWIZZLE_128B operand descriptor; identical fields for a K-major tile (rows of 64 K-elements) and an MN-major tile
-// (rows of 64 MN-elements, 8-row K groups 1024 B apart): start>>4 | LBO 1 | SBO 1024>>4 | version 1 | layout 2
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+
+// One CTA = 128 queries of one (sequence, head), 384 threads: warp 0 of warpgroup 0 is the TMA producer (Q once, then K/V
+// 64-key tiles through a three-stage ring), warpgroups 1 and 2 own 64 queries each.  Per key tile a consumer warpgroup computes
+// S = Q K^T (wgmma, 64 x 64 fp32 in registers), applies mask / bias and an online softmax in registers (the four threads of a
+// quad share a row: row maxima and sums are quad shuffles), rescales its O accumulator and issues O += P V with P taken straight
+// from the S registers (the accumulator layout of S is the register A-operand layout of the P V MMA) and V consumed MN-major
+// from the TMA tile (transposed-B wgmma), so no transpose is ever materialised.
+// BIAS: an additive score term read from global memory, bias(i, j) = ubias[((s0 + i) * H + h) * ldu + ucenter - i + j]: the
+// relative-position term of the conformer attention (transformer/attention.py:249-330), where row t of U = (q + pos_bias_v) p[t]^T
+// has been produced by relpos_u_kernel and the reference's rel_shift (attention.py:225-247) is the index map (i, j) -> center - (i - j).
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h2);
 }
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// issue-only variant: several loads can be in flight before one tmem_wait() (each tcgen05.wait::ld is a full TMEM round trip)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Pipeline (all hand-offs are mbarriers; one elected MMA thread, one TMA thread, 256 softmax threads).  The unit of work is a
-// HALF tile of 64 keys: K/V arrive in three 16 KB stages, S half tiles rotate through three 64-column TMEM buffers ([0,64)
-// [64,128) [192,256); O lives in [128,192)) and P through two 16 KB shared-memory buffers.
-//   pass 1  the MMA thread runs up to three S half tiles ahead of the softmax threads, which only reduce row maxima;
-//   pass 2  the MMA thread issues S(g+1) before it waits for P(g): the tensor pipe computes the next scores while the softmax
-//           threads (two per query row, 32 keys each) turn S(g) into P(g), and P(g+1) is written while P(g) V is being read.
-// 97 KB of shared memory and 256 TMEM columns per CTA: two CTAs (16 softmax warps) per SM.
-__global__ void __launch_bounds__(AT_THREADS, 2)
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk, const __grid_constant__ CUtensorMap tmv,
+template <bool BIAS>
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk, const __grid_constant__ CUtensorMap tmv,
                const int* __restrict__ start, const int* __restrict__ len, int chunk, float scale_log2e, int kv_div,
-               bf16* __restrict__ out, int ldo, const int* __restrict__ kstart, const int* __restrict__ klen, const int* __restrict__ qoff) {
+               bf16* __restrict__ out, int ldo, const int* __restrict__ kstart, const int* __restrict__ klen, const int* __restrict__ qoff,
+               const float* __restrict__ ubias, int ldu, int ucenter) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_q, bar_o, bar_p1done;
+  __shared__ __align__(8) uint64_t bar_q;
   __shared__ __align__(8) uint64_t bar_full[AT_KVST], bar_empty[AT_KVST];   // K/V stages
-  __shared__ __align__(8) uint64_t s1_full[3], s1_free[3];          // pass 1: S half-tile buffers
-  __shared__ __align__(8) uint64_t s_full[3], s_free[3];            // pass 2: S half-tile buffers
-  __shared__ __align__(8) uint64_t p_full[2], p_free[2];            // pass 2: P half-tile buffers
-  __shared__ uint32_t tmem_slot;
-  __shared__ float xch[2][AT_BQ];   // row max / row sum exchange between the two threads of a row
 
   const int b = blockIdx.z, h = blockIdx.y;
   const int L = len[b], s0 = start[b];            // query rows
@@ -129,295 +96,24 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
   if (i0 >= L) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base, sKV = base + Q_BYTES, sP = sKV + AT_KVST * KV_STAGE;
+  const uint32_t sQ = base, sKV = base + Q_BYTES;
   // keys visible to this query tile: all of the sequence, or up to the end of the last query's chunk
-  const int i_last = q0 + min(i0 + AT_BQ, L) - 1;
-  const int kmax = chunk > 0 ? min(Lk, (i_last / chunk + 1) * chunk) : Lk;
-  const int G = (kmax + AT_BK - 1) / AT_BK;      // half tiles per pass
-
-  // instruction descriptors: D=f32, A=B=bf16, M=128;  S: N=64, both K-major;  O: N=64, B (=V) MN-major
-  constexpr uint32_t IDESC_S = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AT_BK >> 3) << 17) | ((uint32_t)(AT_BQ >> 4) << 24);
-  constexpr uint32_t IDESC_O = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((uint32_t)(AT_HD >> 3) << 17) | ((uint32_t)(AT_BQ >> 4) << 24);
-
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bar_q), 1);
-    mbar_init(smem_u32(&bar_o), 1);
-    mbar_init(smem_u32(&bar_p1done), 256);
-    for (int s = 0; s < AT_KVST; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int s = 0; s < 3; ++s) {
-      mbar_init(smem_u32(&s1_full[s]), 1);
-      mbar_init(smem_u32(&s1_free[s]), 256);
-      mbar_init(smem_u32(&s_full[s]), 1);
-      mbar_init(smem_u32(&s_free[s]), 256);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&p_full[s]), 256);
-      mbar_init(smem_u32(&p_free[s]), 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_slot, tO = tmem_slot + 128;
-  // S half-tile buffer g%3 -> first TMEM column
-  auto scol = [](int g) -> uint32_t { const int sb = g % 3; return sb == 0 ? 0u : (sb == 1 ? 64u : 192u); };
-
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_expect_tx(smem_u32(&bar_q), Q_BYTES);
-      tma_load_2d(sQ, &tmq, smem_u32(&bar_q), h * AT_HD, s0 + i0);
-      for (int it = 0; it < 2 * G; ++it) {
-        const int st = it % AT_KVST;
-        const uint32_t round = (uint32_t)(it / AT_KVST);
-        const bool pass2 = it >= G;
-        const int g = pass2 ? it - G : it;
-        mbar_wait(smem_u32(&bar_empty[st]), (round & 1u) ^ 1u);
-        const uint32_t fb = smem_u32(&bar_full[st]);
-        mbar_expect_tx(fb, pass2 ? KV_STAGE : K_BYTES);
-        tma_load_2d(sKV + st * KV_STAGE, &tmk, fb, (h / kv_div) * AT_HD, ks0 + g * AT_BK);
-        if (pass2) tma_load_2d(sKV + st * KV_STAGE + K_BYTES, &tmv, fb, (h / kv_div) * AT_HD, ks0 + g * AT_BK);
-      }
-    }
-  } else if (warp == 9) {
-    if (lane == 0) {
-      mbar_wait(smem_u32(&bar_q), 0);
-      // ---- pass 1: S(g) into buffer g%3; the K stage is released as soon as the MMA has consumed it
-      for (int g = 0; g < G; ++g) {
-        const int st = g % AT_KVST, sb = g % 3;
-        mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((g / AT_KVST) & 1));
-        mbar_wait(smem_u32(&s1_free[sb]), (uint32_t)(((g / 3) & 1) ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sK = sKV + st * KV_STAGE;
-#pragma unroll
-        for (int k = 0; k < AT_HD / 16; ++k) umma(tbase + scol(g), desc_sw128(sQ + k * 32), desc_sw128(sK + k * 32), IDESC_S, k > 0 ? 1u : 0u);
-        umma_commit(smem_u32(&s1_full[sb]));
-        umma_commit(smem_u32(&bar_empty[st]));
-      }
-      // every pass-1 score has been read before pass 2 reuses the columns
-      mbar_wait(smem_u32(&bar_p1done), 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      // ---- pass 2
-      auto issue_s = [&](int g) {
-        const int it = G + g, st = it % AT_KVST;
-        mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((it / AT_KVST) & 1));
-        mbar_wait(smem_u32(&s_free[g % 3]), (uint32_t)(((g / 3) & 1) ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sK = sKV + st * KV_STAGE;
-#pragma unroll
-        for (int k = 0; k < AT_HD / 16; ++k) umma(tbase + scol(g), desc_sw128(sQ + k * 32), desc_sw128(sK + k * 32), IDESC_S, k > 0 ? 1u : 0u);
-        umma_commit(smem_u32(&s_full[g % 3]));
-      };
-      issue_s(0);
-      for (int g = 0; g < G; ++g) {
-        if (g + 1 < G) issue_s(g + 1);
-        const int it = G + g, st = it % AT_KVST, pb = g & 1;
-        mbar_wait(smem_u32(&p_full[pb]), (uint32_t)((g >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sV = sKV + st * KV_STAGE + K_BYTES;
-        const uint32_t pa = sP + pb * 16384;
-#pragma unroll
-        for (int k = 0; k < AT_BK / 16; ++k)      // 64 keys = 4 steps of 16: A = P (K-major, 32 B per step), B = V (MN-major, 2048 B per step)
-          umma(tO, desc_sw128(pa + k * 32), desc_sw128(sV + k * 2048), IDESC_O, (g > 0 || k > 0) ? 1u : 0u);
-        umma_commit(smem_u32(&p_free[pb]));
-        umma_commit(smem_u32(&bar_empty[st]));
-      }
-      umma_commit(smem_u32(&bar_o));
-    }
-  } else {
-    // softmax warps: two threads per query row, keys [0,32) / [32,64) of every half tile
-    const int q4 = warp & 3, half = warp >> 2;
-    const int row = q4 * 32 + lane;
-    const int i = i0 + row;
-    const int klim = i < L ? (chunk > 0 ? min(Lk, ((q0 + i) / chunk + 1) * chunk) : Lk) : 0;
-    const uint32_t trow = ((uint32_t)(q4 * 32) << 16);
-    const int cb2 = half * 32;
-    float m = -INFINITY;
-    for (int g = 0; g < G; ++g) {
-      const int sb = g % 3;
-      mbar_wait(smem_u32(&s1_full[sb]), (uint32_t)((g / 3) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int j0 = g * AT_BK + cb2;
-      const bool full = j0 + 32 <= klim;
-      const uint32_t tS = tbase + scol(g) + trow + (uint32_t)cb2;
-      uint32_t rr[2][16];
-      tmem_ld16_nowait(tS, rr[0]);
-      tmem_ld16_nowait(tS + 16u, rr[1]);
-      tmem_wait();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(&s1_free[sb]));       // the scores are in registers: the buffer may be overwritten
-      if (full) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) m = fmaxf(m, fmaxf(__uint_as_float(rr[0][e]), __uint_as_float(rr[1][e])));
-      } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          if (j0 + e < klim) m = fmaxf(m, __uint_as_float(rr[0][e]));
-          if (j0 + 16 + e < klim) m = fmaxf(m, __uint_as_float(rr[1][e]));
-        }
-      }
-    }
-    mbar_arrive(smem_u32(&bar_p1done));
-    xch[half][row] = m;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    m = fmaxf(xch[0][row], xch[1][row]);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float mneg = (m == -INFINITY) ? 0.f : -m * scale_log2e;
-    float lsum = 0.f;
-    for (int g = 0; g < G; ++g) {
-      const int pb = g & 1;
-      mbar_wait(smem_u32(&s_full[g % 3]), (uint32_t)((g / 3) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int j0 = g * AT_BK + cb2;
-      const bool full = j0 + 32 <= klim;
-      uint32_t rr[2][16];
-      const uint32_t tS = tbase + scol(g) + trow + (uint32_t)cb2;
-      tmem_ld16_nowait(tS, rr[0]);
-      tmem_ld16_nowait(tS + 16u, rr[1]);
-      tmem_wait();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(&s_free[g % 3]));
-      mbar_wait(smem_u32(&p_free[pb]), (uint32_t)(((g >> 1) & 1) ^ 1));    // P(g-2) has been consumed by its MMA
-      const uint32_t prow = sP + (uint32_t)pb * 16384u + (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u;
-#pragma unroll
-      for (int c4 = 0; c4 < 2; ++c4) {
-        const int c = c4 * 16;
-        uint32_t pk[8];
-#pragma unroll
-        for (int e = 0; e < 16; e += 2) {
-          float p0 = fast_ex2(fmaf(__uint_as_float(rr[c4][e]), scale_log2e, mneg));
-          float p1 = fast_ex2(fmaf(__uint_as_float(rr[c4][e + 1]), scale_log2e, mneg));
-          if (!full) {
-            if (j0 + c + e >= klim) p0 = 0.f;
-            if (j0 + c + e + 1 >= klim) p1 = 0.f;
-          }
-          lsum += p0 + p1;
-          __nv_bfloat162 h2 = __floats2bfloat162_rn(p0, p1);
-          pk[e >> 1] = *reinterpret_cast<uint32_t*>(&h2);
-        }
-        // keys cb2+c .. +15 of the half tile -> 16-B chunks ch, ch+1 of the 128-B row, XOR-swizzled by (row & 7)
-        const uint32_t ch = (uint32_t)((cb2 + c) >> 3);
-        const uint32_t a0 = prow + (((ch) ^ (uint32_t)(row & 7)) << 4);
-        const uint32_t a1 = prow + (((ch + 1) ^ (uint32_t)(row & 7)) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a1), "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7]) : "memory");
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy P stores -> visible to the tensor (async) proxy
-      mbar_arrive(smem_u32(&p_full[pb]));
-    }
-    xch[half][row] = lsum;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    lsum = xch[0][row] + xch[1][row];
-    mbar_wait(smem_u32(&bar_o), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const float inv = lsum > 0.f ? 1.f / lsum : 0.f;
-#pragma unroll 1
-    for (int c = half * 32; c < half * 32 + 32; c += 16) {
-      float v[16];
-      tmem_ld16(tO + trow + (uint32_t)c, v);
-      if (i < L) {
-        __align__(16) bf16 t[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) t[e] = __float2bfloat16_rn(v[e] * inv);
-        bf16* op = out + (size_t)(s0 + i) * ldo + h * AT_HD + c;
-        *reinterpret_cast<uint4*>(op) = *reinterpret_cast<uint4*>(t);
-        *reinterpret_cast<uint4*>(op + 8) = *reinterpret_cast<uint4*>(t + 8);
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 9) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(256u) : "memory");
-  }
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-
-// ---- single-pass variant ---------------------------------------------------------------------------------------------------
-// Same tiling, roles and hand-offs as attn_tc_kernel, but every score tile is computed and read ONCE.  The two softmax threads of
-// a query row (keys [0,32) / [32,64) of every half tile) each keep their OWN running maximum, row sum and output accumulator:
-// P V for the first two K16 steps of a half tile accumulates into O_A (TMEM columns [128,192)), for the last two into O_B
-// ([192,256)), so neither thread ever needs the other's maximum inside the loop (they sit in different warps; an exchange per
-// tile would be a 256-thread barrier).  The maximum is lazy: a thread keeps its stale m while the tile maximum exceeds it by at
-// most 8 (P <= 2^8: harmless in fp32 sums and in bf16, which has fp32's exponent range) and otherwise rescales its accumulator
-// row in TMEM (after the previous P V has completed, before releasing this tile's P) - a handful of times per row.  The two
-// partial results are merged flash-decoding style at the end: O = (w_A O_A + w_B O_B) / (w_A l_A + w_B l_B), w = 2^(m - max m).
-// TMEM: S half tiles in two 64-column buffers [0,64) [64,128); 256 columns per CTA, two CTAs per SM as before.
-constexpr float AT_LAZY = 8.f;
-// BIAS: an additive score term read from global memory, bias(i, j) = ubias[((s0 + i) * H + h) * ldu + ucenter - i + j]: the
-// relative-position term of the conformer attention (transformer/attention.py:249-330), where row t of U = (q + pos_bias_v) p[t]^T
-// has been produced by relpos_u_kernel and the reference's rel_shift (attention.py:225-247) is the index map (i, j) -> center - (i - j).
-template <bool BIAS>
-__global__ void __launch_bounds__(AT_THREADS, 2)
-attn_tc1_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk, const __grid_constant__ CUtensorMap tmv,
-                const int* __restrict__ start, const int* __restrict__ len, int chunk, float scale_log2e, int kv_div,
-                bf16* __restrict__ out, int ldo, const int* __restrict__ kstart, const int* __restrict__ klen, const int* __restrict__ qoff,
-                const float* __restrict__ ubias, int ldu, int ucenter) {
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_q, bar_o;
-  __shared__ __align__(8) uint64_t bar_full[AT_KVST], bar_empty[AT_KVST];   // K/V stages
-  __shared__ __align__(8) uint64_t s_full[2], s_free[2];            // S half-tile buffers
-  __shared__ __align__(8) uint64_t p_full[2], p_free[2];            // P half-tile buffers
-  __shared__ uint32_t tmem_slot;
-  __shared__ float xm[2][AT_BQ], xl[2][AT_BQ];   // (max, sum) exchange between the two threads of a row
-
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int L = len[b], s0 = start[b];
-  const int Lk = klen ? klen[b] : L, ks0 = kstart ? kstart[b] : s0, q0 = qoff ? qoff[b] : 0;
-  const int i0 = blockIdx.x * AT_BQ;
-  if (i0 >= L) return;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base, sKV = base + Q_BYTES, sP = sKV + AT_KVST * KV_STAGE;
   const int i_last = q0 + min(i0 + AT_BQ, L) - 1;
   const int kmax = chunk > 0 ? min(Lk, (i_last / chunk + 1) * chunk) : Lk;
   const int G = (kmax + AT_BK - 1) / AT_BK;
 
-  constexpr uint32_t IDESC_S = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AT_BK >> 3) << 17) | ((uint32_t)(AT_BQ >> 4) << 24);
-  constexpr uint32_t IDESC_O = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((uint32_t)(AT_HD >> 3) << 17) | ((uint32_t)(AT_BQ >> 4) << 24);
-
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(&bar_q), 1);
-    mbar_init(smem_u32(&bar_o), 1);
     for (int s = 0; s < AT_KVST; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&s_full[s]), 1);
-      mbar_init(smem_u32(&s_free[s]), 256);
-      mbar_init(smem_u32(&p_full[s]), 256);
-      mbar_init(smem_u32(&p_free[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_slot, tOA = tmem_slot + 128, tOB = tmem_slot + 192;
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       mbar_expect_tx(smem_u32(&bar_q), Q_BYTES);
       tma_load_2d(sQ, &tmq, smem_u32(&bar_q), h * AT_HD, s0 + i0);
       for (int g = 0; g < G; ++g) {
@@ -429,185 +125,114 @@ attn_tc1_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
         tma_load_2d(sKV + st * KV_STAGE + K_BYTES, &tmv, fb, (h / kv_div) * AT_HD, ks0 + g * AT_BK);
       }
     }
-  } else if (warp == 9) {
-    if (lane == 0) {
-      mbar_wait(smem_u32(&bar_q), 0);
-      auto issue_s = [&](int g) {
-        const int st = g % AT_KVST, sb = g & 1;
-        mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((g / AT_KVST) & 1));
-        mbar_wait(smem_u32(&s_free[sb]), (uint32_t)(((g >> 1) & 1) ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sK = sKV + st * KV_STAGE;
-#pragma unroll
-        for (int k = 0; k < AT_HD / 16; ++k) umma(tbase + (uint32_t)sb * 64u, desc_sw128(sQ + k * 32), desc_sw128(sK + k * 32), IDESC_S, k > 0 ? 1u : 0u);
-        umma_commit(smem_u32(&s_full[sb]));
-      };
-      issue_s(0);
-      for (int g = 0; g < G; ++g) {
-        if (g + 1 < G) issue_s(g + 1);
-        const int st = g % AT_KVST, pb = g & 1;
-        mbar_wait(smem_u32(&p_full[pb]), (uint32_t)((g >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sV = sKV + st * KV_STAGE + K_BYTES;
-        const uint32_t pa = sP + pb * 16384;
-#pragma unroll
-        for (int k = 0; k < AT_BK / 16; ++k)      // keys [0,32) -> O_A, keys [32,64) -> O_B
-          umma(k < 2 ? tOA : tOB, desc_sw128(pa + k * 32), desc_sw128(sV + k * 2048), IDESC_O, (g > 0 || (k & 1)) ? 1u : 0u);
-        umma_commit(smem_u32(&p_free[pb]));
-        umma_commit(smem_u32(&bar_empty[st]));
-      }
-      umma_commit(smem_u32(&bar_o));
-    }
-  } else {
-    const int q4 = warp & 3, half = warp >> 2;
-    const int row = q4 * 32 + lane;
-    const int i = i0 + row;
-    const int klim = i < L ? (chunk > 0 ? min(Lk, ((q0 + i) / chunk + 1) * chunk) : Lk) : 0;
-    const uint32_t trow = ((uint32_t)(q4 * 32) << 16);
-    const int cb2 = half * 32;
-    const uint32_t tMine = (half ? tOB : tOA) + trow;
-    float m_run = -INFINITY;       // in log2 units (score * scale * log2 e)
-    float lsum = 0.f;
-    for (int g = 0; g < G; ++g) {
-      const int pb = g & 1;
-      mbar_wait(smem_u32(&s_full[pb]), (uint32_t)((g >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int j0 = g * AT_BK + cb2;
-      const bool full = j0 + 32 <= klim;
-      uint32_t rr[2][16];
-      const uint32_t tS = tbase + (uint32_t)pb * 64u + trow + (uint32_t)cb2;
-      float bia[BIAS ? 32 : 1];
-      if (BIAS) {       // issued before the TMEM load: the two latencies overlap
-        const float* ub = ubias + ((size_t)(s0 + i) * gridDim.y + h) * ldu + (ucenter - (q0 + i) + j0);
-#pragma unroll
-        for (int e = 0; e < 32; ++e) bia[e] = (j0 + e < klim) ? __ldg(ub + e) : 0.f;
-      }
-      tmem_ld16_nowait(tS, rr[0]);
-      tmem_ld16_nowait(tS + 16u, rr[1]);
-      tmem_wait();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(&s_free[pb]));
-      if (BIAS) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          rr[0][e] = __float_as_uint(__uint_as_float(rr[0][e]) + bia[e]);
-          rr[1][e] = __float_as_uint(__uint_as_float(rr[1][e]) + bia[16 + e]);
-        }
-      }
-      float tm = -INFINITY;
-      if (full) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) tm = fmaxf(tm, fmaxf(__uint_as_float(rr[0][e]), __uint_as_float(rr[1][e])));
-      } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          if (j0 + e < klim) tm = fmaxf(tm, __uint_as_float(rr[0][e]));
-          if (j0 + 16 + e < klim) tm = fmaxf(tm, __uint_as_float(rr[1][e]));
-        }
-      }
-      tm *= scale_log2e;             // scale > 0: max commutes with the scaling
-      const bool need = tm > m_run + AT_LAZY;          // also the first tile with a visible key (m_run = -inf)
-      const bool resc = need && m_run != -INFINITY;    // something has been accumulated under the old maximum
-      // tcgen05.ld / .st are warp-collective (.sync.aligned): the whole warp takes the rescale path when any row needs it, rows
-      // that do not scale by 1
-      if (__any_sync(0xffffffffu, resc)) {
-        // every P V issued so far has to be complete before the accumulator rows are rewritten: P V(g-1) is the last one
-        mbar_wait(smem_u32(&p_free[pb ^ 1]), (uint32_t)(((g - 1) >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const float f = resc ? fast_ex2(m_run - tm) : 1.f;
-        lsum *= f;
-#pragma unroll 1
-        for (int c = 0; c < AT_HD; c += 16) {
-          float v[16];
-          tmem_ld16(tMine + (uint32_t)c, v);
-#pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] *= f;
-          tmem_st16(tMine + (uint32_t)c, v);
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      }
-      if (need) m_run = tm;
-      const float mneg = (m_run == -INFINITY) ? 0.f : -m_run;
-      mbar_wait(smem_u32(&p_free[pb]), (uint32_t)(((g >> 1) & 1) ^ 1));    // P(g-2) has been consumed by its MMA
-      const uint32_t prow = sP + (uint32_t)pb * 16384u + (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u;
-#pragma unroll
-      for (int c4 = 0; c4 < 2; ++c4) {
-        const int c = c4 * 16;
-        uint32_t pk[8];
-#pragma unroll
-        for (int e = 0; e < 16; e += 2) {
-          float p0 = fast_ex2(fmaf(__uint_as_float(rr[c4][e]), scale_log2e, mneg));
-          float p1 = fast_ex2(fmaf(__uint_as_float(rr[c4][e + 1]), scale_log2e, mneg));
-          if (!full) {
-            if (j0 + c + e >= klim) p0 = 0.f;
-            if (j0 + c + e + 1 >= klim) p1 = 0.f;
-          }
-          lsum += p0 + p1;
-          __nv_bfloat162 h2 = __floats2bfloat162_rn(p0, p1);
-          pk[e >> 1] = *reinterpret_cast<uint32_t*>(&h2);
-        }
-        const uint32_t ch = (uint32_t)((cb2 + c) >> 3);
-        const uint32_t a0 = prow + (((ch) ^ (uint32_t)(row & 7)) << 4);
-        const uint32_t a1 = prow + (((ch + 1) ^ (uint32_t)(row & 7)) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a1), "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7]) : "memory");
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(smem_u32(&p_full[pb]));
-    }
-    xm[half][row] = m_run;
-    xl[half][row] = lsum;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float mA = xm[0][row], mB = xm[1][row];
-    const float mm = fmaxf(mA, mB);
-    const float wA = (mA == -INFINITY) ? 0.f : fast_ex2(mA - mm), wB = (mB == -INFINITY) ? 0.f : fast_ex2(mB - mm);
-    const float den = wA * xl[0][row] + wB * xl[1][row];
-    mbar_wait(smem_u32(&bar_o), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const float inv = den > 0.f ? 1.f / den : 0.f;
-    const float fA = wA * inv, fB = wB * inv;
-#pragma unroll 1
-    for (int c = half * 32; c < half * 32 + 32; c += 16) {
-      uint32_t ra[16], rb[16];
-      tmem_ld16_nowait(tOA + trow + (uint32_t)c, ra);
-      tmem_ld16_nowait(tOB + trow + (uint32_t)c, rb);
-      tmem_wait();
-      if (i < L) {
-        __align__(16) bf16 t[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          // an accumulator that never saw a visible key holds P = 0 products only, but guard against 0 * garbage all the same
-          const float a = wA > 0.f ? __uint_as_float(ra[e]) * fA : 0.f;
-          const float bb = wB > 0.f ? __uint_as_float(rb[e]) * fB : 0.f;
-          t[e] = __float2bfloat16_rn(a + bb);
-        }
-        bf16* op = out + (size_t)(s0 + i) * ldo + h * AT_HD + c;
-        *reinterpret_cast<uint4*>(op) = *reinterpret_cast<uint4*>(t);
-        *reinterpret_cast<uint4*>(op + 8) = *reinterpret_cast<uint4*>(t + 8);
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 9) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(256u) : "memory");
+  const int wg = (threadIdx.x - 128) >> 7;
+  const int q = lane & 3;
+  const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // tile rows rbase (h = 0) and rbase + 8 (h = 1)
+  int ii[2], klim[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    ii[hh] = i0 + rbase + 8 * hh;
+    klim[hh] = ii[hh] < L ? (chunk > 0 ? min(Lk, ((q0 + ii[hh]) / chunk + 1) * chunk) : Lk) : 0;
+  }
+  const uint64_t dq = wg_desc_sw128(sQ + (uint32_t)wg * (Q_BYTES / 2));
+  float o[32], m_run[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
+#pragma unroll
+  for (int e = 0; e < 32; ++e) o[e] = 0.f;
+  mbar_wait(smem_u32(&bar_q), 0);
+  for (int g = 0; g < G; ++g) {
+    const int st = g % AT_KVST;
+    const int j0 = g * AT_BK;
+    float bia[BIAS ? 32 : 1];
+    if (BIAS) {       // issued before the score MMA: the two latencies overlap
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        const int hh = (e >> 1) & 1, j = j0 + 8 * (e >> 2) + 2 * q + (e & 1);
+        bia[e] = (ii[hh] < L && j < klim[hh])
+                     ? __ldg(ubias + ((size_t)(s0 + ii[hh]) * gridDim.y + h) * ldu + (ucenter - (q0 + ii[hh]) + j)) : 0.f;
+      }
+    }
+    mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((g / AT_KVST) & 1));
+    const uint32_t sK = sKV + st * KV_STAGE, sV = sK + K_BYTES;
+    float s[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) s[e] = 0.f;
+    wg_fence();
+    const uint64_t dk = wg_desc_sw128(sK);
+#pragma unroll
+    for (int k = 0; k < AT_HD / 16; ++k) wgmma_ss<64, 0>(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), 1);
+    wg_commit();
+    wg_wait<0>();
+    wg_touch<32>(s);
+    // s[e]: row rbase + 8 ((e >> 1) & 1), key j0 + 8 (e >> 2) + 2 q + (e & 1)
+    float tm[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int e = 0; e < 32; ++e) {
+      const int hh = (e >> 1) & 1, j = j0 + 8 * (e >> 2) + 2 * q + (e & 1);
+      if (BIAS) s[e] += bia[e];
+      if (j >= klim[hh]) s[e] = -INFINITY;
+      tm[hh] = fmaxf(tm[hh], s[e]);
+    }
+    float f[2], mneg[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float mt = quad_max(tm[hh]) * scale_log2e;     // scale > 0: max commutes with the scaling
+      const float mn = fmaxf(m_run[hh], mt);
+      f[hh] = m_run[hh] == -INFINITY ? 1.f : fast_ex2(m_run[hh] - mn);   // nothing accumulated yet: o and lsum are 0
+      m_run[hh] = mn;
+      mneg[hh] = mn == -INFINITY ? 0.f : -mn;
+      lsum[hh] *= f[hh];
+    }
+#pragma unroll
+    for (int e = 0; e < 32; ++e) {
+      const int hh = (e >> 1) & 1;
+      const float p = s[e] == -INFINITY ? 0.f : fast_ex2(fmaf(s[e], scale_log2e, mneg[hh]));
+      s[e] = p;
+      lsum[hh] += p;
+      o[e] *= f[hh];
+    }
+    uint32_t pa[4][4];      // P as the A operand of 4 K16 steps: rows rbase / rbase + 8, keys 16 kk + 2 q (+8)
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      pa[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+    wg_fence();
+    const uint64_t dv = wg_desc_sw128(sV);
+#pragma unroll
+    for (int kk = 0; kk < AT_BK / 16; ++kk) wgmma_rs_tb_m64n64(o, pa[kk], dv + (uint64_t)(128 * kk), 1);   // +2048 B per 16 keys
+    wg_commit();
+    wg_wait<0>();
+    wg_touch<32>(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[st]));
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const float den = quad_sum(lsum[hh]);
+    const float inv = den > 0.f ? 1.f / den : 0.f;
+    if (ii[hh] < L) {
+      bf16* op = out + (size_t)(s0 + ii[hh]) * ldo + h * AT_HD + 2 * q;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(op + 8 * jj) = pack_bf16(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+    }
   }
 }
 
-
 // ---- relative-position scores of the conformer attention ---------------------------------------------------------------------
 // U[(s0 + i) * H + h][t] = (q_i + pos_bias_v)_h . p[t]_h for the table rows t that query tile i0 can address (t = center - (i - j),
-// j < L): one CTA per (query tile, head, sequence), 64-row tiles of the position table through the same TMA / tcgen05 pipeline as
-// the score pass of the attention kernel; the eight epilogue warps write fp32 rows (two threads per query row, 32 columns each).
-__global__ void __launch_bounds__(AT_THREADS, 2)
+// j < L): one CTA per (query tile, head, sequence), 64-row tiles of the position table through the same TMA / wgmma pipeline as
+// the score MMA of the attention kernel; each consumer warpgroup writes the fp32 rows of its 64 queries.
+__global__ void __launch_bounds__(AT_THREADS, 1)
 relpos_u_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmp, const int* __restrict__ start,
                 const int* __restrict__ len, int center, int pos_rows, float* __restrict__ U, int ldu) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_q;
   __shared__ __align__(8) uint64_t bar_full[AT_KVST], bar_empty[AT_KVST];
-  __shared__ __align__(8) uint64_t s_full[3], s_free[3];
-  __shared__ uint32_t tmem_slot;
   const int b = blockIdx.z, h = blockIdx.y;
   const int L = len[b], s0 = start[b];
   const int i0 = blockIdx.x * AT_BQ;
@@ -619,29 +244,17 @@ relpos_u_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
   const int t_lo = max(center - i_hi, 0), t_hi = min(center - i0 + L - 1, pos_rows - 1);
   const int t0 = (t_lo / AT_BK) * AT_BK;
   const int G = (t_hi - t0) / AT_BK + 1;
-  constexpr uint32_t IDESC_S = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AT_BK >> 3) << 17) | ((uint32_t)(AT_BQ >> 4) << 24);
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(&bar_q), 1);
     for (int s = 0; s < AT_KVST; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int s = 0; s < 3; ++s) {
-      mbar_init(smem_u32(&s_full[s]), 1);
-      mbar_init(smem_u32(&s_free[s]), 256);
+      mbar_init(smem_u32(&bar_empty[s]), 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = tmem_slot;
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       mbar_expect_tx(smem_u32(&bar_q), Q_BYTES);
       tma_load_2d(sQ, &tmq, smem_u32(&bar_q), h * AT_HD, s0 + i0);
       for (int g = 0; g < G; ++g) {
@@ -652,56 +265,40 @@ relpos_u_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
         tma_load_2d(sP + st * K_BYTES, &tmp, fb, h * AT_HD, t0 + g * AT_BK);
       }
     }
-  } else if (warp == 9) {
-    if (lane == 0) {
-      mbar_wait(smem_u32(&bar_q), 0);
-      for (int g = 0; g < G; ++g) {
-        const int st = g % AT_KVST, sb = g % 3;
-        mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((g / AT_KVST) & 1));
-        mbar_wait(smem_u32(&s_free[sb]), (uint32_t)(((g / 3) & 1) ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sK = sP + st * K_BYTES;
-#pragma unroll
-        for (int k = 0; k < AT_HD / 16; ++k) umma(tbase + (uint32_t)sb * 64u, desc_sw128(sQ + k * 32), desc_sw128(sK + k * 32), IDESC_S, k > 0 ? 1u : 0u);
-        umma_commit(smem_u32(&s_full[sb]));
-        umma_commit(smem_u32(&bar_empty[st]));
-      }
-    }
-  } else {
-    const int q4 = warp & 3, half = warp >> 2;
-    const int row = q4 * 32 + lane;
-    const int i = i0 + row;
-    const uint32_t trow = ((uint32_t)(q4 * 32) << 16);
-    const int cb2 = half * 32;
-    float* urow = U + ((size_t)(s0 + i) * gridDim.y + h) * ldu;
-    for (int g = 0; g < G; ++g) {
-      const int sb = g % 3;
-      mbar_wait(smem_u32(&s_full[sb]), (uint32_t)((g / 3) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t rr[2][16];
-      const uint32_t tS = tbase + (uint32_t)sb * 64u + trow + (uint32_t)cb2;
-      tmem_ld16_nowait(tS, rr[0]);
-      tmem_ld16_nowait(tS + 16u, rr[1]);
-      tmem_wait();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(&s_free[sb]));
-      if (i < L) {
-        float4* dst = reinterpret_cast<float4*>(urow + t0 + g * AT_BK + cb2);      // ldu and t0 are multiples of 4
-#pragma unroll
-        for (int c4 = 0; c4 < 2; ++c4)
-#pragma unroll
-          for (int e = 0; e < 16; e += 4)
-            dst[c4 * 4 + (e >> 2)] = make_float4(__uint_as_float(rr[c4][e]), __uint_as_float(rr[c4][e + 1]), __uint_as_float(rr[c4][e + 2]),
-                                                 __uint_as_float(rr[c4][e + 3]));
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 9) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(256u) : "memory");
+  const int wg = (threadIdx.x - 128) >> 7;
+  const int q = lane & 3;
+  const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint64_t dq = wg_desc_sw128(sQ + (uint32_t)wg * (Q_BYTES / 2));
+  mbar_wait(smem_u32(&bar_q), 0);
+  for (int g = 0; g < G; ++g) {
+    const int st = g % AT_KVST;
+    mbar_wait(smem_u32(&bar_full[st]), (uint32_t)((g / AT_KVST) & 1));
+    float s[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) s[e] = 0.f;
+    wg_fence();
+    const uint64_t dp = wg_desc_sw128(sP + st * K_BYTES);
+#pragma unroll
+    for (int k = 0; k < AT_HD / 16; ++k) wgmma_ss<64, 0>(s, dq + (uint64_t)(2 * k), dp + (uint64_t)(2 * k), 1);
+    wg_commit();
+    wg_wait<0>();
+    wg_touch<32>(s);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[st]));
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int i = i0 + rbase + 8 * hh;
+      if (i < L) {
+        float* urow = U + ((size_t)(s0 + i) * gridDim.y + h) * ldu + t0 + g * AT_BK + 2 * q;     // ldu and t0 are even
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) *reinterpret_cast<float2*>(urow + 8 * jj) = make_float2(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]);
+      }
+    }
   }
 }
+
 
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -738,20 +335,13 @@ void attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& q, const Mat& k,
   make_map(ctx, &tv, v, AT_BK);
   static bool attr = false;
   if (!attr) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_tc1_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_tc1_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(relpos_u_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
     attr = true;
   }
   dim3 grid(ceil_div(s.max_len, AT_BQ), H, s.B);
-  if (ctx->attn_single_pass)
-    attn_tc1_kernel<false><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, kv_div, out.b16(), out.ld,
-                                                              kg ? kg->d_kstart : nullptr, kg ? kg->d_klen : nullptr, kg ? kg->d_qoff : nullptr,
-                                                              nullptr, 0, 0);
-  else
-  attn_tc_kernel<<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, kv_div, out.b16(), out.ld,
-                                                    kg ? kg->d_kstart : nullptr, kg ? kg->d_klen : nullptr, kg ? kg->d_qoff : nullptr);
+  attn_wg_kernel<false><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, kv_div, out.b16(), out.ld,
+                                                           kg ? kg->d_kstart : nullptr, kg ? kg->d_klen : nullptr, kg ? kg->d_qoff : nullptr,
+                                                           nullptr, 0, 0);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }
@@ -773,7 +363,7 @@ void relpos_attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& qu, const
   make_map(ctx, &tp, pos, AT_BK);
   static bool attr = false;
   if (!attr) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_tc1_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
     CVK_CHECK_CUDA(cudaFuncSetAttribute(relpos_u_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
     attr = true;
   }
@@ -781,7 +371,7 @@ void relpos_attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& qu, const
   relpos_u_kernel<<<grid, AT_THREADS, AT_SMEM, st>>>(tqv, tp, s.d_start, s.d_len, pos_center, pos_rows, U.f32(), U.ld);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
-  attn_tc1_kernel<true><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, 1, out.b16(), out.ld,
+  attn_wg_kernel<true><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, 1, out.b16(), out.ld,
                                                           nullptr, nullptr, nullptr, U.f32(), U.ld, pos_center);
   ctx->launches++;
   CVK_LAUNCH_CHECK();

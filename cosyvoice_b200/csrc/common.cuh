@@ -23,7 +23,7 @@ struct EpiDev {
   void* out2;
   int out2_dtype;
   int out2_ld;
-  int ab_f16;        // tcgen05 GEMM: operands are IEEE half (instruction-descriptor formats 0) instead of bf16
+  int ab_f16;        // wgmma GEMM: operands are IEEE half (the .f16 instruction variant) instead of bf16
 };
 
 inline EpiDev to_dev(const Epilogue& e) {
@@ -145,10 +145,9 @@ __device__ __forceinline__ float apply_act_fast(int act, float x, float param, f
   }
 }
 // 16 values at once: the dispatch on the (run-time) activation kind happens ONCE, outside the element loop.  With the switch
-// inside an unrolled loop every element paid the whole dispatch (~60 issue slots per element, measured: any activation made the
-// tcgen05 GEMM epilogue 2.4x slower than none).
+// inside an unrolled loop every element would pay the whole dispatch.
 // tanh-form GELU of 16 values with the tanh of TWO arguments per MUFU instruction (tanh.approx.f16x2): the GELU epilogue of
-// ff.net.0 is MUFU-bound (32 768 tanh per 128 x 256 tile at 16 per clock per SM; +11 us per launch against no activation).  The
+// ff.net.0 is MUFU-bound (one tanh per output element, 16 per clock per SM).  The
 // half-precision tanh is off by <= 5e-4 absolute, i.e. <= 2.5e-4 |x| in the GELU - below the bf16 rounding of the stored result
 // (3.9e-3 |x|); only the bf16-mode epilogues come here.
 __device__ __forceinline__ void gelu16_packed(float* v) {

@@ -159,7 +159,7 @@ struct cvk_ctx {
   int device = 0;
   int precision = CVK_PREC_FP32;
   int act_dtype = DT_F32;
-  int num_sms = 148;
+  int num_sms = 132;
   std::string last_error;
   std::map<std::string, RawTensor> raw;     // tensors handed over by cvk_set_tensor, consumed by cvk_finalize
   std::vector<void*> owned;                 // device allocations owned by the context
@@ -177,11 +177,8 @@ struct cvk_ctx {
   int op_out_bf16 = 0;                      // cvk_op_conv1d: bf16 output matrix (the estimator's usual epilogue) instead of fp32
   int op_iters = 0;                         // cvk_op_conv1d: repeat the GEMM launch this many times and time it
   double op_ms = 0.0;
-  int tc_epi = 2;                           // tcgen05 GEMM epilogue: 2 = smem-staged TMA stores, 0 = direct stores, 1 = direct + prefetch
-  int tc_persist = 2;                       // tcgen05 GEMM, tiles > SMs: persistent CTAs + double-buffered TMEM accumulators (2 = 16 epilogue warps, 1 = 8, 0 = off)
-  int tc_pbn256 = 1;                        // persistent tcgen05 GEMM: 128x256 tiles for 16-bit outputs with N % 256 == 0 (halves the A re-reads out of L2)
-  int tc_bn256 = 0;                         // experiment: 128x256 tiles (1 CTA/SM) instead of 128x128 (2 CTAs/SM)
-  void* dbg = nullptr;                      // device int64[1024] timeline buffer (debug option)
+  int tc_epi = 2;                           // wgmma GEMM epilogue: 2 = smem-staged TMA stores, otherwise direct stores
+  int tc_persist = 2;                       // wgmma GEMM, tiles > SMs: persistent CTAs, one per SM (0 = one CTA per tile)
   void* tl = nullptr;                       // device int64[4096] LM-chain timeline (debug option chain_timeline): 4 slots per launch
   int tl_seq = 0;
   long long* tl_next() {                    // slot block of the next launch of the decode chain (null when the option is off)
@@ -198,15 +195,14 @@ struct cvk_ctx {
   int lm_fused = 1;                         // LM decode: fused finish+rmsnorm / rope+attention / SwiGLU-epilogue kernels
   int hift_f16 = 1;                         // tensor-core mode: vocoder operands in IEEE half (TF32-class mantissa) instead of bf16
   int build_f16 = 0;                        // set while a stage whose weights need the half copy is being finalised
-  int enc_tc_attn = 1;                      // conformer relative-position attention on the tcgen05 kernels (attention_tc.cu) instead of CUDA cores
-  int attn_single_pass = 1;                 // flow attention: one-pass kernel with per-thread lazy maxima (attention_tc.cu)
-  int lm_mega = 0;                          // LM decode: all layers of a step in one persistent cooperative kernel (llm_mega.cu); measured
-                                            // 973 us / step against 886 us for the PDL-chained per-op path at batch 32 (profiles/r02_lm_decode.md): off by default
+  int enc_tc_attn = 1;                      // conformer relative-position attention on the wgmma kernels (attention_tc.cu) instead of CUDA cores
+  int lm_mega = 0;                          // LM decode: all layers of a step in one persistent cooperative kernel (llm_mega.cu); off by
+                                            // default: not faster than the PDL-chained per-op path in earlier measurements
   int mega_coop = 1;                        // ... launched with the cooperative attribute (co-residency guaranteed by the driver)
   int use_skinny = 1;                       // LM decode GEMMs on the weight-streaming split-K kernel
-  int use_tc_attn = 1;                      // bf16 mode: tcgen05 attention kernel (0 = CUDA-core flash kernel)
+  int use_tc_attn = 1;                      // bf16 mode: wgmma attention kernel (0 = CUDA-core flash kernel)
   int use_graph = 1;                        // LM decode step replayed as a CUDA graph
-  int use_tc = 1;                           // bf16 mode: route GEMMs to the tcgen05 kernel (0 = debug: SIMT on converted operands)
+  int use_tc = 1;                           // bf16 mode: route GEMMs to the wgmma kernel (0 = debug: SIMT on converted operands)
 
   void* dmalloc(size_t bytes) {
     void* p = nullptr;
@@ -254,7 +250,7 @@ float* fold_weight_norm(cvk_ctx* ctx, const std::string& prefix, int64_t* numel_
 void finish_convw(cvk_ctx* ctx, ConvW& w);   // create bf16 copy if needed
 float* dev_copy_f32(cvk_ctx* ctx, const float* src_dev, size_t n);
 
-// conv-GEMM (dispatches SIMT fp32 / tcgen05 bf16 on A.dtype)
+// conv-GEMM (dispatches SIMT fp32 / wgmma bf16 on A.dtype)
 void conv_gemm(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_simt(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);

@@ -389,7 +389,7 @@ __global__ void bcast_rows_kernel(const float* __restrict__ vec, int C, int vec_
 
 inline int grid_for(size_t total, int threads = 256) {
   size_t g = (total + threads - 1) / threads;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (g < 1) g = 1;
   return (int)g;
 }

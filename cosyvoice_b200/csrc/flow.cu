@@ -1019,7 +1019,7 @@ void ln_mod(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Seqs& s, const fl
 }
 
 void gate_add(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat& o, const Seqs& s, const float* gate, int gate_ld) {
-  dit_gate_add_kernel<<<148 * 8, 256, 0, st>>>(x.f32(), x.ld, o.f32(), o.ld, x.rows, s.d_row2seq, gate, gate_ld);
+  dit_gate_add_kernel<<<132 * 8, 256, 0, st>>>(x.f32(), x.ld, o.f32(), o.ld, x.rows, s.d_row2seq, gate, gate_ld);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }

@@ -1,26 +1,22 @@
 // Weight-streaming GEMM for the LM decode step (at most 64 activation rows): out[b, n] = sum_k x[b, k] * W[n, k].
 //
 // The step is HBM-bound on the weights (SURVEY.md §8d: 727.6 MB of bf16 weights per step shared by all rows), so the
-// kernel is organised around memory-level parallelism, not MMA rate: operands are swapped (the 128-row UMMA M dimension
-// holds 128 output features of W, the UMMA N dimension holds the <= 64 batch rows), K is split across CTAs so that
-// ~all 148 SMs stream disjoint weight slabs, and each CTA keeps 8 TMA stages (160 KB) in flight.  fp32 accumulation in
-// TMEM; split-K partial sums go to a [splits][rows][N] scratch and are reduced in fixed order by a finishing kernel that
+// kernel is organised around memory-level parallelism, not MMA rate: operands are swapped (the wgmma M side holds 128 output
+// features of W, 64 per warpgroup, the wgmma N dimension holds the <= 64 batch rows), K is split across CTAs so that ~all SMs
+// stream disjoint weight slabs, and each CTA keeps 8 TMA stages (160 / 192 KB) in flight.  fp32 accumulation in registers;
+// split-K partial sums go to a [splits][rows][N] scratch and are reduced in fixed order by a finishing kernel that
 // applies the same fused epilogue as the big GEMM (deterministic - no atomics).
 // Serves transformers' Qwen2 q/k/v/o/gate/up/down projections and the llm_decoder head at decode time
 // (cosyvoice/llm/llm.py:244-251, 542).
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int SK_BM = 128;      // output features per CTA (UMMA M)
+constexpr int SK_BM = 128;      // output features per CTA (wgmma M of two warpgroups)
 constexpr int SK_BK = 64;
 constexpr int SK_STAGES = 8;
-constexpr int SK_THREADS = 288;   // warp 0: TMA producer; warps 1, 6, 7, 8: MMA issuers; warps 2..5: epilogue
-// With N <= 64 an MMA is 16-32 cycles of tensor-core work, but ONE issuing thread spends ~0.35 us per 64-K chunk on the
-// instruction stream itself (mbarrier wait ~0.16 us + 4 MMAs and a commit ~0.19 us; in-kernel stamps, profiles/r02_lm_mega.md)
-// - 4.9 us of the 8.8 us gate|up GEMM of a decode step.  The chunks are therefore dealt round-robin to SK_NACC issuer warps,
-// each accumulating into its own TMEM tile; the epilogue adds the tiles.
-constexpr int SK_NACC = 4;
+constexpr int SK_THREADS = 384;   // warp 0: TMA producer; warpgroups 1-2: wgmma + epilogue, 64 features each
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -59,37 +55,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 // plain (non-tensor) bulk copy global -> shared, completion counted on an mbarrier
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 // W [N][K] bf16 row-major -> streaming layout: [N/128 tiles][K/64 chunks] blocks of 16 KB, each block being the exact
 // shared-memory image of a K-major SWIZZLE_128B operand tile (row r, 16-byte chunk c stored at r*128 + ((c ^ (r & 7)) << 4)),
 // so that one stage is ONE contiguous 16 KB bulk copy: DRAM sees perfectly sequential reads instead of 128 strided rows.
@@ -112,25 +85,21 @@ __global__ void tile_weights_kernel(const bf16* __restrict__ w, bf16* __restrict
   }
 }
 
-// grid: (N tiles, splits).  BPAD = padded batch (UMMA N): 32 or 64.
+// grid: (N tiles, splits).  BPAD = padded batch (wgmma N): 32 or 64.  Warp 0 streams the stages; warpgroups 1 and 2 each
+// accumulate 64 of the tile's 128 output features over the CTA's K chunks (fp32 in registers) and run the epilogue on them.
 template <int BPAD>
 __global__ void __launch_bounds__(SK_THREADS, 1)
 skinny_gemm_kernel(const bf16* __restrict__ w_tiled, const __grid_constant__ CUtensorMap tmap_x, int N, int K, int rows,
                    int chunks_per_split, float* __restrict__ partial /*[splits][rows][N] or null*/, EpiDev ep, int swiglu,
-                   long long* __restrict__ dbg, long long* __restrict__ tl) {
+                   long long* __restrict__ tl) {
   extern __shared__ uint8_t smem_raw[];
   pdl_trigger();
   tl_stamp(tl, 0);
-  long long t_entry = 0;
-  if (dbg) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_entry));
   __shared__ __align__(8) uint64_t bar_full[SK_STAGES];
   __shared__ __align__(8) uint64_t bar_empty[SK_STAGES];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_slot;
   constexpr uint32_t A_BYTES = SK_BM * SK_BK * 2;    // 16 KB of weights
   constexpr uint32_t B_BYTES = BPAD * SK_BK * 2;     // activations
   constexpr uint32_t STAGE = A_BYTES + B_BYTES;
-  constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BPAD >> 3) << 17) | ((uint32_t)(SK_BM >> 4) << 24);
 
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -143,32 +112,14 @@ skinny_gemm_kernel(const bf16* __restrict__ w_tiled, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     for (int s = 0; s < SK_STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
     }
-    mbar_init(smem_u32(&bar_acc), SK_NACC);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"((uint32_t)(SK_NACC * BPAD))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_slot;
-  const bool trace = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
-  if (trace && threadIdx.x == 0) dbg[0] = clock64();
-  const int cta_lin = blockIdx.y * gridDim.x + blockIdx.x;
-  if (dbg && threadIdx.x == 0 && cta_lin < 200) {
-    long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    dbg[128 + cta_lin * 4 + 0] = t_entry;
-    dbg[128 + cta_lin * 4 + 1] = t;
-  }
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       // The weights are written by no kernel of the chain: the first ring of weight slabs is requested BEFORE waiting for the
       // producer of the activations, so the HBM stream of this kernel overlaps the tail of the previous one.
       const int pre = min(iters, SK_STAGES);
@@ -179,10 +130,7 @@ skinny_gemm_kernel(const bf16* __restrict__ w_tiled, const __grid_constant__ CUt
       }
       pdl_wait();
       tl_stamp(tl, 1);
-      for (int it = 0; it < pre; ++it) {
-        tma_load_2d(base + it * STAGE + A_BYTES, &tmap_x, smem_u32(&bar_full[it]), (kc0 + it) * SK_BK, 0);
-        if (trace && it < 32) dbg[8 + it] = clock64();
-      }
+      for (int it = 0; it < pre; ++it) tma_load_2d(base + it * STAGE + A_BYTES, &tmap_x, smem_u32(&bar_full[it]), (kc0 + it) * SK_BK, 0);
       for (int it = pre; it < iters; ++it) {
         const int s = it % SK_STAGES;
         const uint32_t round = (uint32_t)(it / SK_STAGES);
@@ -192,101 +140,57 @@ skinny_gemm_kernel(const bf16* __restrict__ w_tiled, const __grid_constant__ CUt
         mbar_expect_tx(fb, STAGE);
         bulk_load(sa, w_tiled + ((size_t)blockIdx.x * kchunks + (kc0 + it)) * (SK_BM * SK_BK), A_BYTES, fb);
         tma_load_2d(sb, &tmap_x, fb, (kc0 + it) * SK_BK, 0);
-        if (trace && it < 32) dbg[8 + it] = clock64();
       }
     } else {
       pdl_wait();
     }
-  } else if (warp == 1 || warp >= 6) {
-    // MMA issuers: issuer ii takes chunks ii, ii + SK_NACC, ... into accumulator tile ii
-    const int ii = warp == 1 ? 0 : warp - 5;
+  } else {
+    const int wg = (threadIdx.x - 128) >> 7;
+    const int q = lane & 3;
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile features fr (acc[4 j + 0/1]) and fr + 8 (acc[4 j + 2/3])
+    float bias_n[2];                                           // fetched while the weights stream
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) bias_n[hh] = (!partial && !swiglu && ep.bias && n0 + fr + 8 * hh < N) ? ep.bias[n0 + fr + 8 * hh] : 0.f;
     pdl_wait();
-    if (lane == 0) {
-      const uint32_t tacc = tmem + (uint32_t)ii * BPAD;
-      for (int it = ii; it < iters; it += SK_NACC) {
-        const int s = it % SK_STAGES;
-        const uint32_t round = (uint32_t)(it / SK_STAGES);
-        mbar_wait(smem_u32(&bar_full[s]), round & 1u);
-        if (trace && it < 32) dbg[40 + it] = clock64();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = base + s * STAGE, sb = sa + A_BYTES;
-        const uint64_t da = desc_sw128(sa), db = desc_sw128(sb);
+    float acc[BPAD / 2];
 #pragma unroll
-        for (int k = 0; k < SK_BK / 16; ++k) umma(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, (it >= SK_NACC || k > 0) ? 1u : 0u);
-        umma_commit(smem_u32(&bar_empty[s]));
-      }
-      if (ii < iters) umma_commit(smem_u32(&bar_acc));
-      else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&bar_acc)) : "memory");    // no chunk for this issuer
+    for (int e = 0; e < BPAD / 2; ++e) acc[e] = 0.f;
+    for (int it = 0; it < iters; ++it) {
+      const int s = it % SK_STAGES;
+      mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(it / SK_STAGES) & 1u);
+      const uint32_t sa = base + s * STAGE + (uint32_t)wg * (A_BYTES / 2), sb = base + s * STAGE + A_BYTES;
+      const uint64_t da = wg_desc_sw128(sa), db = wg_desc_sw128(sb);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < SK_BK / 16; ++k) wgmma_ss<BPAD, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      wg_commit();
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bar_empty[s]));
     }
-  } else {      // warps 2..5: epilogue (TMEM lane quarter = warp & 3)
-    const int q = warp & 3;
-    const int n_pre = n0 + q * 32 + lane;
-    const float bias_n = (!partial && !swiglu && ep.bias && n_pre < N) ? ep.bias[n_pre] : 0.f;   // fetched while the weights stream
-    pdl_wait();
-    mbar_wait(smem_u32(&bar_acc), 0);
-    if (trace && threadIdx.x == 64) dbg[1] = clock64();
-    if (dbg && threadIdx.x == 64 && cta_lin < 200) {
-      long long t;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-      dbg[128 + cta_lin * 4 + 2] = t;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int n = n0 + q * 32 + lane;          // this thread's output feature
-    const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < BPAD; c += 16) {
-      float acc[16];
-      tmem_ld16(trow + (uint32_t)c, acc);
+    wg_touch<BPAD / 2>(acc);
+    const bool plain = ep.act1 == ACT_NONE && !ep.resid && !ep.rowvec && !ep.row2seq && !ep.accumulate && !ep.out2 && ep.scale == 1.f;
+    // acc[e]: feature n0 + fr + 8 ((e >> 1) & 1), batch row 8 (e >> 2) + 2 q + (e & 1)
 #pragma unroll
-      for (int a = 1; a < SK_NACC; ++a) {
-        if (a < iters) {                    // tiles of issuers without a chunk were never written
-          float t2[16];
-          tmem_ld16(trow + (uint32_t)(a * BPAD + c), t2);
-#pragma unroll
-          for (int e = 0; e < 16; ++e) acc[e] += t2[e];
-        }
-      }
-      if (trace && threadIdx.x == 64) dbg[3 + (c >> 4)] = clock64();
+    for (int e = 0; e < BPAD / 2; ++e) {
+      const int hh = (e >> 1) & 1;
+      const int n = n0 + fr + 8 * hh, b = 8 * (e >> 2) + 2 * q + (e & 1);
       if (swiglu) {
-        // rows of W are interleaved (2i = gate_i, 2i+1 = up_i): lanes pair up, the even lane emits silu(g) * u
-        // (Qwen2 MLP act_fn(gate_proj(x)) * up_proj(x), modeling_qwen2.py:46-48) into column n/2
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const float other = __shfl_xor_sync(0xffffffffu, acc[e], 1);
-          const int b = c + e;
-          if (!(lane & 1) && n + 1 < N && b < rows) {
-            const float g = acc[e];
-            st_any(ep.out, ep.out_dtype, (size_t)b * ep.out_ld + (n >> 1), __fdividef(g, 1.f + fast_exp(-g)) * other);
-          }
+        // rows of W are interleaved (2i = gate_i, 2i+1 = up_i): features n and n + 1 sit in lanes l and l + 4, the even one emits
+        // silu(g) * u (Qwen2 MLP act_fn(gate_proj(x)) * up_proj(x), modeling_qwen2.py:46-48) into column n/2
+        const float other = __shfl_xor_sync(0xffffffffu, acc[e], 4);
+        if (!((lane >> 2) & 1) && n + 1 < N && b < rows) {
+          const float g = acc[e];
+          st_any(ep.out, ep.out_dtype, (size_t)b * ep.out_ld + (n >> 1), __fdividef(g, 1.f + fast_exp(-g)) * other);
         }
-      } else if (n < N) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int b = c + e;
-          if (b < rows) {
-            if (partial) partial[((size_t)blockIdx.y * rows + b) * N + n] = acc[e];
-            else if (ep.act1 == ACT_NONE && !ep.resid && !ep.rowvec && !ep.row2seq && !ep.accumulate && !ep.out2 && ep.scale == 1.f)
-              st_any(ep.out, ep.out_dtype, (size_t)b * ep.out_ld + n, acc[e] + bias_n);   // plain Linear (+bias): no loads in the store loop
-            else epi_store(ep, b, n, acc[e]);
-          }
-        }
+      } else if (n < N && b < rows) {
+        if (partial) partial[((size_t)blockIdx.y * rows + b) * N + n] = acc[e];
+        else if (plain) st_any(ep.out, ep.out_dtype, (size_t)b * ep.out_ld + n, acc[e] + bias_n[hh]);   // plain Linear (+bias): no loads in the store loop
+        else epi_store(ep, b, n, acc[e]);
       }
     }
-  }
-  if (trace && threadIdx.x == 64) dbg[5] = clock64();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (trace && threadIdx.x == 64) dbg[6] = clock64();
-  if (trace && threadIdx.x == 0) dbg[2] = clock64();
-  if (dbg && threadIdx.x == 0 && cta_lin < 200) {
-    long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    dbg[128 + cta_lin * 4 + 3] = t;
   }
   tl_stamp(tl, 2);
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)(SK_NACC * BPAD)) : "memory");
-  }
 }
 
 // out = epilogue(sum_s partial[s]) in fixed split order
@@ -310,14 +214,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 template <int BPAD>
 void launch(cudaStream_t st, dim3 grid, const bf16* tw, const CUtensorMap& tx, const ConvW& W, int rows, int cps, float* partial,
-            const EpiDev& e, int swiglu, long long* dbg, bool pdl, long long* tl) {
+            const EpiDev& e, int swiglu, bool pdl, long long* tl) {
   constexpr size_t smem = (size_t)SK_STAGES * (SK_BM * SK_BK * 2 + BPAD * SK_BK * 2) + 1024;
   static bool attr = false;
   if (!attr) {
     CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<BPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
-  launch_ex(skinny_gemm_kernel<BPAD>, grid, dim3(SK_THREADS), smem, st, pdl, tw, tx, W.N, W.K, rows, cps, partial, e, swiglu, dbg, tl);
+  launch_ex(skinny_gemm_kernel<BPAD>, grid, dim3(SK_THREADS), smem, st, pdl, tw, tx, W.N, W.K, rows, cps, partial, e, swiglu, tl);
 }
 
 }  // namespace
@@ -330,7 +234,7 @@ const bf16* skinny_tiled_weights(cvk_ctx* ctx, const ConvW& W) {
   CVK_REQUIRE(!cvk_in_capture, "skinny_tiled_weights: weight was not pre-tiled before graph capture");
   const int tiles = ceil_div(W.N, SK_BM), kchunks = ceil_div(W.K, SK_BK);
   bf16* out = (bf16*)ctx->dmalloc((size_t)tiles * kchunks * SK_BM * SK_BK * sizeof(bf16));
-  tile_weights_kernel<<<148 * 8, 256>>>(W.w16, out, W.N, W.K, tiles, kchunks);
+  tile_weights_kernel<<<ctx->num_sms * 8, 256>>>(W.w16, out, W.N, W.K, tiles, kchunks);
   CVK_LAUNCH_CHECK();
   CVK_CHECK_CUDA(cudaDeviceSynchronize());
   ctx->tiled[W.w16] = out;
@@ -389,14 +293,14 @@ int conv_gemm_skinny_ex(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW
   dim3 grid(tiles, splits);
   float* partial = (splits > 1 || mode == 1) ? scratch : nullptr;
   long long* tl = ctx->tl_next();
-  if (BPAD == 32) launch<32>(st, grid, tw, tx, W, rows, cps, partial, e, mode == 2, (long long*)ctx->dbg, ctx->pdl != 0, tl);
-  else launch<64>(st, grid, tw, tx, W, rows, cps, partial, e, mode == 2, (long long*)ctx->dbg, ctx->pdl != 0, tl);
+  if (BPAD == 32) launch<32>(st, grid, tw, tx, W, rows, cps, partial, e, mode == 2, ctx->pdl != 0, tl);
+  else launch<64>(st, grid, tw, tx, W, rows, cps, partial, e, mode == 2, ctx->pdl != 0, tl);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   if (splits > 1 && mode == 0) {
     size_t total = (size_t)rows * W.N;
     int g = (int)((total + 255) / 256);
-    if (g > 148 * 4) g = 148 * 4;
+    if (g > ctx->num_sms * 4) g = ctx->num_sms * 4;
     launch_ex(splitk_finish_kernel, dim3(g), dim3(256), 0, st, ctx->pdl != 0, (const float*)partial, splits, rows, W.N, e, ctx->tl_next());
     ctx->launches++;
     CVK_LAUNCH_CHECK();

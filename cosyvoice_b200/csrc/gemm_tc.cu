@@ -1,23 +1,21 @@
-// bf16 conv-GEMM on 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM, operands staged by TMA).
+// bf16 / fp16 conv-GEMM on Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers, operands staged by TMA).
 //
 //   out[r, n] = epilogue( sum_{j<taps} sum_{k<K} A[r + shift0 + j*dil, k] * W[n][j][k] ),  fp32 accumulate
 //
-// One CTA computes a 128 x BN output tile.  Warp 0 is the TMA producer, warp 1 allocates TMEM and issues the
-// MMAs (single elected lane), warps 2-9 run the fused epilogue straight out of TMEM (one accumulator row per
-// thread, two warps per 32-row lane quarter splitting the columns).  A convolution tap is just a row-shifted TMA box of the time-major activation matrix; rows outside the
-// matrix and the K tail are zero-filled by the TMA unit, gap rows between ragged sequences hold zeros in memory.
-// Two CTAs are co-resident per SM (3 stages x 32 KB each) so one CTA's epilogue overlaps the other's main loop.
+// A convolution tap is just a row-shifted TMA box of the time-major activation matrix; rows outside the matrix and the K tail
+// are zero-filled by the TMA unit, gap rows between ragged sequences hold zeros in memory.
 //
 // Reference ops served: every dense Linear / Conv1d of the flow estimator + encoder (flow/decoder.py,
 // matcha transformer.py), the LM projections (transformers Qwen2, llm/llm.py:244-251) and the HiFT ResBlock /
 // upsampling convolutions (hifigan/generator.py:110-117, 432-443).
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;   // 64 bf16 = 128 B = one SWIZZLE_128B atom row
-constexpr int TC_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two warps per TMEM lane quarter, half the columns each)
+constexpr int TC_THREADS = 384;   // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue, 64 rows each
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -58,47 +56,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
       "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory operand descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 | LBO(=1, unused for swizzled K-major)<<16 | SBO(8 rows * 128 B = 1024 B)>>4 <<32 | version 1 <<46 | layout 2 <<61
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// issue-only variant: several loads can be in flight before one tmem_wait() (each tcgen05.wait::ld is a full TMEM round trip)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
 }
 
 // 16 consecutive columns of one row through the fused epilogue (vector fast path + scalar tail).
@@ -262,10 +227,9 @@ __device__ __forceinline__ void epi_math16(const EpiDev& e, int r, bool rin, int
   }
 }
 
-// epi_math16 for a full group of 16 columns of the persistent kernel: the row's sequence index has been resolved by the caller
-// (loaded one tile ahead) and the bias of the tile's columns sits in shared memory.  In epi_math16 the dependent row2seq load
-// (an L2 round trip) and the bias loads are issued after tcgen05.wait::ld in every group, four times per tile and thread:
-// removing the math of a to_q/k/v tile took the kernel from 78.9 to 48.2 us (ablation in profiles/r02_flow.md).
+// epi_math16 for a full group of 16 columns: the row's sequence index has been resolved by the caller (loaded before the main
+// loop) and the bias of the tile's columns sits in shared memory, so no dependent global load sits between the accumulator and
+// the stores.
 __device__ __forceinline__ void epi_math16p(const EpiDev& e, int r, bool rin, int seq, bool valid, const float* s_bias, int cl, int n0,
                                             const float* acc, float* v, float* w2) {
 #pragma unroll
@@ -344,346 +308,44 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
 }
 
-template <int BN, int TC_STAGES>
-__global__ void __launch_bounds__(TC_THREADS, 2)
-conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+// One CTA computes 128 x BN output tiles: warp 0 (lane 0) is the TMA producer, warpgroups 1 and 2 each issue wgmma for 64 of the
+// 128 rows and run the fused epilogue on their own accumulators.  With more tiles than CTAs (persistent launch, one CTA per SM)
+// a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (column tile fastest, so CTAs running at the same time share A
+// rows in L2); the operand ring runs across tile boundaries, so the producer fetches the next tile's operands while the
+// epilogue of the current one runs.  epi_mode 2: the tile is staged in SWIZZLE_128B sub-tiles of a dedicated 64 KB region and
+// written by TMA stores (full 128-byte lines; rows / columns outside the matrix are clipped by the tensor map); the elected thread
+// waits for a store to have read the staging tile only before the next tile is staged.  epi_mode 0: direct per-thread stores.
+constexpr uint32_t TC_STG_BYTES = 65536;
+
+template <int BN, int NSTG>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o2, int N, int K, int taps,
-                    int dil, int shift0, int rowsOut, EpiDev ep, int epi_mode, long long* __restrict__ dbg) {
-  extern __shared__ uint8_t smem_raw[];
-  long long t_entry = 0;
-  if (dbg) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_entry));
-  const int cta_lin = blockIdx.y * gridDim.x + blockIdx.x;
-  auto stamp = [&](int slot) {
-    if (dbg && cta_lin < 120) {
-      long long t;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-      dbg[cta_lin * 8 + slot] = t;
-    }
-  };
-  __shared__ __align__(8) uint64_t bar_full[TC_STAGES];
-  __shared__ __align__(8) uint64_t bar_empty[TC_STAGES];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
-  __shared__ __align__(16) float s_bias[BN];
-  __shared__ float s_a1[BN], s_a2[BN];
-
-  constexpr uint32_t A_BYTES = TC_BM * TC_BK * 2;
-  constexpr uint32_t B_BYTES = BN * TC_BK * 2;
-  constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  // UMMA instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): D=f32, A=B=bf16, K-major both,
-  // N>>3 at bit 17, M>>4 at bit 24
-  constexpr uint32_t IDESC_BF = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-  const uint32_t IDESC = ep.ab_f16 ? (IDESC_BF & ~((1u << 7) | (1u << 10))) : IDESC_BF;   // a/b format 0 = IEEE half, 1 = bf16
-
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024-B aligned tiles
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n0 = blockIdx.x * BN;
-  const int r0 = blockIdx.y * TC_BM;
-  const int kchunks = (K + TC_BK - 1) / TC_BK;
-  const int iters = taps * kchunks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    mbar_init(smem_u32(&bar_acc), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    // TMEM: BN fp32 accumulator columns (power of two >= 32)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"((uint32_t)BN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_slot;
-  if (threadIdx.x == 0 && dbg && cta_lin < 120) { dbg[cta_lin * 8 + 0] = t_entry; stamp(1); }
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int it = 0; it < iters; ++it) {
-        const int s = it % TC_STAGES;
-        const uint32_t round = (uint32_t)(it / TC_STAGES);
-        mbar_wait(smem_u32(&bar_empty[s]), (round & 1u) ^ 1u);
-        const int j = it / kchunks, kc = it - j * kchunks;
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-        const uint32_t fb = smem_u32(&bar_full[s]);
-        mbar_expect_tx(fb, STAGE_BYTES);
-        tma_load_2d(sa, &tmap_a, fb, kc * TC_BK, r0 + shift0 + j * dil);
-        tma_load_3d(sb, &tmap_w, fb, kc * TC_BK, j, n0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int it = 0; it < iters; ++it) {
-        const int s = it % TC_STAGES;
-        const uint32_t round = (uint32_t)(it / TC_STAGES);
-        mbar_wait(smem_u32(&bar_full[s]), round & 1u);
-        if (it == 0) stamp(6);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-        const uint64_t da = umma_desc_sw128(sa), db = umma_desc_sw128(sb);
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)     // advance 16 elements = 32 B along K inside the 128-B swizzle atom: +2 in the address field
-          umma_bf16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, (it > 0 || k > 0) ? 1u : 0u);
-        umma_commit(smem_u32(&bar_empty[s]));   // frees the smem stage once these MMAs have read it
-      }
-      umma_commit(smem_u32(&bar_acc));          // accumulator complete
-    }
-  } else {
-    // epilogue: warp w may touch TMEM lanes 32*(w%4) .. +31 only.  Everything that does not depend on the accumulator
-    // (row validity, bias / Snake alphas -> shared memory, first residual chunk) is fetched while the main loop runs, and
-    // the global loads of chunk c+1 are issued before the stores of chunk c (stores would otherwise fence the loads:
-    // the compiler cannot prove the epilogue pointers do not alias, and each chunk would pay a full L2 round trip).
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = r0 + q * 32 + lane;
-    const bool rin = r < rowsOut;
-    if (epi_mode == 2) {
-      // coalesced output: the tile is staged in shared memory (the operand stages are free once the accumulator is
-      // complete) in SWIZZLE_128B sub-tiles and written by TMA stores - full 128-byte lines instead of one 32/64-byte
-      // piece per thread per row; rows / columns outside the matrix are clipped by the tensor map.
-      // the row's sequence index and the bias of the tile's columns are fetched while the main loop runs (epi_math16p)
-      int seq = 0;
-      if (rin && ep.row2seq) seq = ep.row2seq[r];
-      const bool valid = rin && (!ep.row2seq || seq >= 0);
-      for (int i = threadIdx.x - 64; i < BN; i += 256) s_bias[i] = (ep.bias && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(smem_u32(&bar_acc), 0);
-      if (threadIdx.x == 64) stamp(2);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t trow0 = tmem_base + ((uint32_t)(q * 32) << 16);
-      const int row = q * 32 + lane;
-      const uint32_t stg1 = smem_base;
-      const uint32_t stg2 = smem_base + (uint32_t)TC_BM * BN * (ep.out_dtype == DT_F32 ? 4u : 2u);
-#pragma unroll 1
-      for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
-        if (n0 + c >= N) break;
-        const bool full32 = n0 + c + 32 <= N;
-        uint32_t ra[16], rb[16];
-        tmem_ld16_nowait(trow0 + (uint32_t)c, ra);             // two loads in flight, one wait
-        tmem_ld16_nowait(trow0 + (uint32_t)(c + 16), rb);
-        tmem_wait();
-        float acc[16], v[16], w2[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i] = __uint_as_float(ra[i]);
-        if (full32) epi_math16p(ep, r, rin, seq, valid, s_bias, c, n0 + c, acc, v, w2);
-        else epi_math16(ep, r, rin, n0 + c, N, acc, v, w2);
-        stage_store16(stg1, ep.out_dtype, row, c, v);
-        if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c, w2);
-        if (n0 + c + 16 < N) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[i] = __uint_as_float(rb[i]);
-          if (full32) epi_math16p(ep, r, rin, seq, valid, s_bias, c + 16, n0 + c + 16, acc, v, w2);
-          else epi_math16(ep, r, rin, n0 + c + 16, N, acc, v, w2);
-          stage_store16(stg1, ep.out_dtype, row, c + 16, v);
-          if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c + 16, w2);
-        }
-      }
-      if (threadIdx.x == 64) stamp(3);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (threadIdx.x == 64) stamp(4);
-      if (threadIdx.x == 64) {
-        const int w1 = ep.out_dtype == DT_F32 ? 32 : 64;
-        for (int sb = 0; sb * w1 < BN && n0 + sb * w1 < N; ++sb) tma_store_2d(&tmap_o, stg1 + sb * 16384u, n0 + sb * w1, r0);
-        if (ep.out2) {
-          const int w2c = ep.out2_dtype == DT_F32 ? 32 : 64;
-          for (int sb = 0; sb * w2c < BN && n0 + sb * w2c < N; ++sb) tma_store_2d(&tmap_o2, stg2 + sb * 16384u, n0 + sb * w2c, r0);
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the staging tile may be released once it has been read
-        stamp(5);
-      }
-    } else if (epi_mode == 0) {   // simple epilogue: loads inside the per-chunk routine
-      mbar_wait(smem_u32(&bar_acc), 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t trow0 = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 16) {
-        if (n0 + c >= N) break;
-        float acc[16];
-        tmem_ld16(trow0 + (uint32_t)c, acc);
-        if (rin) epi_store16(ep, r, n0 + c, N, acc);
-      }
-    } else {
-    int seq = 0;
-    bool valid = rin;
-    if (rin && ep.row2seq) {
-      seq = ep.row2seq[r];
-      valid = seq >= 0;
-    }
-    for (int i = threadIdx.x - 64; i < BN; i += 256) {
-      const int n = n0 + i;
-      s_bias[i] = (ep.bias && n < N) ? ep.bias[n] : 0.f;
-      s_a1[i] = (ep.alpha1 && n < N) ? ep.alpha1[n] : 1.f;
-      s_a2[i] = (ep.alpha2 && n < N) ? ep.alpha2[n] : 1.f;
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const int c_begin = half * (BN / 2), c_end = (half + 1) * (BN / 2);
-    const float* pa_src = nullptr;      // residual row or per-sequence vector row (never both: checked on the host)
-    if (ep.resid && rin) pa_src = ep.resid + (size_t)r * ep.resid_ld + n0;
-    else if (ep.rowvec && valid) pa_src = ep.rowvec + (size_t)seq * ep.rowvec_ld + n0;
-    const bool pa_is_resid = ep.resid != nullptr;
-    const float* pb_src = (ep.accumulate && rin && ep.out_dtype == DT_F32) ? (const float*)ep.out + (size_t)r * ep.out_ld + n0 : nullptr;
-    float4 pa[4], pb[4];
-    auto prefetch = [&](int c) {
-      const bool full = n0 + c + 16 <= N;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        pa[i] = (pa_src && full) ? *reinterpret_cast<const float4*>(pa_src + c + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        pb[i] = (pb_src && full) ? *reinterpret_cast<const float4*>(pb_src + c + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    };
-    if (n0 + c_begin < N) prefetch(c_begin);
-    mbar_wait(smem_u32(&bar_acc), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c = c_begin; c < c_end; c += 16) {
-      if (n0 + c >= N) break;   // warp-uniform
-      float acc[16];
-      tmem_ld16(trow + (uint32_t)c, acc);
-      if (n0 + c + 16 > N) {    // ragged last chunk: scalar path
-        if (rin)
-          for (int i = 0; i < 16 && n0 + c + i < N; ++i) epi_store<true>(ep, r, n0 + c + i, acc[i]);
-        continue;
-      }
-      float v[16];
-      const float av[16] = {pa[0].x, pa[0].y, pa[0].z, pa[0].w, pa[1].x, pa[1].y, pa[1].z, pa[1].w,
-                            pa[2].x, pa[2].y, pa[2].z, pa[2].w, pa[3].x, pa[3].y, pa[3].z, pa[3].w};
-      const float bv[16] = {pb[0].x, pb[0].y, pb[0].z, pb[0].w, pb[1].x, pb[1].y, pb[1].z, pb[1].w,
-                            pb[2].x, pb[2].y, pb[2].z, pb[2].w, pb[3].x, pb[3].y, pb[3].z, pb[3].w};
-      if (c + 16 < c_end && n0 + c + 16 < N) prefetch(c + 16);   // next chunk's loads go out before this chunk's stores
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        float t = acc[i] + s_bias[c + i];
-        if (!pa_is_resid) t += av[i];
-        if (ep.act1 != ACT_NONE) t = apply_act_fast(ep.act1, t, ep.act1_param, s_a1[c + i]);
-        t *= ep.scale;
-        if (pa_is_resid) t += av[i];
-        if (!valid) t = 0.f;
-        v[i] = t;
-      }
-      if (!rin) continue;
-      const size_t o = (size_t)r * ep.out_ld + n0 + c;
-      if (ep.out_dtype == DT_F32) {
-        float* op = (float*)ep.out + o;
-        if (ep.accumulate) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] += bv[i];
-        }
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(op + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-      } else {
-        unsigned short* op = (unsigned short*)ep.out + o;
-        if (ep.accumulate) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] += f16bits_to_f32(op[i], ep.out_dtype);
-        }
-        __align__(16) unsigned short tt[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) tt[i] = f32_to_16(v[i], ep.out_dtype);
-        *reinterpret_cast<uint4*>(op) = *reinterpret_cast<uint4*>(tt);
-        *reinterpret_cast<uint4*>(op + 8) = *reinterpret_cast<uint4*>(tt + 8);
-      }
-      if (ep.out2) {
-        float w2[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) w2[i] = valid ? apply_act_fast(ep.act2, v[i], ep.act2_param, s_a2[c + i]) : 0.f;
-        const size_t o2 = (size_t)r * ep.out2_ld + n0 + c;
-        if (ep.out2_dtype == DT_F32) {
-          float* op = (float*)ep.out2 + o2;
-#pragma unroll
-          for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(op + i) = make_float4(w2[i], w2[i + 1], w2[i + 2], w2[i + 3]);
-        } else {
-          unsigned short* op = (unsigned short*)ep.out2 + o2;
-          __align__(16) unsigned short tt[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) tt[i] = f32_to_16(w2[i], ep.out2_dtype);
-          *reinterpret_cast<uint4*>(op) = *reinterpret_cast<uint4*>(tt);
-          *reinterpret_cast<uint4*>(op + 8) = *reinterpret_cast<uint4*>(tt + 8);
-        }
-      }
-    }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ persistent variant
-// One CTA per SM walks a static list of 128x128 output tiles (column tile fastest, so the CTAs running at the same time
-// share A rows in L2).  Two TMEM accumulators (2 x 128 columns): the MMA warp fills buffer t&1 for tile t while the eight
-// epilogue warps drain buffer (t-1)&1, so the epilogue (TMEM -> registers -> fused math -> swizzled staging tile -> TMA
-// store) overlaps the next tile's main loop, and barrier setup / TMEM allocation / tensor-map fetch are paid once per SM
-// instead of once per tile.  The operand ring runs across tile boundaries (the producer never drains).
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-// BN = 128 or 256 output columns per tile.  The wide tile halves the re-reads of the A rows: ncu shows the 128 x 128 kernel moving
-// 6.5-6.9 TB/s from L2 to the SMs on the K = 256 / 512 GEMMs of the estimator (l1tex__m_xbar2l1tex_read_bytes: 494 MB for a
-// 32.8 GFLOP to_qkv) - operand traffic out of L2, not the tensor pipe, bounds them (profiles/r02_flow.md).
-template <int NSTG, int EW, int BN>   // EW epilogue warps (8 or 16): EW/4 warps share a TMEM lane quarter and split the columns
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
-conv_gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                            const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o2, int N, int K, int taps,
-                            int dil, int shift0, int rowsOut, EpiDev ep, int ntn, int ntiles, int stg_bufs) {
+                    int dil, int shift0, int rowsOut, EpiDev ep, int epi_mode, int ntn, int ntiles) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[NSTG];
   __shared__ __align__(8) uint64_t bar_empty[NSTG];
-  __shared__ __align__(8) uint64_t bar_accf[2];
-  __shared__ __align__(8) uint64_t bar_acce[2];
-  __shared__ uint32_t tmem_base_slot;
-  __shared__ __align__(16) float s_bias[2][BN];      // bias of the current / next tile's columns (epilogue warps)
+  __shared__ __align__(16) float s_bias[BN];
   constexpr uint32_t A_BYTES = TC_BM * TC_BK * 2;
   constexpr uint32_t B_BYTES = BN * TC_BK * 2;
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t IDESC_BF = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-  const uint32_t IDESC = ep.ab_f16 ? (IDESC_BF & ~((1u << 7) | (1u << 10))) : IDESC_BF;   // a/b format 0 = IEEE half, 1 = bf16
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t stg_base = smem_base + NSTG * STAGE_BYTES;          // 64 KB staging region (one 64 KB or two 32 KB tiles)
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B needs 1024-B aligned tiles
+  const uint32_t stg_base = smem_base + NSTG * STAGE_BYTES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kchunks = (K + TC_BK - 1) / TC_BK;
   const int iters = taps * kchunks;
-  // "part mode": with 16 epilogue warps and a single staging tile, the 64 (16-bit) / 32 (fp32) columns of one group of four warps
-  // are exactly one 16 KB TMA sub-tile.  Each group then runs its own staging pipeline (own named barrier, own elected thread
-  // issuing its sub-tile's store and waiting for it only right before the NEXT tile's first staging write), instead of all 16
-  // warps meeting at two CTA-wide barriers around one thread that issues four stores and waits ~1 us for the whole 64 KB tile to
-  // be read (ablation in profiles/r02_flow.md: the store path cost 19 of 79 us of a to_qkv launch).
-  const bool pm = EW == 16 && stg_bufs == 1 && ep.out2 == nullptr && (BN / 4) * (ep.out_dtype == DT_F32 ? 4 : 2) == 128;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSTG; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&bar_accf[b]), 1);
-      mbar_init(smem_u32(&bar_acce[b]), pm ? 4 : 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"(2u * BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int r0 = (tile / ntn) * TC_BM, n0 = (tile % ntn) * BN;
@@ -699,123 +361,77 @@ conv_gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap tmap_a, const __
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-        const uint32_t buf = tcount & 1u, use = tcount >> 1;
-        mbar_wait(smem_u32(&bar_acce[buf]), (use & 1u) ^ 1u);     // the epilogue has drained this accumulator (first use: free)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + buf * BN;
-        for (int i = 0; i < iters; ++i, ++it) {
-          const uint32_t s = it % NSTG, round = it / NSTG;
-          mbar_wait(smem_u32(&bar_full[s]), round & 1u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
-          const uint32_t sb = sa + A_BYTES;
-          const uint64_t da = umma_desc_sw128(sa), db = umma_desc_sw128(sb);     // +32 bytes along K = +2 in the 16-byte address field
+    return;
+  }
+  const int ct = threadIdx.x - 128;                   // consumer thread 0..255
+  const int wg = ct >> 7;                             // rows [64 wg, 64 wg + 64) of the tile
+  const int q = lane & 3;
+  const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);   // the tile row this thread's epilogue owns
+  const int cq = 16 * (q >> 1);                       // ... and its 16 columns of every 32
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int r0 = (tile / ntn) * TC_BM, n0 = (tile % ntn) * BN;
+    const int r = r0 + row;
+    const bool rin = r < rowsOut;
+    // the previous tile's epilogue has read s_bias, and its TMA store has read the staging tile (thread 0 waited below)
+    if (ct == 0 && epi_mode == 2) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    for (int i = ct; i < BN; i += 256) s_bias[i] = (ep.bias && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
+    int seq = 0;
+    if (rin && ep.row2seq) seq = ep.row2seq[r];
+    const bool valid = rin && (!ep.row2seq || seq >= 0);
+
+    float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) umma_bf16(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, (i > 0 || k > 0) ? 1u : 0u);
-          umma_commit(smem_u32(&bar_empty[s]));
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < iters; ++i, ++it) {
+      const uint32_t s = it % NSTG, round = it / NSTG;
+      mbar_wait(smem_u32(&bar_full[s]), round & 1u);
+      const uint32_t sa = smem_base + s * STAGE_BYTES + (uint32_t)wg * (A_BYTES / 2);
+      const uint32_t sb = smem_base + s * STAGE_BYTES + A_BYTES;
+      const uint64_t da = wg_desc_sw128(sa), db = wg_desc_sw128(sb);
+      wg_fence();
+      if (ep.ab_f16) {
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) wgmma_ss<BN, 1>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      } else {
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) wgmma_ss<BN, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      }
+      wg_commit();
+      // one group stays in flight: the stage of the previous iteration is released once its MMAs have completed
+      wg_wait<1>();
+      __syncwarp();
+      if (i > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(it - 1) % NSTG]));
+    }
+    wg_wait<0>();
+    wg_touch<BN / 2>(acc);
+    __syncwarp();
+    if (iters > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(it - 1) % NSTG]));
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // s_bias complete
+
+    const uint32_t stg1 = stg_base;
+    const uint32_t stg2 = stg_base + (uint32_t)TC_BM * BN * (ep.out_dtype == DT_F32 ? 4u : 2u);
+#pragma unroll
+    for (int cb = 0; cb < BN; cb += 32) {
+      float a16[16], v[16], w2[16];
+      wg_frag_rows16(acc + cb / 2, lane, a16);
+      const int c = cb + cq;
+      if (n0 + c < N) {
+        if (epi_mode == 2) {
+          if (n0 + c + 16 <= N) epi_math16p(ep, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
+          else epi_math16(ep, r, rin, n0 + c, N, a16, v, w2);
+          stage_store16(stg1, ep.out_dtype, row, c, v);
+          if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c, w2);
+        } else if (rin) {
+          epi_store16(ep, r, n0 + c, N, a16);
         }
-        umma_commit(smem_u32(&bar_accf[buf]));
       }
     }
-  } else {
-    const int q = warp & 3;
-    const int part = (warp - 2) >> 2;
-    constexpr int CPP = BN / (EW / 4);                 // columns per warp
-    constexpr int ETHREADS = 32 * EW;
-    const int row = q * 32 + lane;
-    const uint32_t out_tile_bytes = (uint32_t)TC_BM * BN * (ep.out_dtype == DT_F32 ? 4u : 2u);
-    uint32_t tcount = 0;
-    // operands of a tile's epilogue that do not depend on its accumulator are fetched ONE TILE AHEAD, under the previous tile's
-    // column loop: the row's sequence index (register) and the bias of the tile's columns (shared memory, two buffers)
-    auto fetch_seq = [&](int tile) -> int {
-      const int rr = (tile / ntn) * TC_BM + row;
-      return (tile < ntiles && rr < rowsOut && ep.row2seq) ? ep.row2seq[rr] : 0;
-    };
-    const int pt = (int)threadIdx.x - 64 - part * 128;     // index inside the group of four warps that shares `part`
-    const bool elected = pt == 0;
-    const int part_bar = 2 + part;                         // named barriers 2..5 (1 = all epilogue warps, 0 = __syncthreads)
-    auto fetch_bias = [&](int tile, uint32_t b) {
-      if (tile >= ntiles) return;
-      const int nn = (tile % ntn) * BN;
-      if (pm) {
-        for (int i = pt; i < CPP; i += 128) s_bias[b][part * CPP + i] = (ep.bias && nn + part * CPP + i < N) ? ep.bias[nn + part * CPP + i] : 0.f;
-      } else {
-        for (int i = threadIdx.x - 64; i < BN; i += ETHREADS) s_bias[b][i] = (ep.bias && nn + i < N) ? ep.bias[nn + i] : 0.f;
-      }
-    };
-    int seq_next = fetch_seq(blockIdx.x);
-    fetch_bias(blockIdx.x, 0);
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-      const int r0 = (tile / ntn) * TC_BM, n0 = (tile % ntn) * BN;
-      const int r = r0 + row;
-      const bool rin = r < rowsOut;
-      const uint32_t buf = tcount & 1u, use = tcount >> 1;
-      const int seq = seq_next;
-      const bool valid = rin && (!ep.row2seq || seq >= 0);
-      seq_next = fetch_seq(tile + gridDim.x);
-      fetch_bias(tile + gridDim.x, (tcount + 1) & 1u);      // every thread (of the part) is past the column loop of the tile that used this buffer
-      // staging tile of this iteration: with two buffers the one used two tiles ago has been read by its TMA store
-      // (thread 64 waited for that before reaching this barrier)
-      if (!pm) asm volatile("bar.sync 1, %0;" ::"n"(ETHREADS) : "memory");
-      const uint32_t stg1 = stg_base + (stg_bufs == 2 ? (tcount & 1u) * 32768u : 0u);
-      const uint32_t stg2 = stg1 + out_tile_bytes;
-      const float* sb = s_bias[tcount & 1u];
-      mbar_wait(smem_u32(&bar_accf[buf]), use & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t trow0 = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16);
-      bool may_stage = !pm;
-#pragma unroll 1
-      for (int c = part * CPP; c < (part + 1) * CPP; c += 32) {
-        if (n0 + c >= N) break;
-        const bool full32 = n0 + c + 32 <= N;
-        uint32_t ra[16], rb[16];
-        tmem_ld16_nowait(trow0 + (uint32_t)c, ra);
-        tmem_ld16_nowait(trow0 + (uint32_t)(c + 16), rb);
-        tmem_wait();
-        float acc[16], v[16], w2[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i] = __uint_as_float(ra[i]);
-        if (full32) epi_math16p(ep, r, rin, seq, valid, sb, c, n0 + c, acc, v, w2);
-        else epi_math16(ep, r, rin, n0 + c, N, acc, v, w2);
-        if (!may_stage) {
-          // part mode: the sub-tile may be overwritten once the store of the previous tile has read it (and the bias written by the
-          // part's threads for this tile is visible)
-          if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          asm volatile("bar.sync %0, 128;" ::"r"(part_bar) : "memory");
-          may_stage = true;
-        }
-        stage_store16(stg1, ep.out_dtype, row, c, v);
-        if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c, w2);
-        if (n0 + c + 16 < N) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[i] = __uint_as_float(rb[i]);
-          if (full32) epi_math16p(ep, r, rin, seq, valid, sb, c + 16, n0 + c + 16, acc, v, w2);
-          else epi_math16(ep, r, rin, n0 + c + 16, N, acc, v, w2);
-          stage_store16(stg1, ep.out_dtype, row, c + 16, v);
-          if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c + 16, w2);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (epi_mode == 2) {
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      if (pm) {
-        asm volatile("bar.sync %0, 128;" ::"r"(part_bar) : "memory");
-        if (elected) {
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          mbar_arrive(smem_u32(&bar_acce[buf]));      // 4 arrivals: every part has finished reading this accumulator
-          const int w1 = ep.out_dtype == DT_F32 ? 32 : 64;
-          if (n0 + part * w1 < N) tma_store_2d(&tmap_o, stg1 + (uint32_t)part * 16384u, n0 + part * w1, r0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        continue;
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(ETHREADS) : "memory");
-      if (threadIdx.x == 64) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        mbar_arrive(smem_u32(&bar_acce[buf]));      // every epilogue thread has finished reading this accumulator
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (ct == 0) {
         const int w1 = ep.out_dtype == DT_F32 ? 32 : 64;
         for (int sb = 0; sb * w1 < BN && n0 + sb * w1 < N; ++sb) tma_store_2d(&tmap_o, stg1 + sb * 16384u, n0 + sb * w1, r0);
         if (ep.out2) {
@@ -823,18 +439,10 @@ conv_gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap tmap_a, const __
           for (int sb = 0; sb * w2c < BN && n0 + sb * w2c < N; ++sb) tma_store_2d(&tmap_o2, stg2 + sb * 16384u, n0 + sb * w2c, r0);
         }
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        if (stg_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
       }
     }
-    if (pm && elected) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2u * BN) : "memory");
-  }
+  if (ct == 0 && epi_mode == 2) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -852,31 +460,19 @@ EncodeTiledFn get_encode(cvk_ctx* ctx) {
   return (EncodeTiledFn)ctx->encode_tiled;
 }
 
-template <int BN, int TC_STAGES>
-void launch_tc(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const CUtensorMap& to2,
+template <int BN, int NSTG>
+void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const CUtensorMap& to2,
                const ConvW& W, int rowsOut, const EpiDev& e, int epi_mode) {
-  constexpr size_t smem = (size_t)TC_STAGES * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + 1024;
+  constexpr size_t smem = (size_t)NSTG * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + TC_STG_BYTES + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, TC_STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  dim3 grid(ceil_div(W.N, BN), ceil_div(rowsOut, TC_BM));
-  conv_gemm_tc_kernel<BN, TC_STAGES><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode, (long long*)ctx->dbg);
-}
-
-template <int NSTG, int EW, int BN>
-void launch_tc_persist(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const CUtensorMap& to2,
-                       const ConvW& W, int rowsOut, const EpiDev& e, int stg_bufs) {
-  constexpr size_t smem = (size_t)NSTG * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + 65536 + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_tc_persist_kernel<NSTG, EW, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<BN, NSTG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   const int ntn = ceil_div(W.N, BN), ntiles = ntn * ceil_div(rowsOut, TC_BM);
-  const int grid = ntiles < ctx->num_sms ? ntiles : ctx->num_sms;
-  conv_gemm_tc_persist_kernel<NSTG, EW, BN><<<grid, 64 + 32 * EW, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, ntn, ntiles, stg_bufs);
+  // more tiles than SMs: persistent CTAs (one per SM) unless switched off
+  const int grid = (ctx->tc_persist && ntiles > ctx->num_sms) ? ctx->num_sms : ntiles;
+  conv_gemm_wg_kernel<BN, NSTG><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode, ntn, ntiles);
 }
 
 }  // namespace
@@ -888,10 +484,7 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   CVK_REQUIRE(W.K % 8 == 0 && A.ld % 8 == 0 && ((uintptr_t)A.p & 15) == 0, "conv_gemm_tc: operands must be 16-byte aligned");
   CVK_REQUIRE(ep.out.p != nullptr && ep.out.cols >= W.N, "conv_gemm_tc: bad output");
   EncodeTiledFn enc = get_encode(ctx);
-  // persistent 128 x 256 tiles: 16-bit single output (64 KB staging tile), N a multiple of 256, more tiles than SMs
-  const bool persist256 = ctx->tc_persist && ctx->tc_pbn256 && ctx->tc_epi == 2 && W.N % 256 == 0 && ep.out.esize() == 2 && !ep.out2.p && !ep.accumulate &&
-                          (W.N / 256) * ceil_div(ep.out.rows, TC_BM) > ctx->num_sms;
-  const int BN = (persist256 || (ctx->tc_bn256 && W.N > 128)) ? 256 : (W.N > 64 ? 128 : 64);
+  const int BN = W.N > 64 ? 128 : 64;
   CUtensorMap ta, tw;
   {
     cuuint64_t dims[2] = {(cuuint64_t)W.K, (cuuint64_t)A.rows};
@@ -923,15 +516,13 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   const double flops = 2.0 * rowsOut * (double)W.N * W.K * W.taps;
   const double bytes = (double)rowsOut * W.K * 2 + (double)W.N * W.K * W.taps * 2 + (double)rowsOut * W.N * ep.out.esize();
   ProfScope ps(ctx, st, FAM_GEMM_TC, flops, bytes);
-  // epilogue mode: 2 = staged TMA stores (default when the tile fits the free operand stages and no read-modify-write of
-  // the output is needed), 0 = direct per-thread stores, 1 = direct stores with software-pipelined loads (experiment)
-  int epi_mode = ctx->tc_epi;
+  // epilogue mode: 2 = staged TMA stores (default when the output tile(s) fit the staging region and no read-modify-write of the
+  // output is needed), otherwise direct per-thread stores
+  int epi_mode = ctx->tc_epi == 2 ? 2 : 0;
   CUtensorMap to = ta, to2 = ta;
   if (epi_mode == 2) {
-    const int stages = BN == 256 ? 2 : (BN == 128 ? 3 : 4);
-    const size_t stage_bytes = (size_t)stages * (TC_BM * TC_BK * 2 + BN * TC_BK * 2);
     const size_t need = (size_t)TC_BM * BN * ep.out.esize() + (ep.out2.p ? (size_t)TC_BM * BN * ep.out2.esize() : 0);
-    if (ep.accumulate || need > stage_bytes) epi_mode = 0;
+    if (ep.accumulate || need > TC_STG_BYTES) epi_mode = 0;
   }
   if (epi_mode == 2) {
     auto mk = [&](CUtensorMap* m, const Mat& o) {
@@ -946,26 +537,8 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
     mk(&to, ep.out);
     if (ep.out2.p) mk(&to2, ep.out2);
   }
-  const size_t need_stage = (size_t)TC_BM * 128 * ep.out.esize() + (ep.out2.p ? (size_t)TC_BM * 128 * ep.out2.esize() : 0);
-  const int ntiles_p = ceil_div(W.N, 128) * ceil_div(rowsOut, TC_BM);
-  if (persist256 && epi_mode == 2) {
-    if (ctx->tc_persist == 2) launch_tc_persist<3, 16, 256>(ctx, st, ta, tw, to, to2, W, rowsOut, e, 1);
-    else launch_tc_persist<3, 8, 256>(ctx, st, ta, tw, to, to2, W, rowsOut, e, 1);
-    ctx->launches++;
-    CVK_LAUNCH_CHECK();
-    return;
-  }
-  if (ctx->tc_persist && BN == 128 && epi_mode == 2 && need_stage <= 65536 && ntiles_p > ctx->num_sms) {
-    // more tiles than SMs: persistent CTAs with double-buffered accumulators (epilogue overlaps the next main loop)
-    if (ctx->tc_persist == 2) launch_tc_persist<4, 16, 128>(ctx, st, ta, tw, to, to2, W, rowsOut, e, need_stage <= 32768 ? 2 : 1);
-    else launch_tc_persist<4, 8, 128>(ctx, st, ta, tw, to, to2, W, rowsOut, e, need_stage <= 32768 ? 2 : 1);
-    ctx->launches++;
-    CVK_LAUNCH_CHECK();
-    return;
-  }
-  if (BN == 256) launch_tc<256, 2>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);      // 2 x 48 KB stages: two CTAs (2 x 256 TMEM columns) per SM
-  else if (BN == 128) launch_tc<128, 3>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
-  else launch_tc<64, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+  if (BN == 128) launch_wg<128, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+  else launch_wg<64, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }

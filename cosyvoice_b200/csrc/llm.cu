@@ -223,8 +223,7 @@ __global__ void __launch_bounds__(D) finish_rms_kernel(const float* __restrict__
 
 // qkv split-K reduction + bias + RoPE + KV-cache append + GQA decode attention; one CTA per (row, kv head): see
 // llm_decode_attn.cuh (the same unit runs inside the persistent decode kernel, llm_mega.cu).
-// The CUDA-core version this replaces spent 6.8 + 4.7 us in QK^T / P V at 215 keys (bf16->fp32 conversion + FMA per element, per
-// head), a third of the whole decode step.
+// QK^T and P V run on mma.sync instead of CUDA-core FMAs (which would need a bf16->fp32 conversion + FMA per element, per head).
 constexpr int AF_WARPS = 16;
 __global__ void __launch_bounds__(32 * AF_WARPS)
 attn_fused_kernel(const float* __restrict__ partial /*[S][rows][1152]*/, int splits, int rows, const float* __restrict__ bias,
@@ -314,8 +313,7 @@ __device__ __forceinline__ float block_hsum(float seg, float* part, float* total
 // standalone mode (cvk_ras_sample): `scores` already holds log-probs, history given explicitly, no state update.
 //
 // The row lives in SHARED memory for the whole kernel (one coalesced read, one coalesced write-back of the log-probs with the
-// reference's in-place -inf marks): round 1 walked the global row with a 104-byte stride per lane in ~8 dependent passes and took
-// 91 us per decode step (in-kernel stamps, profiles/r02_lm_mega.md) - 9 % of the step.  The arithmetic (segment order of every
+// reference's in-place -inf marks) instead of walking the global row with a 104-byte stride per lane in ~8 dependent passes.  The arithmetic (segment order of every
 // float32 sum, stable tie-break of the nucleus) is unchanged.
 __global__ void __launch_bounds__(SAMPLER_THREADS)
 ras_sampler_kernel(float* __restrict__ scores, int V, int from_logits, const float* __restrict__ uniforms /*[..][B][2]*/, int B,
@@ -363,7 +361,7 @@ ras_sampler_kernel(float* __restrict__ scores, int V, int from_logits, const flo
   const float u2 = standalone ? uniforms[b * 2 + 1] : uniforms[((size_t)cnt * B + b) * 2 + 1];
   __syncthreads();
   // The thread's contiguous segment (<= SAMPLER_PER entries) lives in REGISTERS from here on: every pass below is an unrolled
-  // register loop (the shared-memory version was a chain of ~30-cycle dependent LDS per element: 48 us per step).  Entries past
+  // register loop (a shared-memory version would be a chain of dependent LDS per element).  Entries past
   // the segment hold -inf (scores) / -3 (probabilities) and are skipped by the ordered sums.
   float xr[SAMPLER_PER], pr[SAMPLER_PER];
 #pragma unroll
@@ -413,7 +411,7 @@ ras_sampler_kernel(float* __restrict__ scores, int V, int from_logits, const flo
   }
   SF();
   // (4) nucleus: repeatedly take the largest remaining probability (ties -> lowest index == stable sort).  The 25 rounds are a
-  // serial chain, so a round is kept short (it was ~1 us: two 5-level shuffle trees + a 27-entry rescan by the owner): every
+  // serial chain, so a round is kept short (instead of two 5-level shuffle trees + a 27-entry rescan by the owner): every
   // thread caches the three largest remaining entries of its segment (popped in O(1), rebuilt only when exhausted), the warp
   // winner comes from two redux.sync (probabilities are >= 0, so their bit patterns order like unsigned integers; +1 keeps 0.0
   // above "nothing left"), the 8 warp winners are double-buffered so that one barrier per round suffices, and every thread
@@ -439,7 +437,7 @@ ras_sampler_kernel(float* __restrict__ scores, int V, int from_logits, const flo
   __shared__ unsigned s_thr_key;
   int n_kept = 0;
   float cum = 0.f;
-  // Fast exact selection (replaces 25 serial block-wide rounds, ~0.7 us each): the 25 largest entries are all >= the 25th largest
+  // Fast exact selection (instead of 25 serial block-wide rounds): the 25 largest entries are all >= the 25th largest
   // of the 256 per-thread maxima, so (a) rank the thread maxima (every thread counts how many precede its own: one pass over 256
   // shared entries), (b) gather the entries >= that threshold into a candidate list (typically 25-60 of 6564), (c) rank the
   // candidates the same way - order (value desc, index asc) == the reference's stable descending sort.  If the candidate list
@@ -811,7 +809,7 @@ void layer_forward(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, int li, con
   {
     size_t total = (size_t)rows * DFF;
     int g = (int)((total + 255) / 256);
-    if (g > 148 * 8) g = 148 * 8;
+    if (g > 132 * 8) g = 132 * 8;
     if (gu.dtype == DT_F32) swiglu_kernel<float><<<g, 256, 0, st>>>(gu.f32(), gu.ld, rows, ffa.f32(), ffa.ld);
     else swiglu_kernel<bf16><<<g, 256, 0, st>>>(gu.b16(), gu.ld, rows, ffa.b16(), ffa.ld);
     ctx->launches++;
@@ -880,7 +878,7 @@ void llm_build(cvk_ctx* ctx, const int* cfg, int ncfg) {
     if (ctx->precision == CVK_PREC_BF16) {
       w.gate_up_il.N = 2 * DFF; w.gate_up_il.K = D;
       w.gate_up_il.w32 = (float*)ctx->dmalloc((size_t)2 * DFF * D * sizeof(float));
-      interleave_rows_kernel<<<148 * 8, 256>>>(w.gate_up.w32, w.gate_up_il.w32, DFF, D);
+      interleave_rows_kernel<<<132 * 8, 256>>>(w.gate_up.w32, w.gate_up_il.w32, DFF, D);
       CVK_LAUNCH_CHECK();
       finish_convw(ctx, w.gate_up_il);
     }

@@ -4,7 +4,7 @@
 // qkv split-K reduction + bias + RoPE + KV-cache append + GQA decode attention (transformers Qwen2 attention,
 // SURVEY.md Appendix C; cosyvoice/llm/llm.py:242-254 forward_one_step).  The attention itself is flash-decoding on
 // warp-level tensor-core MMAs (m16n8k16, bf16 in / fp32 accumulate): the 7 query heads of the group are the M rows of the
-// tile (7 of 16 used - tcgen05's M >= 64 would waste 9/10 of the tile and need TMEM), each of the NW warps walks its own
+// tile (7 of 16 used - wgmma's M >= 64 would waste 9/10 of the tile), each of the NW warps walks its own
 // 16-key blocks with an online softmax held in registers, K and V fragments come straight from the cache with 4-byte loads
 // (V's key pairs are formed with byte permutes, the output dims of a 16-dim block are assigned to the two n-tiles as evens /
 // odds so that each lane ends up with 4 consecutive dims), P never leaves registers (the QK^T accumulator layout is the

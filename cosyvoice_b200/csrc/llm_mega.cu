@@ -3,25 +3,25 @@
 // cooperative kernel instead of 7 PDL-chained kernels per layer.
 //
 // Why: the step is HBM-bound in principle (727.6 MB of bf16 weights per step shared by all rows, SURVEY.md §8d) but the
-// per-op chain was latency-bound: 171 kernels per step, each a launch + a few dependent memory round trips over <= 148 CTAs
-// (977 us per step against a 0.126 ms floor, profiles/r01_ncu_summary.md §C).  Here
+// per-op chain is latency-bound: 171 kernels per step, each a launch + a few dependent memory round trips.  Here
 //   * one CTA per SM stays resident for the whole step; phases are separated by grid-wide barriers (one release-add + one
 //     acquire-polled word in L2) instead of kernel boundaries;
-//   * the weights are re-laid out once into PER-CTA STREAMS: the SWIZZLE_128B operand blocks ([64 or 72 output rows] x [64 K],
-//     8 / 9 KB) a CTA will consume, in the order it consumes them, across phases and layers.  Every projection is cut by OUTPUT
-//     ROWS (and K ranges) so that all 148 CTAs carry about the same bytes per layer (~200 KB) and no unit exceeds the ring;
-//     a dedicated producer warp walks the stream with plain bulk copies into an 18-slot (162 KB) shared-memory ring and never
+//   * the weights are re-laid out once into PER-CTA STREAMS: the SWIZZLE_128B operand blocks ([64 .. 80 output rows] x [64 K],
+//     8 - 10 KB) a CTA will consume, in the order it consumes them, across phases and layers.  Every projection is cut by OUTPUT
+//     ROWS (and K ranges) so that all CTAs carry about the same bytes per layer and no unit exceeds the ring;
+//     a dedicated producer warp walks the stream with plain bulk copies into a shared-memory ring of 10 KB slots and never
 //     waits for a phase boundary, so HBM keeps streaming through the barriers and the latency-bound phases.  At most
 //     MG_INFLIGHT blocks of a CTA are in flight at once: a deeper burst only queues in front of the latency-critical loads
-//     and stores of the same SM (measured: activation loads 1.3-2.9 us, release fences up to 2.8 us behind 160 KB bursts);
-//   * GEMMs are swap-AB tcgen05 (weights = the M side: the MMA reads 128 rows from the slot, rows past the block belong to the
-//     next slot and produce accumulator lanes nobody reads; the <= 64 batch rows = UMMA N) with the fp32 accumulator in TMEM;
-//     activations (the B operand) are gathered with ld.global.cg into the swizzled layout after the barrier;
+//     and stores of the same SM;
+//   * GEMMs are swap-AB wgmma (weights = the M side: two warpgroups read 64 rows each from the slot, rows past the block belong
+//     to the next slot and produce accumulator rows nobody reads; the <= 64 batch rows = wgmma N) with fp32 accumulators in
+//     registers; activations (the B operand) are gathered with ld.global.cg into the swizzled layout after the barrier;
 //   * split-K partial sums go to a small fp32 scratch and are reduced in a fixed order (deterministic, no atomics) by the
 //     attention unit (qkv) or by a per-row reduce + residual + RMSNorm phase (o_proj, down_proj).
 // Phases per layer: qkv GEMM | bias + RoPE + cache append + attention | o GEMM | +res, RMSNorm | gate/up GEMM + SwiGLU |
 // down GEMM | +res, RMSNorm.
 #include "llm_decode_attn.cuh"
+#include "wgmma.cuh"
 #include <algorithm>
 #include <type_traits>
 
@@ -29,13 +29,13 @@ using namespace lm;
 
 namespace {
 
-constexpr int MG_THREADS = 512;          // warp 0: weight producer; warps 1..15: workers (1, 2, 3, 8: MMA issue, 4..7: epilogue)
+constexpr int MG_THREADS = 512;          // warp 0: weight producer; warps 1..15: workers (4..11: the two MMA warpgroups)
 constexpr int MG_WORKERS = MG_THREADS - 32;
 constexpr int MG_NW = MG_WORKERS / 32;   // 15
 constexpr int MG_BK = 64;
-constexpr int MG_MAXROWS = 72;           // output rows of a weight block (multiple of 8)
-constexpr uint32_t MG_SLOT = MG_MAXROWS * 128;   // 9 KB ring slot (a 64-row block uses 8 KB of it)
-constexpr int MG_MAX_STAGES = 18;
+constexpr int MG_MAXROWS = 80;           // output rows of a weight block (multiple of 8)
+constexpr uint32_t MG_SLOT = MG_MAXROWS * 128;   // 10 KB ring slot (a 64-row block uses 8 KB of it)
+constexpr int MG_MAX_STAGES = 16;
 constexpr int MG_INFLIGHT = 3;           // bulk copies of one CTA in flight
 constexpr int MG_KCH = D / MG_BK;        // 14 K chunks of the 896-wide activations
 constexpr int MG_PH = 4;                 // GEMM phases per layer: qkv, o, gate_up, down
@@ -46,7 +46,7 @@ constexpr int MG_TILE = 64;                                          // output r
 constexpr int MG_CPU_QKV = 2, MG_CPU_O = 2;                          // K chunks per unit
 constexpr int MG_SPL_QKV = MG_KCH / MG_CPU_QKV;                      // 7
 constexpr int MG_SPL_O = MG_KCH / MG_CPU_O;                          // 7
-constexpr int MG_SPL_DOWN = 10;                                      // 76 K chunks -> 6 units of 8 + 4 of 7 per row tile
+constexpr int MG_SPL_DOWN = 9;                                       // 76 K chunks -> 4 units of 9 + 5 of 8 per row tile
 
 struct MegaUnit { int row0, nrows, kc0, nblk, split; };
 struct MegaLayerDev { const float* qkv_bias; const float* ln2; const float* next_gamma; };
@@ -102,33 +102,11 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void worker_bar() { asm volatile("bar.sync 1, %0;" ::"n"(MG_WORKERS) : "memory"); }
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
+__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 2, 256;" ::: "memory"); }   // the two MMA warpgroups
 __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -147,22 +125,14 @@ __device__ __forceinline__ long long gtime() {
 template <int BPAD>
 __global__ void __launch_bounds__(MG_THREADS, 1)
 lm_mega_kernel(const MegaParams p) {
-  constexpr int NST = BPAD == 32 ? 18 : 12;
+  constexpr int NST = BPAD == 32 ? 16 : 10;
   constexpr uint32_t ACT_CHUNK = BPAD * 128;     // one 64-wide K chunk of the activations: [BPAD rows][128 B], SWIZZLE_128B
-  constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BPAD >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  constexpr int STG_LD = 40;                     // SwiGLU staging pitch (bf16): 36 channels + pad, rows 8-byte aligned
-  // ONE issuing thread spends ~0.35 us per 64-K block on the instruction stream (mbarrier wait ~0.16 us, 4 MMAs + commit ~0.19 us:
-  // in-kernel stamps) - 5 us for the 14 blocks of the gate|up unit.  The blocks of a unit are dealt round-robin to NACC issuer
-  // warps (1, 2, 3, 8), each with its own TMEM accumulator tile; the epilogue adds the tiles.
-  constexpr int NACC = 4;
-  constexpr uint32_t TMEM_COLS = NACC * BPAD;
+  constexpr int STG_LD = 40;                     // SwiGLU staging pitch (bf16): up to 40 channels, rows 8-byte aligned
   static_assert(decode_attn_smem_floats<MG_NW>() * 4 <= MG_KCH * ACT_CHUNK, "attention scratch must fit the activation buffer");
   static_assert(BPAD * STG_LD * 2 <= MG_KCH * ACT_CHUNK, "SwiGLU staging must fit the activation buffer");
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[MG_MAX_STAGES];
   __shared__ __align__(8) uint64_t bar_empty[MG_MAX_STAGES];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_slot;
   __shared__ float red[16];
   __shared__ MegaUnit s_units[MG_PH];
   __shared__ MegaLayerDev s_layers[MG_MAX_LAYERS];
@@ -179,21 +149,13 @@ lm_mega_kernel(const MegaParams p) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < NST; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per MMA warp (warps 4..11)
     }
-    mbar_init(smem_u32(&bar_acc), NACC);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x >= 64 && threadIdx.x < 64 + MG_PH) s_units[threadIdx.x - 64] = p.units[(threadIdx.x - 64) * G + cta];
   if (threadIdx.x >= 128 && threadIdx.x < 128 + p.num_layers) s_layers[threadIdx.x - 128] = p.layers[threadIdx.x - 128];
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_slot;
 
   if (warp == 0) {
     // ---------------------------------------------------------------------------------------- weight producer
@@ -225,7 +187,6 @@ lm_mega_kernel(const MegaParams p) {
     const int ww = warp - 1;
     unsigned bar_target = __ldcg(p.bar + 1);
     const unsigned gen0 = bar_target;
-    uint32_t acc_par = 0;
     int mma_it = 0, tl_i = 0;
     const bool stamp = p.tl != nullptr && cta == 0 && wt == 0;
     if (stamp) p.tl[tl_i++] = gtime();
@@ -291,96 +252,63 @@ lm_mega_kernel(const MegaParams p) {
         worker_bar();
         FS();
       }
-      if (warp <= 3 || warp == 8) {
-        // MMA issuers: issuer ii takes blocks ii, ii + NACC, ... of the unit into accumulator tile ii
-        const int ii = warp <= 3 ? warp - 1 : 3;
-        if (lane == 0) {
-          long long* ms = (p.tl && cta == 0 && fs_on && ph == 2 && ii == 0) ? p.tl + 1280 : nullptr;     // issuer-0 stamps, gate_up of layer 1
-          int ms_i = 0;
-          if (ms) ms[ms_i++] = gtime();
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t tacc = tmem + (uint32_t)ii * BPAD;
-          for (int j = ii; j < u.nblk; j += NACC) {
-            const int it = mma_it + j;
-            const int s = it % NST;
-            mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(it / NST) & 1u);
-            if (ms) ms[ms_i++] = gtime();
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t da = desc_sw128(ring + s * MG_SLOT), db = desc_sw128(act + j * ACT_CHUNK);
+      if (warp >= 4 && warp < 12) {
+        // warpgroup wg: weight rows [64 wg, 64 wg + 64) of every block of the unit (rows past the block belong to the next slot and
+        // produce accumulator rows nobody reads); both warpgroups walk every block so each stage sees its 8 warp arrivals
+        const int wg = (warp - 4) >> 2, q = lane & 3;
+        const bool active = wg * 64 < u.nrows;
+        float acc[BPAD / 2];
 #pragma unroll
-            for (int k = 0; k < MG_BK / 16; ++k) umma(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), IDESC, (j >= NACC || k > 0) ? 1u : 0u);
-            umma_commit(smem_u32(&bar_empty[s]));
-            if (ms) ms[ms_i++] = gtime();
+        for (int e = 0; e < BPAD / 2; ++e) acc[e] = 0.f;
+        for (int j = 0; j < u.nblk; ++j) {
+          const int it = mma_it + j;
+          const int s = it % NST;
+          mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(it / NST) & 1u);
+          if (active) {
+            const uint64_t da = wg_desc_sw128(ring + s * MG_SLOT + (uint32_t)wg * 8192u), db = wg_desc_sw128(act + j * ACT_CHUNK);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < MG_BK / 16; ++k) wgmma_ss<BPAD, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+            wg_commit();
+            wg_wait<0>();
           }
-          if (ii < u.nblk) umma_commit(smem_u32(&bar_acc));
-          else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&bar_acc)) : "memory");   // no block for this issuer
-          if (ms) ms[ms_i++] = gtime();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(&bar_empty[s]));
         }
-        __syncwarp();
-      }
-      if (warp >= 4 && warp < 8) {
-        const int q = warp & 3;
-        const int r = q * 32 + lane;               // accumulator lane = row of the unit
-        const int n = u.row0 + r;
-        const bool warp_has_rows = q * 32 < u.nrows;
+        wg_touch<BPAD / 2>(acc);
         bf16* stage = reinterpret_cast<bf16*>(act_ptr);
-        long long* es = (p.tl && cta == 0 && fs_on && ph == 2 && threadIdx.x == 128) ? p.tl + 1400 : nullptr;
-        int es_i = 0;
-        if (es) es[es_i++] = gtime();
-        if (warp_has_rows) {
-          mbar_wait(smem_u32(&bar_acc), acc_par);
-          if (es) es[es_i++] = gtime();
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-          for (int c = 0; c < BPAD; c += 16) {
-            float acc[16];
-            tmem_ld16(trow + (uint32_t)c, acc);
+        if (mode == 1) epi_bar();     // both warpgroups' MMAs have read the activations the staging tile aliases
+        if (active) {
+          // acc[e]: unit row r = 64 wg + 16 (warp & 3) + lane / 4 + 8 ((e >> 1) & 1), batch row b = 8 (e >> 2) + 2 q + (e & 1)
 #pragma unroll
-            for (int a = 1; a < NACC; ++a) {
-              if (a < u.nblk) {                   // tiles of issuers without a block were never written
-                float t2[16];
-                tmem_ld16(trow + (uint32_t)(a * BPAD + c), t2);
-#pragma unroll
-                for (int e = 0; e < 16; ++e) acc[e] += t2[e];
-              }
-            }
+          for (int e = 0; e < BPAD / 2; ++e) {
+            const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * ((e >> 1) & 1);
+            const int b = 8 * (e >> 2) + 2 * q + (e & 1);
             if (mode == 1) {
-              // rows of W are interleaved (2i = gate_i, 2i+1 = up_i): lanes pair up, the even lane forms silu(g) * u (Qwen2 MLP
-              // act_fn(gate_proj(x)) * up_proj(x)) for channel (row0 + r) / 2 and parks it in the staging tile [b][channel]
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                const float other = __shfl_xor_sync(0xffffffffu, acc[e], 1);
-                const int b = c + e;
-                if (!(lane & 1) && r < u.nrows && b < B) {
-                  const float g = acc[e];
-                  stage[b * STG_LD + (r >> 1)] = __float2bfloat16_rn(__fdividef(g, 1.f + fast_exp(-g)) * other);
-                }
+              // rows of W are interleaved (2i = gate_i, 2i+1 = up_i): rows r and r + 1 sit in lanes l and l + 4, the even one forms
+              // silu(g) * u (Qwen2 MLP act_fn(gate_proj(x)) * up_proj(x)) for channel (row0 + r) / 2 and parks it in the staging
+              // tile [b][channel]
+              const float other = __shfl_xor_sync(0xffffffffu, acc[e], 4);
+              if (!((lane >> 2) & 1) && r < u.nrows && b < B) {
+                const float g = acc[e];
+                stage[b * STG_LD + (r >> 1)] = __float2bfloat16_rn(__fdividef(g, 1.f + fast_exp(-g)) * other);
               }
-            } else if (r < u.nrows) {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                const int b = c + e;
-                if (b < B) out_f32[((size_t)u.split * B + b) * N + n] = acc[e];
-              }
+            } else if (r < u.nrows && b < B) {
+              out_f32[((size_t)u.split * B + b) * N + u.row0 + r] = acc[e];
             }
           }
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          if (es) es[es_i++] = gtime();
         }
         if (mode == 1) {
-          // staging tile -> ffa[b][row0/2 .. + nrows/2) with 8-byte stores (each row's run is 64 or 72 bytes, 8-byte aligned)
+          // staging tile -> ffa[b][row0/2 .. + nrows/2) with 8-byte stores (each row's run is a multiple of 8 bytes, 8-byte aligned)
           epi_bar();
           const int nq = u.nrows >> 3;               // 8-byte chunks per row (4 channels each)
           const int ch0 = u.row0 >> 1;
-          for (int i = threadIdx.x - 128; i < B * nq; i += 128) {
+          for (int i = threadIdx.x - 128; i < B * nq; i += 256) {
             const int b = i / nq, c4 = i % nq;
             *reinterpret_cast<uint2*>(p.ffa + (size_t)b * DFF + ch0 + c4 * 4) = *reinterpret_cast<const uint2*>(stage + b * STG_LD + c4 * 4);
           }
-          if (es) es[es_i++] = gtime();
         }
       }
-      acc_par ^= 1u;
       mma_it += u.nblk;
     };
 
@@ -473,11 +401,6 @@ lm_mega_kernel(const MegaParams p) {
       if (stamp) p.tl[tl_i++] = gtime();
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 // one weight block: rows [row0, row0 + nrows) x K chunk kc of W [N][K] bf16 row-major -> the shared-memory image of a K-major
@@ -494,7 +417,7 @@ __global__ void pack_blocks_kernel(const PackDesc* __restrict__ descs, int n, ui
   }
 }
 
-template <int BPAD> constexpr size_t mega_smem() { return (size_t)(BPAD == 32 ? 18 : 12) * MG_SLOT + (size_t)MG_KCH * BPAD * 128 + 1024; }
+template <int BPAD> constexpr size_t mega_smem() { return (size_t)(BPAD == 32 ? 16 : 10) * MG_SLOT + (size_t)MG_KCH * BPAD * 128 + 1024; }
 
 }  // namespace
 
@@ -585,7 +508,7 @@ void lm_mega_build(cvk_ctx* ctx, LlmModel* m) {
     PackDesc* dd = nullptr;
     CVK_CHECK_CUDA(cudaMalloc((void**)&dd, descs.size() * sizeof(PackDesc)));
     CVK_CHECK_CUDA(cudaMemcpy(dd, descs.data(), descs.size() * sizeof(PackDesc), cudaMemcpyHostToDevice));
-    pack_blocks_kernel<<<148 * 8, 256>>>(dd, (int)descs.size(), mg->wstream);
+    pack_blocks_kernel<<<G * 8, 256>>>(dd, (int)descs.size(), mg->wstream);
     CVK_LAUNCH_CHECK();
     CVK_CHECK_CUDA(cudaDeviceSynchronize());
     cudaFree(dd);

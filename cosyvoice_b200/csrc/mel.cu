@@ -146,7 +146,7 @@ void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int
     conv_gemm_simt(ctx, st, x, g_mel->dft, e);
   }
   Mat mag = arena_mat(ctx, DT_F32, sr.R, N_BINS, BINS_LD);
-  magnitude_kernel<<<148 * 4, 256, 0, st>>>(spec.f32(), spec.ld, sr.R, mag.f32(), mag.ld);
+  magnitude_kernel<<<132 * 4, 256, 0, st>>>(spec.f32(), spec.ld, sr.R, mag.f32(), mag.ld);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   Mat out = arena_mat(ctx, DT_F32, sr.R, N_MEL, N_MEL);
@@ -156,7 +156,7 @@ void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int
     CVK_REQUIRE(fmax_hz == 8000 || fmax_hz == 0 || fmax_hz == SR / 2, "mel_spectrogram: fmax must be 8000 or sr/2 (0 = null)");
     conv_gemm_simt(ctx, st, mag, fmax_hz == 8000 ? g_mel->mel : g_mel->mel_nyq, e);
   }
-  log_clamp_kernel<<<148, 256, 0, st>>>(out.f32(), (size_t)sr.R * N_MEL);
+  log_clamp_kernel<<<132, 256, 0, st>>>(out.f32(), (size_t)sr.R * N_MEL);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   unpack_rows(ctx, st, out, sf, 0, mel, N_MEL);

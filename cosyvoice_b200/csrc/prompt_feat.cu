@@ -228,7 +228,7 @@ Mat features(cvk_ctx* ctx, cudaStream_t st, const float* wav, const int* lens, c
     conv_gemm_simt(ctx, st, x, dft, e);
   }
   Mat pw = arena_mat(ctx, DT_F32, sr.R, bins, round_up(bins, 8));
-  power_kernel<<<148 * 4, 256, 0, st>>>(spec.f32(), spec.ld, sr.R, bins, pw.f32(), pw.ld);
+  power_kernel<<<132 * 4, 256, 0, st>>>(spec.f32(), spec.ld, sr.R, bins, pw.f32(), pw.ld);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   Mat out = arena_mat(ctx, DT_F32, sr.R, n_mel, n_mel);

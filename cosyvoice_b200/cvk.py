@@ -39,7 +39,7 @@ SIGNATURES = {
     "cvk_op_conv1d": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, ctypes.c_int,
                                      ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_op_linear_small": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
-                                           ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_longlong), _vp]),
+                                           ctypes.POINTER(ctypes.c_float), _vp]),
     "cvk_op_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_hift_f0": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_hift_source": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _vp]),
@@ -127,7 +127,7 @@ class Context:
 
     def __init__(self, device=0, precision="bf16", workspace_gb=4.0):
         if not torch.cuda.is_available():
-            raise RuntimeError("cosyvoice_b200 requires a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("cosyvoice_b200 requires a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = load_library()
         self.device = torch.device("cuda", device)
         self.precision = PREC_BF16 if precision in ("bf16", PREC_BF16) else PREC_FP32
@@ -136,7 +136,7 @@ class Context:
         torch.zeros(1, device=self.device)           # make sure the primary context exists
         rc = self.lib.cvk_create(device, self.precision, int(workspace_gb * (1 << 30)), ctypes.byref(h))
         if rc != 0:
-            raise CvkError(f"cvk_create failed with status {rc} (needs an sm_100 GPU)")
+            raise CvkError(f"cvk_create failed with status {rc} (needs an sm_90 GPU: H100)")
         self.h = h
         self.lock = threading.Lock()
 
@@ -186,7 +186,7 @@ class Context:
         self._check(self.lib.cvk_profile_read(self.h, family, ctypes.byref(ms), ctypes.byref(fl), ctypes.byref(by), ctypes.byref(n)))
         return dict(ms=ms.value, flops=fl.value, bytes=by.value, launches=n.value)
 
-    def debug_read(self, n=1024):
+    def debug_read(self, n=4096):
         buf = (ctypes.c_longlong * n)()
         self._check(self.lib.cvk_debug_read(self.h, buf, n))
         return list(buf)
@@ -209,15 +209,14 @@ class Context:
                                            ACT[act], _ptr(out), _stream()))
         return out
 
-    def linear_small(self, x, w, bias=None, iters=0, timeline=False):
+    def linear_small(self, x, w, bias=None, iters=0):
         x, w = _f32(x, self.device), _f32(w, self.device)
         b = _f32(bias, self.device) if bias is not None else None
         out = torch.empty(x.shape[0], w.shape[0], device=self.device)
         ms = ctypes.c_float(0)
-        tl = (ctypes.c_longlong * 1024)() if timeline else None
         self._check(self.lib.cvk_op_linear_small(self.h, _ptr(x), x.shape[0], x.shape[1], _ptr(w), _ptr(b), w.shape[0], _ptr(out), iters,
-                                                 ctypes.byref(ms), tl, _stream()))
-        return out, ms.value, (list(tl) if timeline else None)
+                                                 ctypes.byref(ms), _stream()))
+        return out, ms.value
 
     def attention(self, q, k, v, lens, heads, chunk=0, scale=0.125):
         q, k, v = (_f32(t, self.device) for t in (q, k, v))

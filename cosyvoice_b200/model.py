@@ -5,7 +5,7 @@ of ``cosyvoice.cli.model.CosyVoice2Model`` (cosyvoice/cli/model.py:245-394) so i
 ``cosyvoice.cli.cosyvoice.CosyVoice2`` (``cosyvoice.model = B200CosyVoice2Model(...)``, see INTEGRATION.md), plus
 ``tts_batch`` for the batch-32 metric (the reference has no batched API; its batch is a Python loop).
 
-All arithmetic happens in libcvk (hand-written sm_100a kernels); torch provides device memory, streams and the two
+All arithmetic happens in libcvk (hand-written sm_90a kernels); torch provides device memory, streams and the two
 random streams the reference draws from the global RNG (sampling uniforms, SineGen noise).  No CPU fallback.
 """
 import threading

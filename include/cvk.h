@@ -1,4 +1,4 @@
-/* libcvk - C ABI of the B200-native CosyVoice2 hot path (LM decode -> CFM flow -> HiFT vocoder + mel frontend).
+/* libcvk - C ABI of the H100-native CosyVoice2 hot path (LM decode -> CFM flow -> HiFT vocoder + mel frontend).
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  The reference is pure Python, so there is no FFI to
  * mirror symbol-for-symbol; each entry point replaces one of the engine plug-in granularities the reference itself
@@ -46,7 +46,7 @@ typedef enum {
 
 /* arithmetic of the tensor-core stages */
 #define CVK_PREC_FP32 0 /* everything fp32 on CUDA cores: parity mode, tracks the CPU reference to ~1e-4 */
-#define CVK_PREC_BF16 1 /* dense GEMM / conv operands bf16 on tcgen05 tensor cores, fp32 accumulate + residuals */
+#define CVK_PREC_BF16 1 /* dense GEMM / conv operands bf16 on wgmma tensor cores, fp32 accumulate + residuals */
 
 /* ---------------------------------------------------------------------------------------------- context */
 int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out);
@@ -57,19 +57,19 @@ const char* cvk_version(void);
 int64_t cvk_launch_count(cvk_ctx* ctx);
 /* mean device time (ms) of the kernel timed by the last cvk_op_* call when the "op_iters" option is > 0 (tools/gemm_probe.py) */
 double cvk_last_op_ms(cvk_ctx* ctx);
-/* debug: copy (and clear) the device timeline buffer filled by instrumented kernels when "debug_timeline" is on */
+/* debug: copy the LM decode-chain timeline (4 int64 slots per launch, n must be 4096) recorded while "chain_timeline" is on */
 int cvk_debug_read(cvk_ctx* ctx, long long* out, int n);
 /* workspace arena of the context (SURVEY.md §8b `cvk_workspace_bytes`): capacity given to cvk_create and the high-water mark of
  * the calls made so far - what a caller needs to size cvk_create for its largest batch. */
 int cvk_workspace_bytes(cvk_ctx* ctx, size_t* capacity, size_t* high_water);
 /* Test / measurement switches, NOT part of the drop-in surface (every default is the benchmarked configuration): kernel-variant
- * A/B ("use_tc", "tc_persist", "tc_bn256", "tc_pbn256", "tc_epi", "use_tc_attn", "attn_single_pass", "enc_tc_attn", "use_skinny",
+ * A/B ("use_tc", "tc_persist", "tc_epi", "use_tc_attn", "enc_tc_attn", "use_skinny",
  * "lm_fused", "lm_mega", "mega_coop", "pdl", "use_graph", "hift_f16" - the last one takes effect at the next cvk_finalize("hift")),
- * probes ("op_iters", "op_out_bf16", "debug_timeline", "chain_timeline").  Unknown keys return CVK_ERR_INVALID. */
+ * probes ("op_iters", "op_out_bf16", "chain_timeline").  Unknown keys return CVK_ERR_INVALID. */
 int cvk_set_option(cvk_ctx* ctx, const char* key, int value);
 
 /* Per-kernel-family device timing for the roofline report of bench.py: CUDA events are recorded around every launch
- * of a family while enabled (family 0 = tcgen05 conv-GEMM, 1 = CUDA-core conv-GEMM, 2 = attention).  Launches inside
+ * of a family while enabled (family 0 = wgmma conv-GEMM, 1 = CUDA-core conv-GEMM, 2 = attention).  Launches inside
  * the captured LM decode graph are not instrumented.  cvk_profile_read sums elapsed ms, algorithmic FLOPs and bytes. */
 int cvk_profile(cvk_ctx* ctx, int enable);
 int cvk_profile_read(cvk_ctx* ctx, int family, double* ms, double* flops, double* bytes, int64_t* launches);
@@ -90,10 +90,9 @@ int cvk_finalize(cvk_ctx* ctx, const char* stage, const int* cfg, int ncfg);
 int cvk_op_conv1d(cvk_ctx* ctx, const float* x, const int* lens_host, int B, int K, const float* w, const float* bias,
                   int N, int taps, int dil, int shift0, int act, float* out, void* stream);
 /* out[b,n] = bias[n] + sum_k x[b,k] w[n,k] through the LM decode weight-streaming kernel (bf16 context, rows <= 64);
- * runs it `iters` more times and reports the mean device time; timeline_host (optional, 128 int64) receives the clock64
- * stamps of CTA 0 when the "debug_timeline" option is on. */
+ * runs it `iters` more times and reports the mean device time. */
 int cvk_op_linear_small(cvk_ctx* ctx, const float* x, int rows, int K, const float* w, const float* bias, int N, float* out, int iters,
-                        float* ms_out, long long* timeline_host, void* stream);
+                        float* ms_out, void* stream);
 /* block-causal / full multi-head attention over ragged sequences; q,k,v,out [sum(lens), H*64] */
 int cvk_op_attention(cvk_ctx* ctx, const float* q, const float* k, const float* v, const int* lens_host, int B, int H,
                      int chunk, float scale, float* out, void* stream);

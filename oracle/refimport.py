@@ -1,7 +1,6 @@
-"""Import shims for running the UNMODIFIED reference under /root/reference on CPU.
+"""Import shims for running the UNMODIFIED reference (a CosyVoice checkout, located by $COSYVOICE_REF_ROOT) on CPU.
 
-Used only by ``oracle/make_golden.py`` and by ``tests`` marked ``needs_reference``
-(skipped on the GPU box where /root/reference does not exist).
+Used only by ``oracle/make_golden.py`` to regenerate ``tests/golden/``; no test imports the reference.
 
 The reference imports, at module import time, packages that are absent from this
 image (SURVEY.md §8c): onnxruntime, omegaconf, conformer, diffusers, and

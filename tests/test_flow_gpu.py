@@ -2,7 +2,7 @@
 of the reference (tests/golden/flow_*.npz) and the oracle (oracle/flow.py).
 
 Tolerances: fp32 mode follows the reference's own export check (cosyvoice/bin/export_onnx.py:99-110,
-rtol 1e-2 / atol 1e-4 on the estimator); bf16 mode (tcgen05 operands, fp32 accumulate and residual stream) is held
+rtol 1e-2 / atol 1e-4 on the estimator); bf16 mode (tensor-core operands, fp32 accumulate and residual stream) is held
 to the measured bounds stated next to each assert."""
 import numpy as np
 import pytest
@@ -106,7 +106,7 @@ def test_ragged_batch_vs_oracle(precision):
 
 
 def test_persistent_gemm_flow_bit_identical():
-    """A batch large enough for the persistent tcgen05 GEMM path (tiles > SMs; bf16 and fp32 outputs, second outputs, residual /
+    """A batch large enough for the persistent wgmma GEMM path (tiles > SMs; bf16 and fp32 outputs, second outputs, residual /
     per-sequence-vector epilogues): the whole flow is bit-identical with the path switched off."""
     c, sd, cfg = model("bf16", "small")
     g = torch.Generator().manual_seed(31)
@@ -131,7 +131,7 @@ def test_persistent_gemm_flow_bit_identical():
 
 @pytest.mark.parametrize("tag", ["small", "full"])
 def test_encoder_relpos_attention_tensor_core_vs_cuda_core(tag):
-    """the conformer relative-position attention on the tcgen05 kernels (position scores by relpos_u_kernel, added as a bias inside the
+    """the conformer relative-position attention on the wgmma kernels (position scores by relpos_u_kernel, added as a bias inside the
     one-pass attention kernel) against the CUDA-core flash kernel it replaces (same bf16 operands, fp32 math): ragged batch, offline
     and with the streaming chunk masks + look-ahead context.  Output = after_norm rows, unit scale."""
     c, sd, cfg = model("bf16", tag)

@@ -1,11 +1,12 @@
-"""CPU: the algebra behind four kernels of round 2, restated in numpy / torch exactly as the CUDA code computes it and checked against
+"""CPU: the algebra behind four kernels, restated in numpy / torch exactly as the CUDA code computes it and checked against
 the reference-side formulation (the kernels themselves are checked on the GPU; these tests keep the derivations honest in the
 no-GPU suite):
 
  * prompt_feat.cu: kaldi fbank with DC removal + pre-emphasis + povey window + zero-padded DFT folded into ONE constant matrix applied to
    three rows of 160 samples; whisper framing as three rows of the reflect-padded signal;
  * attention_tc.cu (relpos_u_kernel + BIAS): the conformer's rel_shift as the index map U[i][center - i + j];
- * attention_tc.cu (attn_tc1_kernel): two per-thread lazy running maxima with separate accumulators, merged at the end, == softmax(S) V;
+ * attention_tc.cu (attn_wg_kernel): the register-resident online softmax - the four lanes of a quad own interleaved key columns,
+   share one running maximum per row through quad shuffles, keep partial row sums merged at the end - == softmax(S) V;
  * flow.cu (streaming sessions): a causal convolution over [saved two-row tail | chunk] == the chunk's rows of the convolution over the
    whole sequence."""
 import math
@@ -77,44 +78,43 @@ def test_rel_shift_is_the_index_map_center_minus_i_plus_j():
     center = T - 1
     i = torch.arange(T)[:, None]
     j = torch.arange(T)[None, :]
-    bias = U[0][:, i, center - i + j]                                          # attn_tc1_kernel<BIAS>: ubias[.. + center - i + j]
+    bias = U[0][:, i, center - i + j]                                          # attn_wg_kernel<BIAS>: ubias[.. + center - i + j]
     assert torch.equal(bias, bd[0])
 
 
-def test_two_lazy_maxima_with_separate_accumulators_equal_softmax():
-    """attn_tc1_kernel: thread A owns keys [0,32) of every 64-key half tile, thread B keys [32,64); each keeps a stale maximum while the
-    tile maximum exceeds it by <= 8 (log2 units), rescales its own accumulator otherwise; merge = flash-decoding"""
+def test_quad_online_softmax_equals_softmax():
+    """attn_wg_kernel: per 64-key tile, quad lane q holds the scores of keys 8 jj + 2 q + e (jj < 8, e < 2) of its row; the row maximum
+    is the quad maximum of the lane maxima (log2 units), the accumulator and the per-lane sums are rescaled by 2^(m_old - m_new) when
+    the maximum grows, keys past the row's limit are -inf (P = 0), and the row sum is the quad sum of the lane sums at the end"""
     g = torch.Generator().manual_seed(1)
-    L, d, scale = 300, 16, 0.125 * math.log2(math.e)
-    for trial in range(3):
-        s = torch.randn(L, generator=g, dtype=torch.float64) * 3.0 + torch.arange(L, dtype=torch.float64) * (1.0 * trial)   # a rising trend forces rescales
+    d, scale = 16, 0.125 * math.log2(math.e)
+    rescales = 0
+    for trial, (L, klim) in enumerate(((300, 300), (300, 250), (64, 1), (130, 100))):
+        s = torch.randn(L, generator=g, dtype=torch.float64) * 3.0 + torch.arange(L, dtype=torch.float64) * (0.5 * trial)   # a rising trend forces rescales
         V = torch.randn(L, d, generator=g, dtype=torch.float64)
-        ref = torch.softmax(s * 0.125, 0) @ V
-        m = [-math.inf, -math.inf]
-        l = [0.0, 0.0]
-        O = [torch.zeros(d, dtype=torch.float64), torch.zeros(d, dtype=torch.float64)]
-        rescales = 0
+        ref = torch.softmax(s[:klim] * 0.125, 0) @ V[:klim]
+        m = -math.inf
+        lane_sum = [0.0] * 4
+        O = torch.zeros(d, dtype=torch.float64)
         for j0 in range(0, L, 64):
-            for half in (0, 1):
-                lo, hi = j0 + 32 * half, min(j0 + 32 * half + 32, L)
-                if lo >= hi:
-                    continue
-                x = s[lo:hi] * scale
-                tm = x.max().item()
-                if tm > m[half] + 8.0:
-                    if m[half] != -math.inf:
-                        f = 2.0 ** (m[half] - tm)
-                        l[half] *= f
-                        O[half] *= f
-                        rescales += 1
-                    m[half] = tm
-                p = torch.exp2(x - m[half])
-                assert p.max().item() <= 256.0 + 1e-9                               # the lazy bound the kernel relies on
-                l[half] += p.sum().item()
-                O[half] += p @ V[lo:hi]
-        mm = max(m)
-        wA, wB = 2.0 ** (m[0] - mm), 2.0 ** (m[1] - mm)
-        out = (wA * O[0] + wB * O[1]) / (wA * l[0] + wB * l[1])
+            cols = [[j0 + 8 * jj + 2 * q + e for jj in range(8) for e in range(2)] for q in range(4)]
+            x = [[(s[j].item() if j < klim else -math.inf) for j in cols[q] if j < L] for q in range(4)]
+            mt = max(max(xs, default=-math.inf) for xs in x) * scale                  # quad_max of the lane maxima
+            mn = max(m, mt)
+            f = 1.0 if m == -math.inf else 2.0 ** (m - mn)
+            if f != 1.0:
+                rescales += 1
+            m = mn
+            mneg = 0.0 if mn == -math.inf else -mn
+            O *= f
+            for q in range(4):
+                lane_sum[q] *= f
+                for j, xv in zip(cols[q], x[q]):
+                    p = 0.0 if xv == -math.inf else 2.0 ** (xv * scale + mneg)
+                    lane_sum[q] += p
+                    O += p * V[j]
+        den = sum(lane_sum)                                                             # quad_sum at the end
+        out = O / den
         assert (out - ref).abs().max() < 1e-12
     assert rescales > 0
 

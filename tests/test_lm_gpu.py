@@ -149,7 +149,7 @@ def test_decode_bf16_runs_and_first_token_matches(golden):
 
 
 def test_decode_weight_streaming_gemm_vs_tiled_bf16():
-    """bf16 decode: the split-K weight-streaming GEMM and the tiled tcgen05 GEMM see the same operands (both runs on the
+    """bf16 decode: the split-K weight-streaming GEMM and the tiled wgmma GEMM see the same operands (both runs on the
     one-kernel-per-op attention path); the sampled ids agree until fp32 summation-order noise meets a near-tie (the first
     tokens are required to agree)."""
     c, sd = model("bf16", 2)
@@ -197,7 +197,7 @@ def test_decode_attention_logits_fused_vs_unfused_bf16(n_prompt):
     decode step (the first token is the arg-max of the prefill distribution on every path; the second distribution is a function
     of every layer's decode attention over the n_prompt + few keys in the cache) are compared with the fp32 context (CUDA-core
     kernels, fp32 everything): the fused bf16 path (bf16 P on mma.sync) must be as close to fp32 as the one-kernel-per-op bf16
-    path (fp32-math attention) is - bf16 rounding noise through 24 layers, measured 0.1-0.2 on |logp| <= 25 for both, while one
+    path (fp32-math attention) is - bf16 rounding noise through 24 layers for both, while one
     misplaced fragment element moves the fused path by O(1).  Rows of a batch of 3 have different context lengths."""
     cb, _ = model("bf16", 24)
     cf, _ = model("fp32", 24)

@@ -59,7 +59,7 @@ def test_tts_matches_reference_model(stream, golden):
     wav = torch.cat(chunks, 1)
     ref = torch.from_numpy(g[key + "_wav"])
     # The excitation phase is 2*pi*480*cumsum(f0/sr), so fp32 summation-order differences in the f0 predictor grow along the
-    # utterance (DESIGN.md §4): tight bound on the first second, looser on the rest (measured: 2e-4 / 5e-4 over 5.6 s).
+    # utterance (DESIGN.md §4): tight bound on the first second, looser on the rest.
     d_head = maxdiff(wav[:, :24000], ref[:, :24000])
     rel = ((wav - ref).norm() / ref.norm()).item()
     print(f"[{key}] max|d| first second {d_head:.3g}, relative L2 over {wav.shape[1]} samples {rel:.3g}, max|d| {maxdiff(wav, ref):.3g}")

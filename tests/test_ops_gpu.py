@@ -1,4 +1,4 @@
-"""GPU: per-op parity of the conv-GEMM kernels (fp32 CUDA-core and bf16 tcgen05/TMA) and the attention kernel
+"""GPU: per-op parity of the conv-GEMM kernels (fp32 CUDA-core and bf16 wgmma/TMA) and the attention kernel
 against plain torch fp32 on the CPU, through the C ABI."""
 import pytest
 import torch
@@ -58,7 +58,7 @@ def test_conv_gemm(precision, case):
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 def test_conv_gemm_tc_matches_simt_on_same_operands(precision):
-    """bf16 mode: the tcgen05 kernel and the CUDA-core kernel fed the same bf16 operands agree to fp32 rounding."""
+    """bf16 mode: the wgmma kernel and the CUDA-core kernel fed the same bf16 operands agree to fp32 rounding."""
     if precision == "fp32":
         pytest.skip("single path")
     c = ctx("bf16")
@@ -104,7 +104,7 @@ def test_attention(precision, chunk):
 
 @pytest.mark.parametrize("chunk", [0, 50])
 def test_attention_tcgen05_long_ragged(chunk):
-    """bf16 mode runs the tcgen05 attention kernel: multi-tile sequences, ragged lengths, block-causal mask."""
+    """bf16 mode runs the wgmma attention kernel: multi-tile sequences, ragged lengths, block-causal mask."""
     g = torch.Generator().manual_seed(13)
     lens, H = [650, 129, 300, 7], 8
     q, k, v = (torch.randn(sum(lens), H * 64, generator=g) for _ in range(3))
@@ -125,8 +125,8 @@ def test_attention_tcgen05_long_ragged(chunk):
 @pytest.mark.parametrize("case", [(256, 384, 3, -2, "mish"), (256, 1024, 1, 0, "gelu"), (1024, 256, 1, 0, "none")],
                          ids=["K256N384t3", "K256N1024", "K1024N256"])
 def test_conv_gemm_persistent_tiles(case):
-    """More output tiles than SMs: the persistent tcgen05 kernel (double-buffered TMEM accumulators, operand ring running
-    across tile boundaries) == the one-tile-per-CTA kernel bit for bit, and == torch fp32 to bf16 operand rounding."""
+    """More output tiles than SMs: the persistent wgmma kernel (one CTA per SM, operand ring running across tile boundaries)
+    == the one-tile-per-CTA launch bit for bit, and == torch fp32 to bf16 operand rounding."""
     K, N, taps, shift0, act = case
     g = torch.Generator().manual_seed(K + N)
     lens = [5000, 3333, 4100, 129]                      # ~99 row tiles x 2-8 column tiles, ragged tails

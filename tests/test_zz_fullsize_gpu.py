@@ -24,6 +24,17 @@ def bctx():
     return _c["c"]
 
 
+@pytest.fixture(scope="module", autouse=True)
+def _release_fullsize_context():
+    """The full-size models, their workspace and the batch-32 decode sessions occupy a large share of an 80 GB card: give the
+    memory back before the next module's models are built."""
+    yield
+    c = _c.pop("c", None)
+    if c is not None:
+        c.close()
+    torch.cuda.empty_cache()
+
+
 def test_lm_teacher_forced_logp_fullsize(golden):
     g = golden("z10_full")
     c = bctx()
@@ -43,8 +54,8 @@ def test_lm_teacher_forced_logp_fullsize(golden):
         overlap.append(len(a & b))
     am = int((got.argmax(-1) == ref.argmax(-1)).sum())
     print(f"[full-size LM, bf16] max |dlogp| {d:.4g} on |logp| <= {ref.abs().max().item():.3g}; top-25 overlap per row {overlap}; arg-max equal {am}/{ref.shape[0]}")
-    assert d < 0.35, d                    # measured 0.24 on |logp| <= 32.7
-    assert min(overlap) >= 22, overlap    # measured 24-25 of 25
+    assert d < 0.35, d                    # H100 (700 W limit): 0.21 on |logp| <= 32.7
+    assert min(overlap) >= 22, overlap    # H100 (700 W limit): 24-25 of 25
 
 
 def test_lm_persistent_decode_vs_per_op_chain_batch32():
@@ -110,7 +121,7 @@ def test_flow_mel_fullsize(golden):
     dd = (mel.cpu() - ref).abs()
     print(f"[full-size flow, bf16] mel max |d| {dd.max().item():.4g}, mean |d| {dd.mean().item():.4g} on |mel| <= {ref.abs().max().item():.3g}; "
           f"yardstick (oracle under torch CPU bf16 autocast vs fp32): max {float(g['mel_autocast_bf16_max']):.4g}, mean {float(g['mel_autocast_bf16_mean']):.4g}")
-    # measured on B200: max 0.035, mean 0.0073 - the same as torch's own bf16 autocast shows against fp32 on this model (0.041 / 0.0077)
+    # torch's own bf16 autocast shows max 0.041, mean 0.0077 against fp32 on this model
     assert dd.max().item() < 0.08 and dd.mean().item() < 0.015, (dd.max().item(), dd.mean().item())
 
 
@@ -127,6 +138,6 @@ def test_hift_wav_fullsize(golden):
     d = (wav - ref).abs()
     snr = 10 * torch.log10(ref.pow(2).sum() / (wav - ref).pow(2).sum()).item()
     print(f"[full-size vocoder, ctx precision bf16] wav max |d| {d.max().item():.4g}, rms {d.pow(2).mean().sqrt().item():.4g} on |wav| <= {ref.abs().max().item():.3g}; SNR {snr:.1f} dB")
-    # IEEE-half operands (10-bit mantissa, the class of the reference's default TF32 convolutions): measured 1.0e-3 / 54 dB SNR on B200;
+    # IEEE-half operands (10-bit mantissa, the class of the reference's default TF32 convolutions): the tolerance below is what that operand class allows;
     # SURVEY.md §8(c)(ii) asks for <= 2e-3 with the source injected
     assert d.max().item() < 2e-3 and snr > 48.0, (d.max().item(), snr)

@@ -1,8 +1,7 @@
 """GPU: CosyVoice3 causal vocoder (SURVEY.md §8 row a16) through the C ABI against the committed outputs of the reference
 CausalHiFTGenerator (tests/golden/hift_causal.npz, made by oracle/make_golden.py::gen_hift_causal).
 
-First GPU run: round-1 driver test pass (green, GPUTEST_r01.json); the first-run xfail marker was removed in round 2.  The
-file name still sorts last so that a CUDA fault here cannot disturb the tests that share the process."""
+The file name sorts last so that a CUDA fault here cannot disturb the tests that share the process."""
 import numpy as np
 import pytest
 import torch

@@ -6,7 +6,7 @@ from cosyvoice_b200 import synth
 from cosyvoice_b200.model import B200CosyVoice2Model, cfm_rand_noise
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--opt", default="attn_single_pass")
+ap.add_argument("--opt", default="enc_tc_attn")
 ap.add_argument("--values", default="0,1")
 ap.add_argument("--reps", type=int, default=3)
 ap.add_argument("--batch", type=int, default=32)

@@ -1,5 +1,5 @@
-"""Times the tcgen05 conv-GEMM on the estimator / HiFT shapes: one-tile-per-CTA kernel vs the persistent kernel (8 / 16 epilogue
-warps), fp32 and bf16 outputs.  CUDA events around `op_iters` back-to-back launches inside cvk_op_conv1d."""
+"""Times the wgmma conv-GEMM on the estimator / HiFT shapes: one CTA per tile vs persistent CTAs (one per SM),
+bf16 outputs.  CUDA events around `op_iters` back-to-back launches inside cvk_op_conv1d."""
 import os, sys, itertools
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

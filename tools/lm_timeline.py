@@ -17,8 +17,6 @@ m = B200CosyVoice2Model(precision="bf16", device=0, workspace_gb=8.0)
 m.load_state_dicts(*sds)
 m.ctx.set_option("pdl", a.pdl)
 m.ctx.set_option("chain_timeline", 1)
-if os.environ.get("CVK_AF_PHASES"):
-    m.ctx.set_option("debug_timeline", 1)
 m.min_token_text_ratio = m.max_token_text_ratio = a.steps / 50.0
 inputs = synth.batch32_zero_shot(32)
 ids = m.lm_generate([i["text"] for i in inputs], [i["prompt_text"] for i in inputs], [i["llm_prompt_speech_token"] for i in inputs])
@@ -45,6 +43,3 @@ for k, v in agg.items():
     n = len(v)
     print(f"  {k:12s} n={n:3d} body {sum(x[0] for x in v) / n:6.2f}  period {sum(x[1] for x in v) / n:6.2f}  early {sum(x[2] for x in v) / n:6.2f}")
 print(f"step total (first waited -> last end): {(rows[-1][3] - rows[0][2]) / 1e3:.1f} us")
-if os.environ.get("CVK_AF_PHASES"):
-    ph = m.ctx.debug_read(1024)[1000:]
-    print("attn_fused phases (us since waited): " + " ".join(f"{(ph[i] - ph[0]) / 1e3:.2f}" for i in range(7)))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Single-stage driver for ncu captures (B200_PROFILING.md recipe).  Runs one stage of the batch-32 Z10 workload with
+"""Single-stage runner for profiler captures.  Runs one stage of the batch-32 Z10 workload with
 eager launches (no CUDA graph) so that every kernel shows up as its own launch.
 
   ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/lm.csv python tools/prof.py --stage lm --steps 4
