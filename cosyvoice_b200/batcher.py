@@ -12,7 +12,13 @@ Admission policy: a batch is closed when ``max_batch`` requests are waiting or `
 arrived; requests are never reordered inside a batch (the model's RNG streams are consumed in input order, so a fixed arrival
 order gives fixed results).  One worker thread owns the model; ``tts_batch`` itself is ragged, so no padding or bucketing is
 needed here.
+
+Streaming requests (``submit_stream`` / ``submit_stream_pcm``) are served by ``tts_stream_batch``, which hands out every request's
+chunks as they become ready.  A batch is either all streaming or all offline: it is the run of requests of the same kind at the
+head of the queue, so it also closes early when a request of the other kind is waiting behind it, and no request is ever moved
+ahead of an earlier one of the other kind.
 """
+import queue
 import threading
 import time
 from concurrent.futures import Future
@@ -36,11 +42,40 @@ def pcm16_decode(buf):
     return torch.from_numpy(np.array(np.frombuffer(buf, dtype=np.int16))).unsqueeze(0).float() / (2 ** 15)
 
 
+_END = object()
+
+
+class _Failed:
+    def __init__(self, exc):
+        self.exc = exc
+
+
+class ChunkStream:
+    """Iterator over one streaming request's chunks, filled by the batcher's worker: yields each chunk as soon as it is produced,
+    ends after the request's batch has produced its last chunk, and re-raises the batch's exception if the batch fails."""
+
+    def __init__(self):
+        self._q = queue.Queue()
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        item = self._q.get()
+        if item is _END or isinstance(item, _Failed):
+            self._q.put(item)                    # every later next() ends the same way
+            if item is _END:
+                raise StopIteration
+            raise item.exc
+        return item
+
+
 class TtsBatcher:
     """``submit(**tts_kwargs)`` -> Future of the waveform ([1, N] float32 CPU tensor, what ``tts`` yields for stream=False);
-    ``submit_pcm`` -> Future of the int16 PCM bytes.  ``tts_kwargs`` are the keyword arguments of ``CosyVoice2Model.tts`` that the
-    batched pipeline consumes: text, prompt_text, llm_prompt_speech_token, flow_prompt_speech_token, prompt_speech_feat,
-    flow_embedding."""
+    ``submit_pcm`` -> Future of the int16 PCM bytes.  ``submit_stream`` / ``submit_stream_pcm`` -> iterator over the request's
+    chunks (what ``tts`` yields for stream=True: float [1, n] tensors, or their int16 PCM bytes).  ``tts_kwargs`` are the keyword
+    arguments of ``CosyVoice2Model.tts`` that the batched pipeline consumes: text, prompt_text, llm_prompt_speech_token,
+    flow_prompt_speech_token, prompt_speech_feat, flow_embedding."""
 
     def __init__(self, model, max_batch=32, max_wait_ms=10.0):
         assert max_batch >= 1
@@ -61,14 +96,20 @@ class TtsBatcher:
     def submit_pcm(self, **request):
         return self._enqueue(request, True)
 
-    def _enqueue(self, request, pcm):
-        fut = Future()
+    def submit_stream(self, **request):
+        return self._enqueue(request, False, ChunkStream())
+
+    def submit_stream_pcm(self, **request):
+        return self._enqueue(request, True, ChunkStream())
+
+    def _enqueue(self, request, pcm, stream=None):
+        sink = stream if stream is not None else Future()
         with self._cv:
             if self._closed:
                 raise RuntimeError("TtsBatcher is closed")
-            self._q.append((request, fut, pcm, time.monotonic()))
+            self._q.append((request, sink, pcm, time.monotonic()))
             self._cv.notify_all()
-        return fut
+        return sink
 
     def close(self, wait=True):
         """Stop admitting; requests already queued are still served."""
@@ -92,19 +133,32 @@ class TtsBatcher:
             if not self._q:
                 return None
             deadline = self._q[0][3] + self.max_wait
-            while len(self._q) < self.max_batch and not self._closed:
+            while self._run_length() < self.max_batch and self._run_length() == len(self._q) and not self._closed:
                 left = deadline - time.monotonic()
                 if left <= 0:
                     break
                 self._cv.wait(left)
-            batch, self._q = self._q[:self.max_batch], self._q[self.max_batch:]
+            n = min(self._run_length(), self.max_batch)
+            batch, self._q = self._q[:n], self._q[n:]
             return batch
+
+    def _run_length(self):
+        """requests of the head's kind (streaming or offline) at the head of the queue"""
+        kind = isinstance(self._q[0][1], ChunkStream)
+        n = 1
+        while n < len(self._q) and isinstance(self._q[n][1], ChunkStream) == kind:
+            n += 1
+        return n
 
     def _run(self):
         while True:
             batch = self._take_batch()
             if batch is None:
                 return
+            if isinstance(batch[0][1], ChunkStream):
+                self.batches.append(len(batch))
+                self._run_stream(batch)
+                continue
             live = [b for b in batch if b[1].set_running_or_notify_cancel()]
             if not live:
                 continue
@@ -120,3 +174,16 @@ class TtsBatcher:
                     fut.set_result(pcm16(w) if pcm else w)
                 except BaseException as e:
                     fut.set_exception(e)
+
+    def _run_stream(self, batch):
+        try:
+            for i, out in self.model.tts_stream_batch([b[0] for b in batch]):
+                _, sink, pcm, _ = batch[i]
+                w = out["tts_speech"]
+                sink._q.put(pcm16(w) if pcm else w)
+        except BaseException as e:              # the whole batch shares the failure (one launch sequence per stage)
+            for _, sink, _, _ in batch:
+                sink._q.put(_Failed(e))
+            return
+        for _, sink, _, _ in batch:
+            sink._q.put(_END)

@@ -104,6 +104,19 @@ void cvk_destroy(cvk_ctx* ctx) {
 const char* cvk_last_error(cvk_ctx* ctx) { return ctx ? ctx->last_error.c_str() : "null context"; }
 thread_local int cvk_in_capture = 0;
 int64_t cvk_launch_count(cvk_ctx* ctx) { return ctx ? ctx->launches.load() : 0; }
+int cvk_stream_create(cvk_ctx* ctx, void** out) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(out != nullptr, "cvk_stream_create: bad arguments");
+  cudaStream_t s = nullptr;
+  CVK_CHECK_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  *out = (void*)s;
+  CVK_API_END
+}
+void cvk_stream_destroy(cvk_ctx* ctx, void* stream) {
+  if (!ctx || !stream) return;
+  cudaSetDevice(ctx->device);
+  cudaStreamDestroy((cudaStream_t)stream);
+}
 double cvk_last_op_ms(cvk_ctx* ctx) { return ctx ? ctx->op_ms : 0.0; }
 int cvk_debug_read(cvk_ctx* ctx, long long* out, int n) {
   if (!ctx || !ctx->tl || !out || n != 4096) return CVK_ERR_INVALID;   // the LM-chain timeline ("chain_timeline")
@@ -385,13 +398,19 @@ int cvk_flow_inference(cvk_ctx* ctx, const int32_t* tokens, const int* token_len
 int cvk_flow_stream_create(cvk_ctx* ctx, int max_frames, int n_timesteps, cvk_flow_stream** out) {
   CVK_API_BEGIN
   CVK_REQUIRE(out != nullptr, "cvk_flow_stream_create: bad arguments");
-  *out = flow_stream_create(ctx, max_frames, n_timesteps, 0);
+  *out = flow_stream_create(ctx, 0, 1, max_frames, n_timesteps);
   CVK_API_END
 }
 int cvk_flow3_stream_create(cvk_ctx* ctx, int max_frames, int n_timesteps, cvk_flow_stream** out) {
   CVK_API_BEGIN
   CVK_REQUIRE(out != nullptr, "cvk_flow3_stream_create: bad arguments");
-  *out = flow_stream_create(ctx, max_frames, n_timesteps, 1);
+  *out = flow_stream_create(ctx, 1, 1, max_frames, n_timesteps);
+  CVK_API_END
+}
+int cvk_flow_stream_create_slots(cvk_ctx* ctx, int kind, int slots, int max_frames, int n_timesteps, cvk_flow_stream** out) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(out != nullptr && (kind == 0 || kind == 1) && slots >= 1, "cvk_flow_stream_create_slots: bad arguments");
+  *out = flow_stream_create(ctx, kind, slots, max_frames, n_timesteps);
   CVK_API_END
 }
 void cvk_flow_stream_destroy(cvk_ctx* ctx, cvk_flow_stream* fs) {
@@ -402,14 +421,29 @@ long long cvk_flow_stream_bytes(const cvk_flow_stream* fs) { return fs ? (long l
 int cvk_flow_stream_begin(cvk_ctx* ctx, cvk_flow_stream* fs, const float* prompt_feat, int prompt_frames, const float* embedding, void* stream) {
   CVK_API_BEGIN
   CVK_REQUIRE(fs && embedding && (prompt_feat || prompt_frames == 0), "cvk_flow_stream_begin: bad arguments");
-  flow_stream_begin(ctx, fs, prompt_feat, prompt_frames, embedding, (cudaStream_t)stream);
+  flow_stream_begin(ctx, fs, 0, prompt_feat, prompt_frames, embedding, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_flow_stream_begin_slot(cvk_ctx* ctx, cvk_flow_stream* fs, int slot, const float* prompt_feat, int prompt_frames, const float* embedding,
+                               void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(fs && embedding && (prompt_feat || prompt_frames == 0), "cvk_flow_stream_begin_slot: bad arguments");
+  flow_stream_begin(ctx, fs, slot, prompt_feat, prompt_frames, embedding, (cudaStream_t)stream);
   CVK_API_END
 }
 int cvk_flow_stream_chunk(cvk_ctx* ctx, cvk_flow_stream* fs, const int32_t* tokens, int n_tokens, float* mel_out, int mel_capacity_frames,
                           int* n_frames_out, void* stream) {
   CVK_API_BEGIN
   CVK_REQUIRE(fs && tokens && mel_out && n_frames_out && n_tokens > 3, "cvk_flow_stream_chunk: bad arguments");
-  *n_frames_out = flow_stream_chunk(ctx, fs, tokens, n_tokens, mel_out, mel_capacity_frames, (cudaStream_t)stream);
+  const int slot0 = 0;
+  flow_stream_chunk(ctx, fs, 1, &slot0, tokens, &n_tokens, mel_out, mel_capacity_frames, n_frames_out, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_flow_stream_chunk_batch(cvk_ctx* ctx, cvk_flow_stream* fs, int B, const int* slots_host, const int32_t* tokens, const int* token_lens_host,
+                                float* mel_out, int mel_capacity_frames, int* n_frames_out_host, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(fs && B > 0 && slots_host && tokens && token_lens_host && mel_out && n_frames_out_host, "cvk_flow_stream_chunk_batch: bad arguments");
+  flow_stream_chunk(ctx, fs, B, slots_host, tokens, token_lens_host, mel_out, mel_capacity_frames, n_frames_out_host, (cudaStream_t)stream);
   CVK_API_END
 }
 int cvk_cfm_set_noise(cvk_ctx* ctx, const float* noise_tm, int T, int on_device) {

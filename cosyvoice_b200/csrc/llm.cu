@@ -1128,7 +1128,6 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
   }
   const bool can_graph = ctx->use_graph && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;   // capture is illegal on the default streams
   if (can_graph && !s->graph) {
-    int64_t before = ctx->launches;
     cudaGraph_t graph = nullptr;
     CVK_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     cvk_in_capture = 1;
@@ -1142,10 +1141,22 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
       throw;
     }
     CVK_CHECK_CUDA(cudaStreamEndCapture(st, &graph));
+    // kernels of the step = kernel nodes of the graph (other threads launch concurrently, so the context counter cannot tell); the
+    // captured launches were counted while capturing and are counted again at every replay
+    size_t n_nodes = 0;
+    CVK_CHECK_CUDA(cudaGraphGetNodes(graph, nullptr, &n_nodes));
+    std::vector<cudaGraphNode_t> nodes(n_nodes);
+    if (n_nodes) CVK_CHECK_CUDA(cudaGraphGetNodes(graph, nodes.data(), &n_nodes));
+    int64_t kernels = 0;
+    for (cudaGraphNode_t n : nodes) {
+      cudaGraphNodeType t;
+      CVK_CHECK_CUDA(cudaGraphNodeGetType(n, &t));
+      kernels += t == cudaGraphNodeTypeKernel;
+    }
     CVK_CHECK_CUDA(cudaGraphInstantiate(&s->graph, graph, 0));
     cudaGraphDestroy(graph);
-    s->graph_kernels = ctx->launches - before;
-    ctx->launches -= s->graph_kernels;
+    s->graph_kernels = kernels;
+    ctx->launches -= kernels;
   }
   for (int i = 0; i < n_steps; ++i) {
     if (can_graph && s->graph) {

@@ -28,6 +28,8 @@ SIGNATURES = {
     "cvk_last_error": (ctypes.c_char_p, [_vp]),
     "cvk_version": (ctypes.c_char_p, []),
     "cvk_launch_count": (ctypes.c_int64, [_vp]),
+    "cvk_stream_create": (ctypes.c_int, [_vp, ctypes.POINTER(_vp)]),
+    "cvk_stream_destroy": (None, [_vp, _vp]),
     "cvk_last_op_ms": (ctypes.c_double, [_vp]),
     "cvk_debug_read": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int]),
     "cvk_set_option": (ctypes.c_int, [_vp, ctypes.c_char_p, ctypes.c_int]),
@@ -57,6 +59,9 @@ SIGNATURES = {
     "cvk_flow_stream_bytes": (ctypes.c_longlong, [_vp]),
     "cvk_flow_stream_begin": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_int, _vp, _vp]),
     "cvk_flow_stream_chunk": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, _c_int_p, _vp]),
+    "cvk_flow_stream_create_slots": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp)]),
+    "cvk_flow_stream_begin_slot": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp]),
+    "cvk_flow_stream_chunk_batch": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _c_int_p, _vp, _c_int_p, _vp, ctypes.c_int, _c_int_p, _vp]),
     "cvk_cfm_set_noise": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int]),
     "cvk_hift3_set_noise": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_longlong, ctypes.c_int]),
     "cvk_hift3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]),
@@ -193,6 +198,16 @@ class Context:
 
     def last_op_ms(self):
         return float(self.lib.cvk_last_op_ms(self.h))
+
+    def stream_create(self):
+        """a non-blocking CUDA stream owned by the caller (cvk_stream_create), as a torch ExternalStream; give it back with
+        stream_destroy"""
+        s = ctypes.c_void_p()
+        self._check(self.lib.cvk_stream_create(self.h, ctypes.byref(s)))
+        return torch.cuda.ExternalStream(s.value, device=self.device)
+
+    def stream_destroy(self, stream):
+        self.lib.cvk_stream_destroy(self.h, ctypes.c_void_p(stream.cuda_stream))
 
     def launch_count(self):
         return int(self.lib.cvk_launch_count(self.h))
@@ -350,11 +365,17 @@ class Context:
         return mel, out_lens
 
     # ------------------------------------------------------------------ incremental streaming flow (cvk.h: cvk_flow_stream_*)
-    def flow_stream(self, max_frames, n_timesteps=10, dit=False):
-        """dit=False: CosyVoice2 U-Net estimator (stage "flow"); dit=True: CosyVoice3 DiT (stage "flow3")"""
+    def flow_stream(self, max_frames, n_timesteps=10, dit=False, slots=1):
+        """dit=False: CosyVoice2 U-Net estimator (stage "flow"); dit=True: CosyVoice3 DiT (stage "flow3").  slots > 1: one session
+        holding `slots` independent utterances (cvk_flow_stream_create_slots), driven by flow_stream_begin_slot /
+        flow_stream_chunk_batch."""
         s = ctypes.c_void_p()
-        fn = self.lib.cvk_flow3_stream_create if dit else self.lib.cvk_flow_stream_create
-        self._check(fn(self.h, int(max_frames), int(n_timesteps), ctypes.byref(s)))
+        if slots == 1:
+            fn = self.lib.cvk_flow3_stream_create if dit else self.lib.cvk_flow_stream_create
+            self._check(fn(self.h, int(max_frames), int(n_timesteps), ctypes.byref(s)))
+        else:
+            self._check(self.lib.cvk_flow_stream_create_slots(self.h, int(bool(dit)), int(slots), int(max_frames), int(n_timesteps),
+                                                              ctypes.byref(s)))
         return s
 
     def flow_stream_destroy(self, fs):
@@ -377,6 +398,26 @@ class Context:
         n = ctypes.c_int(0)
         self._check(self.lib.cvk_flow_stream_chunk(self.h, fs, _ptr(tokens), int(tokens.numel()), _ptr(mel), cap, ctypes.byref(n), _stream()))
         return mel[:n.value]
+
+    def flow_stream_begin_slot(self, fs, slot, prompt_feat, embedding):
+        """new utterance in `slot` of a multi-slot session; prompt_feat [Tp,80] (may be empty), embedding [192] or [1,192]"""
+        pf = _f32(prompt_feat, self.device) if prompt_feat is not None and prompt_feat.numel() else None
+        emb = _f32(embedding, self.device)
+        self._check(self.lib.cvk_flow_stream_begin_slot(self.h, fs, int(slot), _ptr(pf), 0 if pf is None else int(pf.shape[0]), _ptr(emb),
+                                                        _stream()))
+
+    def flow_stream_chunk_batch(self, fs, slots, token_list):
+        """One chunk for each slot in `slots`; token_list[b]: 1-D int tokens of slots[b] (as for flow_stream_chunk).  Returns
+        (mel [sum n_b, 80], [n_b]): the new frames of every slot back to back."""
+        toks = torch.cat([t.reshape(-1).to(device=self.device, dtype=torch.int32) for t in token_list]).contiguous()
+        lens = [int(t.numel()) for t in token_list]
+        cap = 2 * sum(lens)
+        mel = torch.empty(cap, 80, device=self.device)
+        n = (ctypes.c_int * len(lens))()
+        self._check(self.lib.cvk_flow_stream_chunk_batch(self.h, fs, len(lens), _ints(slots), _ptr(toks), _ints(lens), _ptr(mel), cap, n,
+                                                         _stream()))
+        out = [int(v) for v in n]
+        return mel[:sum(out)], out
 
     # ------------------------------------------------------------------ LM
     def lm_session(self, max_batch, max_context):

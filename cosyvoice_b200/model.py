@@ -11,7 +11,7 @@ random streams the reference draws from the global RNG (sampling uniforms, SineG
 import threading
 import time
 import uuid
-from contextlib import nullcontext
+from contextlib import contextmanager, nullcontext
 
 import numpy as np
 import torch
@@ -21,6 +21,10 @@ from . import cvk
 TOKEN_MEL_RATIO = 2          # cosyvoice2.yaml:14
 PRE_LOOKAHEAD = 3            # cosyvoice2.yaml:46
 SAMPLES_PER_FRAME = 480
+
+
+class _LmStopped(Exception):
+    """raised into a batched LM generation whose consumer has gone away"""
 
 
 def _count(keys, prefix):
@@ -66,6 +70,16 @@ class B200CosyVoice2Model:
     incremental_flow = True
     flow_stream_dit = False              # which estimator the sessions cache: the CosyVoice2 U-Net (stage "flow") or the CosyVoice3 DiT ("flow3")
     stream_cache_frames = 2048           # mel frames (prompt included) one streaming request can cache (41 s); ~2.3 MB per frame in bf16
+    # tts_stream_batch: the most slots of the one multi-slot flow session the model creates on first use, each caching
+    # stream_cache_frames frames (~2.3 MB per frame for the full-size U-Net in bf16: 16 x 2048 frames would be 75 GB).  The session
+    # takes the largest of stream_batch_slots, /2, /4, ... that allocates and leaves stream_pool_headroom bytes of device memory free
+    # for LM sessions and activations (8 slots next to a full-size model with the default 24 GB workspace on an 80 GB card);
+    # `stream_slots` reports the outcome.  0 = no session.  Requests that find no free slot recompute their prefix like the reference.
+    stream_batch_slots = 16
+    stream_pool_headroom = 8 << 30
+    stream_slots = None                  # slots of the session once tts_stream_batch has tried to create it (0: none fitted)
+    _slot_pool = None                    # the multi-slot cvk_flow_stream handle, once created
+    _free_slots = None                   # its free slot indices
 
     def __init__(self, llm=None, flow=None, hift=None, fp16=False, precision="bf16", device=0, workspace_gb=24.0):
         # attribute names follow cli/model.py:245-275
@@ -92,6 +106,7 @@ class B200CosyVoice2Model:
         self.max_idle_sessions = 4
         self._pool_lock = threading.Lock()
         self._lm_streams = []
+        self._idle_lm_streams = []           # LM job streams not in use (see _lm_stream)
         self.flow_stream_dict = {}           # uuid -> cvk_flow_stream handle, or False once a request has left the chunk grid
         self._idle_flow_streams = []
         self.lm_chains = 1                   # independent decode chains run concurrently (see lm_generate)
@@ -144,8 +159,24 @@ class B200CosyVoice2Model:
                 return key, free.pop()
         return key, self.ctx.lm_session(*key)
 
-    def _new_lm_stream(self):
-        return torch.cuda.Stream(self.device) if self.device.type == "cuda" else None
+    @contextmanager
+    def _lm_stream(self):
+        """A stream that belongs to one LM job until it ends.  The decode step graph is captured on it, so it must never be the
+        model's stream or another job's: torch's pooled streams are handed out round-robin from 32 per device and repeat after 32
+        creations, so they come from cvk_stream_create instead and are recycled here."""
+        if self.device.type != "cuda":
+            yield None
+            return
+        with self._pool_lock:
+            s = self._idle_lm_streams.pop() if self._idle_lm_streams else None
+        if s is None:
+            s = self.ctx.stream_create()
+        try:
+            yield s
+        finally:
+            s.synchronize()
+            with self._pool_lock:
+                self._idle_lm_streams.append(s)
 
     def _checkin_session(self, key, sess):
         evict = []
@@ -212,7 +243,7 @@ class B200CosyVoice2Model:
                         ready.record(self.stream)
                     c["ready"] = ready
             while len(self._lm_streams) < chains:
-                self._lm_streams.append(torch.cuda.Stream(d))
+                self._lm_streams.append(self.ctx.stream_create())
             n = 0
             for c in st:
                 c["left"] = mx                     # upper bound of the steps this chain still needs (refined after every block)
@@ -534,14 +565,15 @@ class B200CosyVoice2Model:
         if hasattr(text, "__next__") or (hasattr(text, "__iter__") and not torch.is_tensor(text)):
             # cli/model.py:113-123: text generator -> bi-stream decoding, tokens appended one by one
             cur_silent, max_silent = 0, 5                  # cli/model.py:102,121-127 (silent_tokens is empty for CosyVoice2)
-            for tok in self.lm_generate_bistream(iter(text), prompt_text, llm_prompt_speech_token, stream=self._new_lm_stream()):
-                if tok in self.silent_tokens:
-                    cur_silent += 1
-                    if cur_silent > max_silent:
-                        continue
-                else:
-                    cur_silent = 0
-                self.tts_speech_token_dict[uuid].append(tok)
+            with self._lm_stream() as lm_stream:
+                for tok in self.lm_generate_bistream(iter(text), prompt_text, llm_prompt_speech_token, stream=lm_stream):
+                    if tok in self.silent_tokens:
+                        cur_silent += 1
+                        if cur_silent > max_silent:
+                            continue
+                    else:
+                        cur_silent = 0
+                    self.tts_speech_token_dict[uuid].append(tok)
             self.llm_end_dict[uuid] = True
             return
 
@@ -561,8 +593,8 @@ class B200CosyVoice2Model:
                 st["consumed"] = n
         # the LM job decodes on its own stream (cli/model.py:103: `with self.llm_context`, a side stream) while token2wav runs on
         # the model's stream
-        self.lm_generate([text], [prompt_text], [llm_prompt_speech_token], steps_per_sync=8, on_progress=progress,
-                         stream=self._new_lm_stream())
+        with self._lm_stream() as lm_stream:
+            self.lm_generate([text], [prompt_text], [llm_prompt_speech_token], steps_per_sync=8, on_progress=progress, stream=lm_stream)
         self.llm_end_dict[uuid] = True
 
     def vc_job(self, source_speech_token, uuid):
@@ -617,3 +649,244 @@ class B200CosyVoice2Model:
             self.hift_cache_dict.pop(this_uuid)
         self._release_flow_stream(this_uuid)
         self.stream.synchronize()
+
+    # ---------------------------------------------------------------- batched streaming
+    def _take_slot(self):
+        """a free slot of the model's multi-slot flow session (created on first use), or None: no session configured, no memory
+        for it, or every slot taken"""
+        if not self.incremental_flow or self.stream_batch_slots <= 0:
+            return None
+        with torch.cuda.stream(self.stream), self.ctx.lock, self._pool_lock:     # the lock order of _flow_stream_chunk
+            if self.stream_slots is None:
+                self._create_slot_pool()
+            return self._free_slots.pop(0) if self._free_slots else None
+
+    def _create_slot_pool(self):
+        """Once per model: the largest slot count of stream_batch_slots, /2, /4, ... whose session allocates and leaves
+        stream_pool_headroom bytes free.  A model that fits none records 0 slots and is not retried."""
+        import warnings
+        n = self.stream_batch_slots
+        while n >= 1:
+            try:
+                pool = self.ctx.flow_stream(self.stream_cache_frames, self.n_timesteps, dit=self.flow_stream_dit, slots=n)
+            except cvk.CvkError:
+                pool = None
+            if pool is not None and self.device.type == "cuda" and torch.cuda.mem_get_info(self.device)[0] < self.stream_pool_headroom:
+                self.ctx.flow_stream_destroy(pool)
+                pool = None
+            if pool is not None:
+                break
+            n //= 2
+        self._slot_pool, self.stream_slots = pool, n if pool is not None else 0
+        self._free_slots = list(range(self.stream_slots))
+        if self.stream_slots < self.stream_batch_slots:
+            warnings.warn(f"tts_stream_batch: {self.stream_slots} of {self.stream_batch_slots} streaming-flow slots of {self.stream_cache_frames} "
+                          "frames fit in device memory; requests beyond them recompute their prefix", RuntimeWarning, stacklevel=4)
+
+    def _give_slot(self, slot):
+        with self._pool_lock:
+            self._free_slots.append(slot)
+            self._free_slots.sort()
+
+    def _noise_for(self, i, n, noise_fns):
+        """vocoder noise of request i for n samples: its own stream when given, else the model's hook or generator"""
+        if noise_fns is not None:
+            return noise_fns[i](n).to(self.device)
+        if self.noise_fn is not None:
+            return self.noise_fn(n).to(self.device)
+        return torch.randn(n, 9, device=self.device, generator=self.generator)
+
+    def tts_stream_batch(self, inputs, uniforms=None, noise_fns=None):
+        """Streaming synthesis of several requests at once: a generator of (i, {'tts_speech': float32 CPU [1, n]}).
+
+        `inputs` are tts() kwargs dicts with tensor `text`, as for tts_batch.  Each request gets exactly the chunks tts(stream=True)
+        yields for it alone (cli/model.py:339-374: first hop token_hop_len + the prompt's padding to the hop grid, then x
+        stream_scale_factor up to token_max_hop_len, 3 look-ahead tokens, a final non-streaming call); its chunks come out in order,
+        requests interleave as their chunks become ready.  One LM generation decodes every row on a side stream (uniforms[:, i]
+        for request i, as in tts_batch); every poll round then makes at most one call per stage for all requests that are ready:
+        one cvk_flow_stream_chunk_batch for requests holding a slot of the model's multi-slot session, one prefix-recompute
+        flow_inference for the others, one final flow_inference for requests that are finishing, and one vocoder call over all of
+        them.  Request i's k-th vocoder call draws noise_fns[i](n) when given, so its audio does not depend on which other
+        requests shared its rounds.  The instance's token_hop_len is not modified.  Closing the generator early (or an
+        exception in it) gives the requests' slots back and ends the LM generation within one block of 8 decode steps."""
+        for r in inputs:
+            if not torch.is_tensor(r.get("text")):
+                raise ValueError("tts_stream_batch takes token tensors as text; a text generator (bi-stream LM) is served by tts()")
+        B = len(inputs)
+        empty = torch.zeros(1, 0, dtype=torch.int32)
+        req = [dict(ptok=r.get("flow_prompt_speech_token", empty), pfeat=r.get("prompt_speech_feat", torch.zeros(1, 0, 80)),
+                    emb=r.get("flow_embedding", torch.zeros(0, 192))) for r in inputs]
+        toks = [[] for _ in range(B)]
+        lm_state = {"end": False, "err": None, "stop": False}
+        consumed, silent = [0] * B, [0] * B
+
+        def progress(out_ids, out_count, live):
+            if lm_state["stop"]:
+                raise _LmStopped()                       # the generator was closed: end the decode at the next block
+            cnt = out_count.cpu().tolist()
+            ids = out_ids.cpu()
+            for b in range(B):
+                if cnt[b] > consumed[b]:
+                    for tok in ids[b, consumed[b]:cnt[b]].tolist():
+                        if tok in self.silent_tokens:            # cli/model.py:121-127
+                            silent[b] += 1
+                            if silent[b] > 5:
+                                continue
+                        else:
+                            silent[b] = 0
+                        toks[b].append(tok)
+                    consumed[b] = cnt[b]
+
+        def llm_job():
+            try:
+                with self._lm_stream() as lm_stream:
+                    self.lm_generate([r["text"] for r in inputs], [r.get("prompt_text", empty) for r in inputs],
+                                     [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms, steps_per_sync=8,
+                                     on_progress=progress, stream=lm_stream)
+            except _LmStopped:
+                pass
+            except BaseException as e:                   # noqa: BLE001  (re-raised by the generator)
+                lm_state["err"] = e
+            finally:
+                lm_state["end"] = True
+
+        hop0 = self.token_hop_len
+        st = []
+        for r in req:
+            P = int(r["ptok"].shape[1])
+            st.append(dict(P=P, pad=int(np.ceil(P / hop0) * hop0 - P), hop=hop0, offset=0, slot=None, eligible=True, cache=None,
+                           done=False))
+        p = threading.Thread(target=llm_job, name="cvk-stream-batch-lm", daemon=True)
+        p.start()
+        try:
+            while not all(s["done"] for s in st):
+                end = lm_state["end"]                    # read first: once the LM has ended, the token lists are complete
+                if lm_state["err"] is not None:
+                    raise lm_state["err"]
+                ready, finishing = [], []
+                for i, s in enumerate(st):
+                    if s["done"]:
+                        continue
+                    this_hop = s["hop"] + s["pad"] if s["offset"] == 0 else s["hop"]
+                    if len(toks[i]) - s["offset"] >= this_hop + PRE_LOOKAHEAD:
+                        ready.append((i, this_hop))
+                    elif end:
+                        finishing.append(i)
+                if not ready and not finishing:
+                    time.sleep(0.005)
+                    continue
+                for i, out in self._stream_round(req, st, toks, ready, finishing, noise_fns):
+                    yield i, out
+            p.join()
+        finally:
+            lm_state["stop"] = True                      # closed or failed early: the LM stops within one block of 8 steps
+            for s in st:
+                if s["slot"] is not None:
+                    self._give_slot(s["slot"])
+                    s["slot"] = None
+            if self.stream is not None:
+                self.stream.synchronize()
+
+    def _stream_round(self, req, st, toks, ready, finishing, noise_fns):
+        """one poll round of tts_stream_batch: flow for every ready / finishing request (at most three calls), one vocoder call,
+        then token2wav's cache and cross-fade bookkeeping per request (cli/model.py:292-326)"""
+        d = self.device
+        slot_grp, prefix_grp = [], []
+        for i, this_hop in ready:
+            s = st[i]
+            ptok, pfeat = req[i]["ptok"], req[i]["pfeat"]
+            n_tok = s["offset"] + this_hop + PRE_LOOKAHEAD
+            this_tok = torch.tensor(toks[i][:n_tok], dtype=torch.int32).unsqueeze(0)
+            if s["eligible"]:
+                # the rule of _flow_stream_chunk: chunk ends on the 50-frame grid, 2 prompt frames per prompt token, capacity, and a
+                # slot from the request's first chunk on
+                total = TOKEN_MEL_RATIO * (s["P"] + n_tok - PRE_LOOKAHEAD)
+                done = TOKEN_MEL_RATIO * (s["P"] + s["offset"]) if s["offset"] else 0
+                ok = (total % 50 == 0 and done % 50 == 0 and int(pfeat.shape[1]) == TOKEN_MEL_RATIO * s["P"]
+                      and total <= self.stream_cache_frames and (s["slot"] is not None or s["offset"] == 0))
+                if ok and s["slot"] is None:
+                    s["slot"] = self._take_slot()
+                    s["begin"] = s["slot"] is not None
+                    ok = s["slot"] is not None
+                if not ok:
+                    s["eligible"] = False
+                    if s["slot"] is not None:
+                        self._give_slot(s["slot"])
+                        s["slot"] = None
+            (slot_grp if s["eligible"] else prefix_grp).append((i, this_hop, this_tok))
+        mels = {}
+        if slot_grp:
+            with torch.cuda.stream(self.stream), self.ctx.lock:
+                for i, _, _ in slot_grp:
+                    if st[i].pop("begin", False):
+                        self.ctx.flow_stream_begin_slot(self._slot_pool, st[i]["slot"], req[i]["pfeat"][0].to(d, non_blocking=True),
+                                                        req[i]["emb"].reshape(-1).to(d, non_blocking=True))
+                token_list = [torch.cat([req[i]["ptok"].reshape(-1), t.reshape(-1)]).to(torch.int32) for i, _, t in slot_grp]
+                mel, lens = self.ctx.flow_stream_chunk_batch(self._slot_pool, [st[i]["slot"] for i, _, _ in slot_grp], token_list)
+            o = 0
+            for (i, _, _), n in zip(slot_grp, lens):
+                mels[i] = mel[o:o + n]
+                o += n
+        for grp, final in ((prefix_grp, False), ([(i, None, torch.tensor(toks[i], dtype=torch.int32).unsqueeze(0)) for i in finishing], True)):
+            grp = [g for g in grp if g[2].shape[1] > 0]
+            if not grp:
+                continue
+            mel, lens = self.flow_batch([t for _, _, t in grp], [req[i]["ptok"] for i, _, _ in grp], [req[i]["pfeat"] for i, _, _ in grp],
+                                        [req[i]["emb"] for i, _, _ in grp], streaming=not final, finalize=final)
+            o = 0
+            for (i, _, _), n in zip(grp, lens):
+                mels[i] = mel[o + st[i]["offset"] * TOKEN_MEL_RATIO:o + n]
+                o += n
+        # vocoder: every request of the round in one call, each with its own cached mel / source
+        order = [i for i, _ in ready] + finishing
+        outs = {}
+        voc = [i for i in order if i in mels]
+        if voc:
+            with torch.cuda.stream(self.stream):
+                tts_mel, lens, cache_src, cache_lens, noise = [], [], [], [], []
+                for i in voc:
+                    c = st[i]["cache"]
+                    m_i = torch.cat([c["mel"], mels[i]], 0) if c is not None else mels[i]
+                    tts_mel.append(m_i)
+                    lens.append(int(m_i.shape[0]))
+                    cache_lens.append(int(c["source"].shape[0]) if c is not None else 0)
+                    if c is not None:
+                        cache_src.append(c["source"])
+                    noise.append(self._noise_for(i, lens[-1] * SAMPLES_PER_FRAME, noise_fns))
+                with self.ctx.lock:
+                    wav, src = self.ctx.hift_inference(torch.cat(tts_mel, 0), lens, torch.cat(noise, 0),
+                                                       torch.cat(cache_src) if cache_src else None, cache_lens if cache_src else None)
+                o = 0
+                for i, m_i, n in zip(voc, tts_mel, lens):
+                    w, s_ = wav[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME], src[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME]
+                    o += n
+                    c = st[i]["cache"]
+                    if c is not None:
+                        w = self._fade_in_out(w, c["speech"])
+                    if i in finishing:
+                        outs[i] = w
+                    else:
+                        st[i]["cache"] = {"mel": m_i[-self.mel_cache_len:].clone(), "source": s_[-self.source_cache_len:].clone(),
+                                          "speech": w[-self.source_cache_len:].clone()}
+                        outs[i] = w[:-self.source_cache_len]
+                flat = torch.cat([outs[i] for i in voc]).cpu() if voc else None       # one D2H for the round
+            if self.stream is not None:
+                self.stream.synchronize()
+        for i, this_hop in ready:
+            st[i]["offset"] += this_hop
+            st[i]["hop"] = min(self.token_max_hop_len, st[i]["hop"] * self.stream_scale_factor)
+        o = 0
+        results = []
+        for i in order:
+            if i in outs:
+                n = int(outs[i].shape[0])
+                results.append((i, {"tts_speech": flat[o:o + n].unsqueeze(0)}))
+                o += n
+            else:
+                results.append((i, {"tts_speech": torch.zeros(1, 0)}))
+        for i in finishing:
+            st[i]["done"] = True
+            if st[i]["slot"] is not None:
+                self._give_slot(st[i]["slot"])
+                st[i]["slot"] = None
+        return results

@@ -25,6 +25,11 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
         # FSQ silent and breath tokens (cli/model.py:423)
         self.silent_tokens = [1, 2, 28, 29, 55, 248, 494, 2241, 2242, 2322, 2323]
 
+    def tts_stream_batch(self, inputs, uniforms=None, noise_fns=None):
+        """Not built for CosyVoice3: the inherited scheduler keeps CosyVoice2's vocoder caches and cross-fade, while CosyVoice3's
+        causal vocoder re-runs over all mel produced so far (cli/model.py:425-450).  The multi-slot DiT sessions exist in libcvk."""
+        raise NotImplementedError("tts_stream_batch is CosyVoice2-only; stream CosyVoice3 requests with tts(stream=True)")
+
     # ---------------------------------------------------------------- weights
     def load_state_dicts(self, llm_sd, flow_sd, hift_sd, rand_ini=None, sine_noise=None):
         """llm_sd: CosyVoice3LM, flow_sd: CausalMaskedDiffWithDiT, hift_sd: CausalHiFTGenerator state_dicts.  rand_ini [1,9] /

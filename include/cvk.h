@@ -55,6 +55,11 @@ const char* cvk_last_error(cvk_ctx* ctx);
 const char* cvk_version(void);
 /* kernels launched by this library since creation (bench.py "gpu_launches") */
 int64_t cvk_launch_count(cvk_ctx* ctx);
+/* A CUDA stream (non-blocking) of the context's device that belongs to the caller alone until cvk_stream_destroy.  For concurrent LM
+ * sessions: the decode step graph is captured on the caller's stream, so two sessions, or a session and the workspace calls, must
+ * never share one (pooled framework streams are reused round-robin and give no such guarantee). */
+int cvk_stream_create(cvk_ctx* ctx, void** out);
+void cvk_stream_destroy(cvk_ctx* ctx, void* stream);
 /* mean device time (ms) of the kernel timed by the last cvk_op_* call when the "op_iters" option is > 0 (tools/gemm_probe.py) */
 double cvk_last_op_ms(cvk_ctx* ctx);
 /* debug: copy the LM decode-chain timeline (4 int64 slots per launch, n must be 4096) recorded while "chain_timeline" is on */
@@ -165,6 +170,22 @@ int cvk_flow_stream_begin(cvk_ctx* ctx, cvk_flow_stream* fs, const float* prompt
                           void* stream);
 int cvk_flow_stream_chunk(cvk_ctx* ctx, cvk_flow_stream* fs, const int32_t* tokens, int n_tokens, float* mel_out,
                           int mel_capacity_frames, int* n_frames_out, void* stream);
+/* Multi-slot sessions: `slots` independent utterances in one session (kind 0: U-Net "flow", 1: DiT "flow3").  All slots share one
+ * cache allocation per Euler step ([n_blocks][2*slots*cap + 64][K|V]; CFG sequence c of slot s owns rows [(2s+c)*cap, (2s+c+1)*cap)),
+ * so one chunk call serves several slots with one launch sequence per stage - the batched form of the reference's per-request
+ * streaming loop (cli/model.py:346-363).  The calls above are the 1-slot session, slot 0.
+ * begin_slot: new utterance in `slot`; the other slots are not touched.
+ * chunk_batch: one chunk for each of B <= slots distinct, begun slots slots_host[0..B).  tokens [sum token_lens_host] ragged, per
+ * slot the argument of cvk_flow_stream_chunk; mel_out receives the new frames of every slot back to back ([sum n_frames_out_host,
+ * 80], capacity mel_capacity_frames rows), n_frames_out_host[b] their counts.  Every rule of cvk_flow_stream_chunk holds per slot;
+ * all arguments are checked before any device work, so a refused call changes no slot's state.
+ * Threading: like every flow call, begin_slot / chunk_batch use the workspace and are serialised by the caller. */
+int cvk_flow_stream_create_slots(cvk_ctx* ctx, int kind, int slots, int max_frames, int n_timesteps, cvk_flow_stream** out);
+int cvk_flow_stream_begin_slot(cvk_ctx* ctx, cvk_flow_stream* fs, int slot, const float* prompt_feat, int prompt_frames,
+                               const float* embedding, void* stream);
+int cvk_flow_stream_chunk_batch(cvk_ctx* ctx, cvk_flow_stream* fs, int B, const int* slots_host, const int32_t* tokens,
+                                const int* token_lens_host, float* mel_out, int mel_capacity_frames, int* n_frames_out_host,
+                                void* stream);
 
 /* ---- CosyVoice3 vocoder (stage "hift3") ------------------------------------------------------------------------------------
  * cosyvoice/hifigan/generator.py:572-726 CausalHiFTGenerator (+ f0_predictor.py:60-103 in float64, generator.py:716-717).
