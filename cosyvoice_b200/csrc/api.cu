@@ -1,6 +1,7 @@
 // extern "C" boundary of libcvk (include/cvk.h): argument checking, error translation, no exceptions across the ABI.
 #include "common.cuh"
 #include <string.h>
+#include <algorithm>
 
 // stage entry points implemented in hift.cu / flow.cu / llm.cu / mel.cu
 void hift_build(cvk_ctx* ctx);
@@ -42,6 +43,8 @@ void llm_feed(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* ids, const int32_t
 void llm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, cudaStream_t st);
 void llm_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* history, int hist_ld, const int32_t* hist_count,
                     const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, cudaStream_t st);
+void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
+                             const int* ctx_len_host, int max_ctx, float* out, cudaStream_t st);
 void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int fmax_hz, float* mel, cudaStream_t st);
 void mel_init(cvk_ctx* ctx);
 void prompt_feat_init(cvk_ctx* ctx);
@@ -227,10 +230,13 @@ int cvk_op_conv1d(cvk_ctx* ctx, const float* x, const int* lens, int B, int K, c
                   int dil, int shift0, int act, float* out, void* stream) {
   CVK_API_BEGIN
   cudaStream_t st = (cudaStream_t)stream;
-  CVK_REQUIRE(x && lens && w && out && B > 0, "cvk_op_conv1d: bad arguments");
+  CVK_REQUIRE(x && lens && w && out && B > 0 && N >= 1 && K >= 1 && taps >= 1 && dil >= 1, "cvk_op_conv1d: bad arguments");
   ctx->arena.reset();
   size_t owned_mark = ctx->owned.size();
-  int gap = 32;
+  // Both kernels read rows r + shift0 + j*dil straight from the packed matrix and rely on zero gap rows between sequences: the gap
+  // must cover the receptive field on either side, or a sequence convolves with its neighbour's edge.
+  const int reach = std::max(-shift0, (taps - 1) * dil + shift0);
+  int gap = std::max(32, round_up(reach, 8));
   Seqs s = make_seqs(ctx, lens, B, gap, 1, 0, st);
   ConvW W = make_conv(ctx, w, bias, N, K, taps, dil, shift0);
   CVK_CHECK_CUDA(cudaDeviceSynchronize());   // weight repack runs on the default stream
@@ -275,34 +281,47 @@ int cvk_op_linear_small(cvk_ctx* ctx, const float* x, int rows, int K, const flo
                         float* ms_out, void* stream) {
   CVK_API_BEGIN
   cudaStream_t st = (cudaStream_t)stream;
-  CVK_REQUIRE(x && w && out && rows > 0 && rows <= 64 && ctx->precision == CVK_PREC_BF16, "cvk_op_linear_small: bf16 context, rows <= 64");
+  // every argument is checked before the first allocation or launch: the weight streaming layout needs K % 8 == 0 (finish_convw
+  // makes no bf16 copy otherwise) and at least one K chunk and one output tile (the split count divides by both)
+  CVK_REQUIRE(x && w && out && rows >= 1 && rows <= 64 && N >= 1 && K >= 8 && K % 8 == 0 && iters >= 0 &&
+                  ctx->precision == CVK_PREC_BF16,
+              "cvk_op_linear_small: bf16 context, 1 <= rows <= 64, N >= 1, K >= 8 and K % 8 == 0");
   ctx->arena.reset();
   size_t owned_mark = ctx->owned.size();
-  ConvW W = make_conv(ctx, w, bias, N, K, 1, 1, 0);
-  skinny_tiled_weights(ctx, W);
-  CVK_CHECK_CUDA(cudaDeviceSynchronize());
-  Mat a32((void*)x, DT_F32, rows, K, K);
-  Mat a = arena_mat(ctx, DT_BF16, rows, K);
-  convert_mat(ctx, st, a32, a);
-  Mat o(out, DT_F32, rows, N, N);
-  size_t sf = skinny_scratch_floats(rows, N);
-  float* scratch = (float*)ctx->arena.alloc(sf * sizeof(float));
-  Epilogue e;
-  e.out = o;
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  conv_gemm_skinny(ctx, st, a, W, e, scratch, sf);
-  cudaEventRecord(e0, st);
-  for (int i = 0; i < iters; ++i) conv_gemm_skinny(ctx, st, a, W, e, scratch, sf);
-  cudaEventRecord(e1, st);
-  CVK_CHECK_CUDA(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  if (ms_out) *ms_out = iters > 0 ? ms / iters : 0.f;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  ctx->tiled.erase(W.w16);
-  for (size_t i = owned_mark; i < ctx->owned.size(); ++i) cudaFree(ctx->owned[i]);
-  ctx->owned.resize(owned_mark);
+  ConvW W;
+  auto release = [&]() {      // the weight copies live only for this call; a stale `tiled` entry would outlive its source buffer
+    if (W.w16) ctx->tiled.erase(W.w16);
+    for (size_t i = owned_mark; i < ctx->owned.size(); ++i) cudaFree(ctx->owned[i]);
+    ctx->owned.resize(owned_mark);
+  };
+  try {
+    W = make_conv(ctx, w, bias, N, K, 1, 1, 0);
+    skinny_tiled_weights(ctx, W);
+    CVK_CHECK_CUDA(cudaDeviceSynchronize());
+    Mat a32((void*)x, DT_F32, rows, K, K);
+    Mat a = arena_mat(ctx, DT_BF16, rows, K);
+    convert_mat(ctx, st, a32, a);
+    Mat o(out, DT_F32, rows, N, N);
+    size_t sf = skinny_scratch_floats(rows, N);
+    float* scratch = (float*)ctx->arena.alloc(sf * sizeof(float));
+    Epilogue e;
+    e.out = o;
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    conv_gemm_skinny(ctx, st, a, W, e, scratch, sf);
+    cudaEventRecord(e0, st);
+    for (int i = 0; i < iters; ++i) conv_gemm_skinny(ctx, st, a, W, e, scratch, sf);
+    cudaEventRecord(e1, st);
+    CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    if (ms_out) *ms_out = iters > 0 ? ms / iters : 0.f;
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+  } catch (...) {
+    release();
+    throw;
+  }
+  release();
   CVK_API_END
 }
 
@@ -310,7 +329,8 @@ int cvk_op_attention(cvk_ctx* ctx, const float* q, const float* k, const float* 
                      float scale, float* out, void* stream) {
   CVK_API_BEGIN
   cudaStream_t st = (cudaStream_t)stream;
-  CVK_REQUIRE(q && k && v && out && lens && B > 0 && H > 0, "cvk_op_attention: bad arguments");
+  // scale > 0: the tensor-core kernel takes the row maximum of the unscaled scores
+  CVK_REQUIRE(q && k && v && out && lens && B > 0 && H > 0 && chunk >= 0 && scale > 0.f, "cvk_op_attention: bad arguments");
   ctx->arena.reset();
   Seqs s = make_seqs(ctx, lens, B, 8, 1, 0, st);
   int C = H * 64;
@@ -322,6 +342,49 @@ int cvk_op_attention(cvk_ctx* ctx, const float* q, const float* k, const float* 
   pack_rows(ctx, st, v, C, s, mv);
   attention_fwd(ctx, st, mq, mk, mv, s, H, chunk, scale, mo);
   unpack_rows(ctx, st, mo, s, 0, out, C);
+  CVK_API_END
+}
+
+int cvk_op_attention_ex(cvk_ctx* ctx, const float* q, const float* k, const float* v, const int* q_lens, const int* k_lens,
+                        const int* q_offset, int B, int H, int kv_heads, int chunk, float scale, float* out, void* stream) {
+  CVK_API_BEGIN
+  cudaStream_t st = (cudaStream_t)stream;
+  CVK_REQUIRE(q && k && v && out && q_lens && k_lens && q_offset && B > 0 && H > 0 && kv_heads > 0 && H % kv_heads == 0 && chunk >= 0 &&
+                  scale > 0.f,
+              "cvk_op_attention_ex: bad arguments");
+  for (int b = 0; b < B; ++b)
+    CVK_REQUIRE(q_lens[b] >= 1 && k_lens[b] >= 1 && q_offset[b] >= 0, "cvk_op_attention_ex: empty sequence or negative offset");
+  ctx->arena.reset();
+  // queries and keys are packed separately, the keys addressed through a cache geometry: the layout of the LM prefill (GQA) and of
+  // the streaming flow sessions (key cache longer than the new query rows)
+  Seqs s = make_seqs(ctx, q_lens, B, 8, 1, 0, st);
+  Seqs ks = make_seqs(ctx, k_lens, B, 8, 1, 0, st, false);
+  int* d_qoff = (int*)ctx->arena.alloc(sizeof(int) * B);
+  CVK_CHECK_CUDA(cudaMemcpyAsync(d_qoff, q_offset, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  KvGeom kg;
+  kg.d_kstart = ks.d_start;
+  kg.d_klen = ks.d_len;
+  kg.d_qoff = d_qoff;
+  const int C = H * 64, Ck = kv_heads * 64;
+  Mat mq = arena_mat(ctx, ctx->act_dtype, s.R, C), mo = arena_mat(ctx, ctx->act_dtype, s.R, C);
+  Mat mk = arena_mat(ctx, ctx->act_dtype, ks.R, Ck), mv = arena_mat(ctx, ctx->act_dtype, ks.R, Ck);
+  zero_mat(ctx, st, mq); zero_mat(ctx, st, mk); zero_mat(ctx, st, mv); zero_mat(ctx, st, mo);
+  pack_rows(ctx, st, q, C, s, mq);
+  pack_rows(ctx, st, k, Ck, ks, mk);
+  pack_rows(ctx, st, v, Ck, ks, mv);
+  attention_fwd(ctx, st, mq, mk, mv, s, H, chunk, scale, mo, H / kv_heads, &kg);
+  unpack_rows(ctx, st, mo, s, 0, out, C);
+  CVK_API_END
+}
+
+int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
+                            const int* ctx_len, int max_ctx, float* out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(partial && bias && k_cache && v_cache && ctx_len && out && splits >= 1 && rows >= 1 && max_ctx >= 1 &&
+                  ctx->precision == CVK_PREC_BF16,
+              "cvk_op_decode_attention: bad arguments (bf16 context)");
+  for (int b = 0; b < rows; ++b) CVK_REQUIRE(ctx_len[b] >= 0 && ctx_len[b] < max_ctx, "cvk_op_decode_attention: ctx_len outside [0, max_ctx)");
+  llm_decode_attention_op(ctx, partial, splits, rows, bias, k_cache, v_cache, ctx_len, max_ctx, out, (cudaStream_t)stream);
   CVK_API_END
 }
 

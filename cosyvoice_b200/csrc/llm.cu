@@ -186,6 +186,17 @@ decode_attn_kernel(const T* __restrict__ qkv, int ld, const T* __restrict__ kc, 
   op[lane + 32] = from_f32<T>(o1 * inv);
 }
 
+// qkv[b] = sum_s partial[s][b] + bias, in split order, rounded to the activation dtype: the split-K reduction of the per-op
+// (unfused) decode path, cvk_op_decode_attention with lm_fused = 0
+__global__ void qkv_reduce_kernel(const float* __restrict__ partial, int splits, int rows, const float* __restrict__ bias, bf16* __restrict__ qkv) {
+  const size_t total = (size_t)rows * QKV_N;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int s = 0; s < splits; ++s) acc += partial[(size_t)s * total + i];
+    qkv[i] = __float2bfloat16_rn(acc + bias[i % QKV_N]);
+  }
+}
+
 // ---- fused decode kernels (bf16 path) -----------------------------------------------------------------------------
 // x[b] += sum_s partial[s][b] (+bias); xn[b] = rmsnorm(x[b]) * gamma  - split-K reduction, residual add and the next
 // RMSNorm (modeling_qwen2.py:258-263) in one pass; one CTA per row.
@@ -831,7 +842,65 @@ void head_logits(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, const Mat& hi
   lm_gemm(ctx, st, xn_act, m->head, e, sess);
 }
 
+// Let decode_attn_kernel hold the scores of max_ctx positions for its 7 query heads in shared memory.  The limit is per function,
+// not per session: it is never lowered for a smaller context requested later.
+void decode_attn_allow_ctx(int max_ctx) {
+  static int decode_attn_smem = 0;
+  const size_t need = (size_t)(NH / NKV) * max_ctx * sizeof(float);
+  CVK_REQUIRE(need <= 200 * 1024, "session context too long for the decode attention kernel (max ~7300 positions)");
+  if ((int)need > decode_attn_smem) {
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    decode_attn_smem = (int)need;
+  }
+}
+
+constexpr size_t ATTN_FUSED_SMEM = ((NH / NKV + 2) * HD + AF_WARPS * 8 * 2 + AF_WARPS * (NH / NKV) * HD) * sizeof(float);
+
 }  // namespace
+
+// RoPE frequencies of the half-split rotation (theta 1e6): the table every LM decode / prefill kernel reads
+void lm_rope_inv_freq(float* out) {
+  for (int i = 0; i < HD / 2; ++i) out[i] = 1.0f / powf(ROPE_THETA, (float)(2 * i) / (float)HD);
+}
+
+// One decode-attention step on a caller-supplied cache, without a loaded LM (cvk_op_decode_attention): the qkv split-K partial sums
+// [splits][rows][1152] + bias -> RoPE at position ctx_len[b] -> append k, v to the cache -> GQA attention over positions
+// 0..ctx_len[b].  The caches [rows][NKV][max_ctx][64] cross the call as fp32 and run as bf16, as in a session.  lm_fused selects
+// attn_fused_kernel (the decode graph's kernel) or the per-op pair rope_append_kernel + decode_attn_kernel.
+void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
+                             const int* ctx_len_host, int max_ctx, float* out, cudaStream_t st) {
+  decode_attn_allow_ctx(max_ctx);      // the context limit of a session, whichever kernel runs
+  ctx->arena.reset();
+  float inv[HD / 2];
+  lm_rope_inv_freq(inv);
+  float* d_inv = (float*)ctx->arena.alloc(sizeof(inv));
+  CVK_CHECK_CUDA(cudaMemcpyAsync(d_inv, inv, sizeof(inv), cudaMemcpyHostToDevice, st));
+  int* d_len = upload(ctx, std::vector<int>(ctx_len_host, ctx_len_host + rows), st);
+  const int cache_rows = rows * NKV * max_ctx;
+  Mat k32(k_cache, DT_F32, cache_rows, HD, HD), v32(v_cache, DT_F32, cache_rows, HD, HD);
+  Mat kc = arena_mat(ctx, DT_BF16, cache_rows, HD, HD), vc = arena_mat(ctx, DT_BF16, cache_rows, HD, HD);
+  Mat att = arena_mat(ctx, DT_BF16, rows, D, D);
+  convert_mat(ctx, st, k32, kc);
+  convert_mat(ctx, st, v32, vc);
+  if (ctx->lm_fused) {
+    launch_ex(attn_fused_kernel, dim3(rows, NKV), dim3(32 * AF_WARPS), ATTN_FUSED_SMEM, st, false, partial, splits, rows, bias, kc.b16(),
+              vc.b16(), (const int*)d_len, max_ctx, (const float*)d_inv, att.b16(), att.ld, (long long*)nullptr);
+    ctx->launches++;
+  } else {
+    Mat qkv = arena_mat(ctx, DT_BF16, rows, QKV_N, QKV_N);
+    qkv_reduce_kernel<<<ceil_div(rows * QKV_N, 256), 256, 0, st>>>(partial, splits, rows, bias, qkv.b16());
+    rope_append_kernel<bf16><<<dim3(1, rows), 128, 0, st>>>(qkv.b16(), qkv.ld, nullptr, nullptr, d_len, d_inv, kc.b16(), vc.b16(), max_ctx, 1);
+    decode_attn_kernel<bf16><<<dim3(rows, NKV), (NH / NKV) * 32, (NH / NKV) * max_ctx * sizeof(float), st>>>(
+        qkv.b16(), qkv.ld, kc.b16(), vc.b16(), d_len, max_ctx, att.b16(), att.ld);
+    ctx->launches += 3;
+  }
+  CVK_LAUNCH_CHECK();
+  convert_mat(ctx, st, kc, k32);
+  convert_mat(ctx, st, vc, v32);
+  convert_mat(ctx, st, att, Mat(out, DT_F32, rows, D, D));
+  CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+}
 
 // ================================================================================================ build / session
 void llm_build(cvk_ctx* ctx, const int* cfg, int ncfg) {
@@ -891,7 +960,7 @@ void llm_build(cvk_ctx* ctx, const int* cfg, int ncfg) {
     }
     m->layers.push_back(w);
   }
-  for (int i = 0; i < HD / 2; ++i) m->inv_freq[i] = 1.0f / powf(ROPE_THETA, (float)(2 * i) / (float)HD);
+  lm_rope_inv_freq(m->inv_freq);
   m->d_inv_freq = (float*)ctx->dmalloc(sizeof(m->inv_freq));
   CVK_CHECK_CUDA(cudaMemcpy(m->d_inv_freq, m->inv_freq, sizeof(m->inv_freq), cudaMemcpyHostToDevice));
   CVK_CHECK_CUDA(cudaDeviceSynchronize());
@@ -920,25 +989,14 @@ cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context)
   s->base_len = (int*)alloc(sizeof(int) * max_batch);
   CVK_CHECK_CUDA(cudaFuncSetAttribute(ras_sampler_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem(VOUT3_PAD)));
   CVK_REQUIRE((NH / NKV) * max_context * sizeof(float) <= 200 * 1024, "session context too long for the decode attention kernel");
-  {
-    // the limit is per function, not per session: never lower it for a smaller session created later
-    static int decode_attn_smem = 0;
-    const int need = (int)((NH / NKV) * max_context * sizeof(float));
-    CVK_REQUIRE(need <= 200 * 1024, "session context too long for the decode attention kernel (max ~7300 positions)");
-    if (need > decode_attn_smem) {
-      CVK_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, need));
-      CVK_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, need));
-      decode_attn_smem = need;
-    }
-  }
+  decode_attn_allow_ctx(max_context);
   // keep every kernel of the decode step on the same (maximum) shared-memory carveout: alternating carveouts between
   // consecutive kernels forces an SM reconfiguration (idle + several microseconds) at every boundary
   CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(finish_rms_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(ras_sampler_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   skinny_set_carveout();
-  CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(((NH / NKV + 2) * HD + AF_WARPS * 8 * 2 + AF_WARPS * (NH / NKV) * HD) * sizeof(float))));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATTN_FUSED_SMEM));
   s->count = (int*)alloc(sizeof(int) * max_batch);
   s->done = (int*)alloc(sizeof(int) * max_batch);
   s->live = (int*)alloc(sizeof(int));

@@ -43,6 +43,9 @@ SIGNATURES = {
     "cvk_op_linear_small": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
                                            ctypes.POINTER(ctypes.c_float), _vp]),
     "cvk_op_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp, _vp]),
+    "cvk_op_attention_ex": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, _c_int_p, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_int, ctypes.c_float, _vp, _vp]),
+    "cvk_op_decode_attention": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_hift_f0": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_hift_source": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _vp]),
     "cvk_hift_decode": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _vp]),
@@ -239,6 +242,25 @@ class Context:
         self._check(self.lib.cvk_op_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ints(lens), len(lens), heads, chunk, scale,
                                               _ptr(out), _stream()))
         return out
+
+    def attention_ex(self, q, k, v, q_lens, k_lens, q_offset, heads, kv_heads, chunk=0, scale=0.125):
+        """q [sum q_lens, heads*64], k / v [sum k_lens, kv_heads*64]; query i of sequence b at position q_offset[b] + i"""
+        q, k, v = (_f32(t, self.device) for t in (q, k, v))
+        out = torch.empty_like(q)
+        self._check(self.lib.cvk_op_attention_ex(self.h, _ptr(q), _ptr(k), _ptr(v), _ints(q_lens), _ints(k_lens), _ints(q_offset),
+                                                 len(q_lens), heads, kv_heads, chunk, scale, _ptr(out), _stream()))
+        return out
+
+    def decode_attention(self, partial, bias, k_cache, v_cache, ctx_len):
+        """one LM decode-attention step: partial [splits, rows, 1152], bias [1152], caches [rows, 2, max_ctx, 64] (copies are
+        returned with the new row appended), ctx_len [rows] (python ints).  Returns (out [rows, 896], k_cache, v_cache)."""
+        partial, bias = _f32(partial, self.device), _f32(bias, self.device)
+        k_cache, v_cache = _f32(k_cache, self.device).clone(), _f32(v_cache, self.device).clone()
+        splits, rows = partial.shape[0], partial.shape[1]
+        out = torch.empty(rows, 896, device=self.device)
+        self._check(self.lib.cvk_op_decode_attention(self.h, _ptr(partial), splits, rows, _ptr(bias), _ptr(k_cache), _ptr(v_cache),
+                                                     _ints(ctx_len), k_cache.shape[2], _ptr(out), _stream()))
+        return out, k_cache, v_cache
 
     # ------------------------------------------------------------------ HiFT
     def hift_f0(self, mel, lens):

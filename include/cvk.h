@@ -91,16 +91,32 @@ int cvk_finalize(cvk_ctx* ctx, const char* stage, const int* cfg, int ncfg);
 /* ---------------------------------------------------------------------------------------------- generic ops
  * exposed for per-op parity tests (tests/test_ops_gpu.py); same kernels the stages use. */
 /* out[r,n] = act(bias[n] + sum_j sum_k x[r + shift0 + j*dil, k] * w[n,k,j]) for one zero-padded sequence per
- * entry of lens_host.  w is a torch Conv1d weight [N,K,taps] fp32 on the device. */
+ * entry of lens_host, at any receptive field (rows outside a sequence read as zero, never as a neighbouring sequence).
+ * w is a torch Conv1d weight [N,K,taps] fp32 on the device; N, K, taps, dil >= 1. */
 int cvk_op_conv1d(cvk_ctx* ctx, const float* x, const int* lens_host, int B, int K, const float* w, const float* bias,
                   int N, int taps, int dil, int shift0, int act, float* out, void* stream);
-/* out[b,n] = bias[n] + sum_k x[b,k] w[n,k] through the LM decode weight-streaming kernel (bf16 context, rows <= 64);
- * runs it `iters` more times and reports the mean device time. */
+/* out[b,n] = bias[n] + sum_k x[b,k] w[n,k] through the LM decode weight-streaming kernel (bf16 context, 1 <= rows <= 64, N >= 1,
+ * K >= 8 with K % 8 == 0; anything else is refused with CVK_ERR_INVALID before any device work); runs it `iters` more times and
+ * reports the mean device time. */
 int cvk_op_linear_small(cvk_ctx* ctx, const float* x, int rows, int K, const float* w, const float* bias, int N, float* out, int iters,
                         float* ms_out, void* stream);
-/* block-causal / full multi-head attention over ragged sequences; q,k,v,out [sum(lens), H*64] */
+/* block-causal / full multi-head attention over ragged sequences; q,k,v,out [sum(lens), H*64]; scale > 0 */
 int cvk_op_attention(cvk_ctx* ctx, const float* q, const float* k, const float* v, const int* lens_host, int B, int H,
                      int chunk, float scale, float* out, void* stream);
+/* the same kernels with grouped-query heads and a key cache, as the LM prefill and the streaming flow sessions run them:
+ * q, out [sum q_lens, H*64], k, v [sum k_lens, kv_heads*64] (ragged, packed separately); query head h reads kv head h / (H / kv_heads).
+ * Query row i of sequence b sits at absolute position q_offset_host[b] + i; key j of sequence b is visible iff j < k_lens_host[b] and,
+ * when chunk > 0, j < ((q_offset_host[b] + i) / chunk + 1) * chunk.  With k_lens == q_lens and q_offset == 0 this is cvk_op_attention.
+ * Requires H % kv_heads == 0, scale > 0, lengths >= 1. */
+int cvk_op_attention_ex(cvk_ctx* ctx, const float* q, const float* k, const float* v, const int* q_lens_host, const int* k_lens_host,
+                        const int* q_offset_host, int B, int H, int kv_heads, int chunk, float scale, float* out, void* stream);
+/* One LM decode-attention step (Qwen2 GQA 14/2 x 64, half-split RoPE theta 1e6) on a caller-supplied cache, bf16 context only:
+ * partial [splits][rows][1152] are the split-K sums of the qkv projection, bias [1152]; k_cache, v_cache [rows][2][max_ctx][64] fp32,
+ * in / out (run as bf16, as in a session, and written back as fp32 with the new row appended); ctx_len_host[b] in [0, max_ctx) is the
+ * position of the new token, i.e. the number of history rows; out [rows][896].  Option "lm_fused" selects the fused kernel of the
+ * decode graph (default) or, at 0, the per-op reduction + RoPE/append + attention kernels.  max_ctx obeys the session limit. */
+int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
+                            const int* ctx_len_host, int max_ctx, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------- HiFT vocoder
  * replaces cosyvoice/hifigan/generator.py:557-569 (HiFTGenerator.inference) and its parts. */
