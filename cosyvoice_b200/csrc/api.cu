@@ -388,6 +388,132 @@ int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int 
   CVK_API_END
 }
 
+int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, int operand, const int* seq_start, const int* seq_len, int B,
+                     const float* w, const float* bias, int N, int taps, int dil, int shift0, int act1, float act1_param, const float* alpha1,
+                     const float* resid, int resid_ld, int resid_is_out, int accumulate, float* out, int out_dtype, int out_ld, int act2,
+                     float act2_param, const float* alpha2, float* out2, int out2_dtype, int out2_ld, void* stream) {
+  CVK_API_BEGIN
+  cudaStream_t st = (cudaStream_t)stream;
+  auto dt_ok = [](int d) { return d == DT_F32 || d == DT_BF16 || d == DT_F16; };
+  auto act_ok = [](int a) { return a >= ACT_NONE && a <= ACT_GELU_TANH; };
+  auto esize = [](int d) { return d == DT_F32 ? (size_t)4 : (size_t)2; };
+  // every argument is checked before the first allocation or launch
+  CVK_REQUIRE(x && seq_start && seq_len && w && out && B >= 1 && rows >= 1 && K >= 1 && x_ld >= K && N >= 1 && taps >= 1 && dil >= 1 &&
+                  dt_ok(operand) && dt_ok(out_dtype) && out_ld >= N && act_ok(act1) && act_ok(act2) &&
+                  (!out2 || (dt_ok(out2_dtype) && out2_ld >= N)) && (!resid || resid_ld >= N) && !(resid && resid_is_out) &&
+                  (!resid_is_out || out_dtype == DT_F32),
+              "cvk_op_conv_gemm: bad arguments");
+  CVK_REQUIRE(operand == DT_F32 || (ctx->precision == CVK_PREC_BF16 && K % 8 == 0),
+              "cvk_op_conv_gemm: a 16-bit operand needs a bf16 context and K % 8 == 0 (no 16-bit weight copy otherwise)");
+  // output row r reads rows r + shift0 + j*dil, j < taps: a gap narrower than that reach lets a sequence see its neighbour
+  const long long reach = std::max(0LL, std::max(-(long long)shift0, (long long)shift0 + (long long)(taps - 1) * dil));
+  std::vector<int> order(B);
+  for (int b = 0; b < B; ++b) {
+    order[b] = b;
+    CVK_REQUIRE(seq_len[b] >= 1 && seq_start[b] >= 0 && (long long)seq_start[b] + seq_len[b] <= rows,
+                "cvk_op_conv_gemm: empty sequence or sequence outside [0, rows)");
+  }
+  std::sort(order.begin(), order.end(), [&](int a, int b) { return seq_start[a] < seq_start[b]; });
+  for (int i = 1; i < B; ++i) {
+    const long long gap = (long long)seq_start[order[i]] - ((long long)seq_start[order[i - 1]] + seq_len[order[i - 1]]);
+    CVK_REQUIRE(gap >= reach, "cvk_op_conv_gemm: sequences overlap or are closer than the receptive field");
+  }
+  if (operand != DT_F32 && ctx->use_tc)
+    CVK_REQUIRE(x_ld % 8 == 0 && ((size_t)out_ld * esize(out_dtype)) % 16 == 0 && (!out2 || ((size_t)out2_ld * esize(out2_dtype)) % 16 == 0) &&
+                    (!resid || (resid_ld % 4 == 0 && ((uintptr_t)resid & 15) == 0)),
+                "cvk_op_conv_gemm: the wgmma kernel needs 16-byte aligned rows of x, out, out2 and resid");
+  ctx->arena.reset();
+  const size_t owned_mark = ctx->owned.size();
+  auto release = [&]() {      // the weight copies live only for this call
+    for (size_t i = owned_mark; i < ctx->owned.size(); ++i) cudaFree(ctx->owned[i]);
+    ctx->owned.resize(owned_mark);
+  };
+  try {
+    ConvW W;
+    {
+      // fp16 operands: the IEEE-half weight copy the vocoder stage builds, instead of the bf16 one
+      struct F16Scope { cvk_ctx* c; F16Scope(cvk_ctx* c_, bool on) : c(c_) { c->build_f16 = on; } ~F16Scope() { c->build_f16 = 0; } } f16scope(ctx, operand == DT_F16);
+      W = make_conv(ctx, w, bias, N, K, taps, dil, shift0);
+    }
+    CVK_CHECK_CUDA(cudaDeviceSynchronize());   // weight repack runs on the default stream
+    std::vector<int> row2seq(rows, -1);
+    for (int b = 0; b < B; ++b)
+      for (int i = 0; i < seq_len[b]; ++i) row2seq[seq_start[b] + i] = b;
+    int* d_row2seq = (int*)ctx->arena.alloc(sizeof(int) * (size_t)rows);
+    CVK_CHECK_CUDA(cudaMemcpyAsync(d_row2seq, row2seq.data(), sizeof(int) * (size_t)rows, cudaMemcpyHostToDevice, st));
+    // the operand keeps x's pitch, so the columns [K, x_ld) travel with it and must stay unread
+    Mat a((void*)x, DT_F32, rows, K, x_ld);
+    if (operand != DT_F32) {
+      Mat a16 = arena_mat(ctx, operand, rows, x_ld, x_ld);
+      convert_mat(ctx, st, Mat((void*)x, DT_F32, rows, x_ld, x_ld), a16);
+      a = Mat(a16.p, operand, rows, K, x_ld);
+    }
+    auto stage = [&](float* p, int dt, int ld) {      // the whole caller matrix, pad columns included, in the output dtype
+      Mat m = arena_mat(ctx, dt, rows, ld, ld);
+      convert_mat(ctx, st, Mat(p, DT_F32, rows, ld, ld), m);
+      return m;
+    };
+    Mat o = stage(out, out_dtype, out_ld);
+    Epilogue e;
+    e.act1 = act1;
+    e.act1_param = act1_param;
+    e.alpha1 = alpha1;
+    if (resid_is_out) e.resid = Mat(o.p, DT_F32, rows, N, out_ld);
+    else if (resid) e.resid = Mat((void*)resid, DT_F32, rows, N, resid_ld);
+    e.row2seq = d_row2seq;
+    e.accumulate = accumulate;
+    e.out = Mat(o.p, out_dtype, rows, N, out_ld);
+    e.act2 = act2;
+    e.act2_param = act2_param;
+    e.alpha2 = alpha2;
+    Mat o2;
+    if (out2) {
+      o2 = stage(out2, out2_dtype, out2_ld);
+      e.out2 = Mat(o2.p, out2_dtype, rows, N, out2_ld);
+    }
+    if (operand == DT_F32) conv_gemm_simt(ctx, st, a, W, e);
+    else conv_gemm(ctx, st, a, W, e);
+    convert_mat(ctx, st, o, Mat(out, DT_F32, rows, out_ld, out_ld));
+    if (out2) convert_mat(ctx, st, o2, Mat(out2, DT_F32, rows, out2_ld, out2_ld));
+    CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+  } catch (...) {
+    release();
+    throw;
+  }
+  release();
+  CVK_API_END
+}
+
+int cvk_op_relpos_attention(cvk_ctx* ctx, const float* q, const float* k, const float* v, const float* pos, int center, const float* bias_u,
+                            const float* bias_v, const int* lens, int B, int H, int chunk, float scale, float* out, void* stream) {
+  CVK_API_BEGIN
+  cudaStream_t st = (cudaStream_t)stream;
+  // scale > 0: the tensor-core kernel takes the row maximum of the unscaled scores
+  CVK_REQUIRE(q && k && v && pos && bias_u && bias_v && lens && out && B >= 1 && H >= 1 && chunk >= 0 && scale > 0.f && center < (1 << 24),
+              "cvk_op_relpos_attention: bad arguments");
+  int max_len = 0;
+  for (int b = 0; b < B; ++b) {
+    CVK_REQUIRE(lens[b] >= 1, "cvk_op_relpos_attention: empty sequence");
+    max_len = std::max(max_len, lens[b]);
+  }
+  CVK_REQUIRE(center >= max_len - 1, "cvk_op_relpos_attention: the table must hold the relative positions -(max(lens)-1) .. max(lens)-1");
+  ctx->arena.reset();
+  Seqs s = make_seqs(ctx, lens, B, 8, 1, 0, st);
+  const int C = H * 64, adt = ctx->act_dtype, pos_rows = 2 * center + 1;
+  Mat mq = arena_mat(ctx, adt, s.R, C), mk = arena_mat(ctx, adt, s.R, C), mv = arena_mat(ctx, adt, s.R, C), mo = arena_mat(ctx, adt, s.R, C);
+  zero_mat(ctx, st, mq); zero_mat(ctx, st, mk); zero_mat(ctx, st, mv); zero_mat(ctx, st, mo);
+  pack_rows(ctx, st, q, C, s, mq);
+  pack_rows(ctx, st, k, C, s, mk);
+  pack_rows(ctx, st, v, C, s, mv);
+  // zero rows up to a multiple of 128, as the encoder builds its table (flow.cu make_pe)
+  Mat pe = arena_mat(ctx, adt, round_up(pos_rows, 128), C);
+  zero_mat(ctx, st, pe);
+  convert_mat(ctx, st, Mat((void*)pos, DT_F32, pos_rows, C, C), Mat(pe.p, adt, pos_rows, C, pe.ld));
+  relpos_attention_fwd(ctx, st, mq, mk, mv, pe, center, bias_u, bias_v, s, H, chunk, scale, mo);
+  unpack_rows(ctx, st, mo, s, 0, out, C);
+  CVK_API_END
+}
+
 // ---------------------------------------------------------------------------------------------- HiFT
 int cvk_hift_f0(cvk_ctx* ctx, const float* mel, const int* lens, int B, float* f0, void* stream) {
   CVK_API_BEGIN

@@ -1,5 +1,5 @@
 // fp32 CUDA-core conv-GEMM: the parity path (CVK_PREC_FP32) and the kernel for the precision-critical layers
-// (f0 predictor, mel DFT) in every mode.
+// (f0 predictor, mel DFT) in every mode; with use_tc = 0 it also takes the bf16 / fp16 operands of the tensor-core mode.
 //
 //   out[r, n] = epilogue( sum_{j<taps} sum_{k<K} A[r + shift0 + j*dil, k] * W[n][j][k] )
 //
@@ -95,6 +95,11 @@ void conv_gemm_simt(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W,
   if (A.dtype == DT_F32) {
     conv_gemm_simt_kernel<float, float><<<grid, 256, 0, st>>>(A.f32(), A.ld, A.rows, W.w32, W.N, W.K, W.taps, W.dil, W.shift0,
                                                               rowsOut, e);
+  } else if (A.dtype == DT_F16) {
+    // the vocoder's IEEE-half operands (use_tc = 0 in a bf16 context): its weights carry only the half copy
+    CVK_REQUIRE(W.wf16 != nullptr, "conv_gemm: fp16 operand but no fp16 weights");
+    conv_gemm_simt_kernel<__half, __half><<<grid, 256, 0, st>>>((const __half*)A.p, A.ld, A.rows, W.wf16, W.N, W.K, W.taps, W.dil,
+                                                                W.shift0, rowsOut, e);
   } else {
     CVK_REQUIRE(W.w16 != nullptr, "conv_gemm: bf16 operand but no bf16 weights");
     conv_gemm_simt_kernel<bf16, bf16><<<grid, 256, 0, st>>>(A.b16(), A.ld, A.rows, W.w16, W.N, W.K, W.taps, W.dil, W.shift0,

@@ -522,7 +522,10 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   CUtensorMap to = ta, to2 = ta;
   if (epi_mode == 2) {
     const size_t need = (size_t)TC_BM * BN * ep.out.esize() + (ep.out2.p ? (size_t)TC_BM * BN * ep.out2.esize() : 0);
-    if (ep.accumulate || need > TC_STG_BYTES) epi_mode = 0;
+    // the TMA store of a tile whose last column ends inside a 16-byte chunk of the row also overwrote the columns past N (an H100
+    // wrote the pad columns of N = 1 in pitch 4 and of N = 18 in pitch 24, fp32): such widths take the direct stores, which write [0, N) only
+    const bool whole16 = (W.N * ep.out.esize()) % 16 == 0 && (!ep.out2.p || (W.N * ep.out2.esize()) % 16 == 0);
+    if (ep.accumulate || need > TC_STG_BYTES || !whole16) epi_mode = 0;
   }
   if (epi_mode == 2) {
     auto mk = [&](CUtensorMap* m, const Mat& o) {

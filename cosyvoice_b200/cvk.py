@@ -13,7 +13,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "lib", "libcvk.so")
 
 PREC_FP32, PREC_BF16 = 0, 1
-ACT = dict(none=0, gelu=1, silu=2, mish=3, elu=4, lrelu=5, snake=6, tanh=7, abs=8)
+ACT = dict(none=0, gelu=1, silu=2, mish=3, elu=4, lrelu=5, snake=6, tanh=7, abs=8, gelu_tanh=9)
+DTYPE = dict(fp32=0, bf16=1, fp16=2)       # CVK_DT_*
 
 _lib = None
 _lib_lock = threading.Lock()
@@ -46,6 +47,12 @@ SIGNATURES = {
     "cvk_op_attention_ex": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, _c_int_p, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_op_decode_attention": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
+    "cvk_op_conv_gemm": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_int_p, _c_int_p, ctypes.c_int,
+                                        _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp,
+                                        _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                        ctypes.c_float, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]),
+    "cvk_op_relpos_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int,
+                                               ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_hift_f0": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_hift_source": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _vp]),
     "cvk_hift_decode": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _vp]),
@@ -261,6 +268,33 @@ class Context:
         self._check(self.lib.cvk_op_decode_attention(self.h, _ptr(partial), splits, rows, _ptr(bias), _ptr(k_cache), _ptr(v_cache),
                                                      _ints(ctx_len), k_cache.shape[2], _ptr(out), _stream()))
         return out, k_cache, v_cache
+
+    def conv_gemm(self, x, seq_start, seq_len, w, bias=None, dil=1, shift0=0, operand="fp32", act1="none", act1_param=0.0, alpha1=None,
+                  resid=None, resid_is_out=False, accumulate=False, out=None, out_dtype="fp32", act2="none", act2_param=0.0, alpha2=None,
+                  out2=None, out2_dtype="fp32"):
+        """One conv-GEMM launch with the stage epilogue on packed matrices (cvk_op_conv_gemm): x [rows, x_ld] (columns >= K =
+        w.shape[1] are never read), w a torch Conv1d weight [N,K,taps], sequences b at rows [seq_start[b], + seq_len[b]).  out / out2:
+        fp32 [rows, ld] initial contents (out required, out2 None for no second output); returns the updated (out, out2) copies."""
+        x, w = _f32(x, self.device), _f32(w, self.device)
+        b, a1, a2, r = (_f32(t, self.device) if t is not None else None for t in (bias, alpha1, alpha2, resid))
+        out = _f32(out, self.device).clone()
+        out2 = _f32(out2, self.device).clone() if out2 is not None else None
+        N, K, taps = w.shape
+        self._check(self.lib.cvk_op_conv_gemm(
+            self.h, _ptr(x), x.shape[0], K, x.shape[1], DTYPE[operand], _ints(seq_start), _ints(seq_len), len(seq_len), _ptr(w), _ptr(b),
+            N, taps, dil, shift0, ACT[act1], act1_param, _ptr(a1), _ptr(r), r.shape[1] if r is not None else 0, int(resid_is_out),
+            int(accumulate), _ptr(out), DTYPE[out_dtype], out.shape[1], ACT[act2], act2_param, _ptr(a2), _ptr(out2), DTYPE[out2_dtype],
+            out2.shape[1] if out2 is not None else 0, _stream()))
+        return out, out2
+
+    def relpos_attention(self, q, k, v, pos, center, bias_u, bias_v, lens, heads, chunk=0, scale=0.125):
+        """conformer relative-position attention (cvk_op_relpos_attention): q, k, v [sum lens, heads*64], pos [2*center+1, heads*64]
+        (row t: relative position center - t), bias_u / bias_v [heads*64]"""
+        q, k, v, pos, bu, bv = (_f32(t, self.device) for t in (q, k, v, pos, bias_u, bias_v))
+        out = torch.empty_like(q)
+        self._check(self.lib.cvk_op_relpos_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(pos), int(center), _ptr(bu), _ptr(bv),
+                                                     _ints(lens), len(lens), heads, chunk, scale, _ptr(out), _stream()))
+        return out
 
     # ------------------------------------------------------------------ HiFT
     def hift_f0(self, mel, lens):

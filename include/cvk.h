@@ -117,6 +117,37 @@ int cvk_op_attention_ex(cvk_ctx* ctx, const float* q, const float* k, const floa
  * decode graph (default) or, at 0, the per-op reduction + RoPE/append + attention kernels.  max_ctx obeys the session limit. */
 int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
                             const int* ctx_len_host, int max_ctx, float* out, void* stream);
+/* element types of the cvk_op_conv_gemm operand and outputs */
+#define CVK_DT_F32 0
+#define CVK_DT_BF16 1
+#define CVK_DT_F16 2 /* IEEE half (the vocoder's operands in the bf16 context); stores saturate at +-65504 */
+/* One conv-GEMM launch with the fused epilogue the stages use, on caller-packed matrices (tests):
+ *   v    = act1(bias[n] + sum_j sum_k x[r + shift0 + j*dil, k] * w[n,k,j]; act1_param, alpha1[n]) (+ resid[r,n])
+ *   v    = valid(r) ? v : 0,  out[r,n] = accumulate ? out[r,n] + v : v,  out2[r,n] = valid(r) ? act2(v; act2_param, alpha2[n]) : 0
+ * x [rows, x_ld] fp32 (x_ld >= K; columns [K, x_ld) are never read) is converted to `operand` (CVK_DT_*; 16-bit operands need a bf16
+ * context and K % 8 == 0; fp16 operands use the half weight copy the vocoder stage builds).  Rows outside [0, rows) read as zero.  Sequence b
+ * occupies rows [seq_start_host[b], + seq_len_host[b]); every other row is a gap row (invalid) and must hold zeros in x.  Sequences must
+ * lie inside [0, rows), not overlap, and be separated by gaps at least as wide as the receptive field (max(-shift0, shift0 +
+ * (taps-1)*dil) rows).  w is a torch Conv1d weight [N,K,taps], bias [N] or NULL, alpha1 / alpha2 [N] or NULL (alpha 1).
+ * resid [rows, resid_ld] fp32 or NULL; resid_is_out = 1 adds the fp32 out itself (in place; resid must be NULL).  out / out2 (out2 may be
+ * NULL) are fp32 [rows, out_ld] / [rows, out2_ld] (ld >= N) in / out: their contents are rounded to out_dtype / out2_dtype to form the
+ * device matrices (accumulate input, untouched pad columns [N, ld) and rows) and the whole matrices are converted back.
+ * Path: fp32 operand -> CUDA-core kernel; 16-bit operand -> wgmma (options "tc_epi", "tc_persist") or, with "use_tc" 0, CUDA cores.
+ * A wgmma launch needs 16-byte aligned rows of x (as `operand`), out and out2 (as their dtypes) and resid_ld % 4 == 0.  Every argument is
+ * checked before any device work; a refusal returns CVK_ERR_INVALID. */
+int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, int operand, const int* seq_start_host,
+                     const int* seq_len_host, int B, const float* w, const float* bias, int N, int taps, int dil, int shift0, int act1,
+                     float act1_param, const float* alpha1, const float* resid, int resid_ld, int resid_is_out, int accumulate,
+                     float* out, int out_dtype, int out_ld, int act2, float act2_param, const float* alpha2, float* out2, int out2_dtype,
+                     int out2_ld, void* stream);
+/* The conformer relative-position attention (tests): score(i, j) = ((q_i + bias_u) . k_j + (q_i + bias_v) . pos[center - (i - j)]) * scale
+ * per head, block-causal when chunk > 0 (key j visible iff j < (i / chunk + 1) * chunk), softmax over the visible keys, times v.
+ * q, k, v, out [sum lens, H*64] ragged; pos [2*center+1, H*64] (row t holds relative position center - t; the library pads it to a
+ * multiple of 128 rows); bias_u, bias_v [H*64].  fp32 context: CUDA-core fp32 kernel; bf16 context: the wgmma pair, or the CUDA-core
+ * kernel on bf16 operands when "enc_tc_attn" or "use_tc_attn" is 0.  Requires H >= 1, chunk >= 0, scale > 0, lengths >= 1 and
+ * center >= max(lens) - 1. */
+int cvk_op_relpos_attention(cvk_ctx* ctx, const float* q, const float* k, const float* v, const float* pos, int center, const float* bias_u,
+                            const float* bias_v, const int* lens_host, int B, int H, int chunk, float scale, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------- HiFT vocoder
  * replaces cosyvoice/hifigan/generator.py:557-569 (HiFTGenerator.inference) and its parts. */

@@ -1,5 +1,8 @@
-"""Plain fp64 CPU references of the kernels checked by test_kernel_edges_gpu.py.  test_kernel_refs_cpu.py checks them against
-torch's scaled_dot_product_attention and the oracle LM, so that the yardsticks are trusted before they judge a kernel."""
+"""Plain fp64 CPU references of the kernels checked by test_kernel_edges_gpu.py and test_kernel_epilogues_gpu.py.
+test_kernel_refs_cpu.py checks them against torch's scaled_dot_product_attention, F.conv1d and activations, the oracle LM and the
+oracle conformer layer, so that the yardsticks are trusted before they judge a kernel."""
+import math
+
 import torch
 
 from oracle import lm as olm
@@ -12,6 +15,16 @@ QKV_N = (NH + 2 * NKV) * HD                 # 1152
 def bf16(x):
     """round to bf16 (nearest even), returned in x's dtype"""
     return x.to(torch.bfloat16).to(x.dtype)
+
+
+def f16(x):
+    """round to IEEE half (nearest even) with the kernels' saturation at +-65504 (common.cuh from_f32<__half>), in x's dtype"""
+    return x.clamp(-65504.0, 65504.0).to(torch.float16).to(x.dtype)
+
+
+def round_to(x, dtype):
+    """x rounded to a storage dtype of the conv-GEMM ("fp32", "bf16" or "fp16"), in x's dtype"""
+    return {"fp32": lambda t: t.float().to(t.dtype), "bf16": bf16, "fp16": f16}[dtype](x)
 
 
 def bf16_ulp(x):
@@ -89,3 +102,93 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, ctx_len):
         s = (q[b].double()[:, None, :] @ kk.transpose(1, 2))[:, 0] * 0.125                 # [14, L+1]
         out[b] = (torch.softmax(s, -1)[:, None, :] @ vv)[:, 0].reshape(-1)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ conv-GEMM and its epilogue
+def act(name, x, param=0.0, alpha=None):
+    """the epilogue activations in x's dtype, written from their definitions: GELU with erf, GELU's tanh form
+    (F.gelu(approximate='tanh')), SiLU, Mish, ELU (alpha 1), leaky ReLU (slope param), Snake x + sin^2(a x) / (a + 1e-9) with a per
+    column (alpha [N], 1 when None; oracle/hift.py snake), tanh, |x|"""
+    if name == "none":
+        return x
+    if name == "gelu":
+        return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+    if name == "gelu_tanh":
+        return 0.5 * x * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x ** 3)))
+    if name == "silu":
+        return x / (1.0 + torch.exp(-x))
+    if name == "mish":
+        return x * torch.tanh(torch.log1p(torch.exp(x.clamp(max=40.0))))     # tanh(softplus(x)) == 1 in fp64 from x = 20 on
+    if name == "elu":
+        return torch.where(x > 0, x, torch.expm1(x))
+    if name == "lrelu":
+        return torch.where(x > 0, x, x * param)
+    if name == "snake":
+        a = torch.ones_like(x[0]) if alpha is None else alpha.to(x.dtype)
+        return x + torch.sin(a * x) ** 2 / (a + 1e-9)
+    if name == "tanh":
+        return torch.tanh(x)
+    if name == "abs":
+        return x.abs()
+    raise ValueError(name)
+
+
+def conv_rows(x, w, dil=1, shift0=0):
+    """the conv-GEMM product on a packed matrix in fp64: acc[r, n] = sum_j sum_k x[r + shift0 + j*dil, k] w[n, k, j], rows outside
+    [0, rows) read as zero.  x [rows, K], w a torch Conv1d weight [N, K, taps] (on x's device)."""
+    x, w = x.double(), w.double()
+    rows = x.shape[0]
+    N, K, taps = w.shape
+    acc = torch.zeros(rows, N, dtype=torch.float64, device=x.device)
+    for j in range(taps):
+        s = shift0 + j * dil
+        lo, hi = max(0, -s), min(rows, rows - s)          # output rows whose input row r + s lies inside the matrix
+        if lo < hi:
+            acc[lo:hi] += x[lo + s:hi + s] @ w[:, :, j].t()
+    return acc
+
+
+def conv_epilogue(acc, valid, bias=None, act1="none", act1_param=0.0, alpha1=None, resid=None, out_init=None, accumulate=False,
+                  act2=None, act2_param=0.0, alpha2=None):
+    """the fused epilogue of the conv-GEMM (struct Epilogue, cvk_internal.h) in fp64, in its order:
+      v = act1(acc + bias) (+ resid);  v = 0 on invalid rows;  out = out_init + v if accumulate else v;
+      out2 = act2(out) on valid rows (applied to the unrounded value), 0 on invalid rows.
+    acc [rows, N], valid [rows] bool, bias / alpha [N], resid / out_init [rows, N].  Returns (out, out2 or None)."""
+    v = acc.double() + (bias.double()[None] if bias is not None else 0.0)
+    v = act(act1, v, act1_param, alpha1)
+    if resid is not None:
+        v = v + resid.double()
+    v = torch.where(valid[:, None], v, 0.0)
+    if accumulate:
+        v = out_init.double() + v
+    out2 = None
+    if act2 is not None:
+        out2 = torch.where(valid[:, None], act(act2, v, act2_param, alpha2), 0.0)
+    return v, out2
+
+
+# ------------------------------------------------------------------------------------------------ relative-position attention
+def rel_shift(x):
+    """the reference conformer's rel_shift (transformer/attention.py:225-247, oracle/flow.py _rel_shift) on [H, t, 2t-1] -> [H, t, t]"""
+    h, t, n = x.shape
+    xp = torch.cat([x.new_zeros(h, t, 1), x], -1).view(h, n + 1, t)
+    return xp[:, 1:].reshape(h, t, n)[:, :, : n // 2 + 1]
+
+
+def relpos_attention(q, k, v, pos, center, bias_u, bias_v, lens, H, chunk, scale):
+    """cvk_op_relpos_attention in fp64, computed the way the reference conformer layer does (oracle/flow.py _enc_layer):
+    ac = (q + u) k^T, bd = rel_shift((q + v) p^T), softmax((ac + bd) * scale) over the visible keys, times v.  A sequence of length L
+    uses the 2L-1 central rows of the table, center - (L-1) .. center + (L-1) (relative positions L-1 .. -(L-1)), which is the table
+    the reference builds for it.  q, k, v [sum lens, H*64], pos [2*center+1, H*64], bias_u / bias_v [H*64]."""
+    q, k, v, pos = (t.double() for t in (q, k, v, pos))
+    u, vb = bias_u.double().view(H, 1, HD), bias_v.double().view(H, 1, HD)
+    outs, o = [], 0
+    for L in lens:
+        qq, kk, vv = (t[o:o + L].view(L, H, HD).transpose(0, 1) for t in (q, k, v))
+        pp = pos[center - (L - 1):center + L].view(2 * L - 1, H, HD).transpose(0, 1)
+        ac = (qq + u) @ kk.transpose(1, 2)
+        bd = rel_shift((qq + vb) @ pp.transpose(1, 2))
+        s = ((ac + bd) * scale).masked_fill(~visible(L, L, 0, chunk)[None], float("-inf"))
+        outs.append((torch.softmax(s, -1) @ vv).transpose(0, 1).reshape(L, H * HD))
+        o += L
+    return torch.cat(outs, 0)

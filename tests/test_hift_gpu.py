@@ -75,6 +75,26 @@ def test_inference_ragged_batch_vs_oracle(precision, sd):
     assert wav.abs().max().item() <= 0.99 + 1e-6
 
 
+def test_inference_cuda_cores_in_bf16_context(sd):
+    """use_tc 0 (the A/B switch to the CUDA-core conv-GEMM) in a bf16 context: the vocoder's IEEE-half operands and half weight copies
+    run on the CUDA cores and give the default (wgmma) run's waveform within the bf16-mode bound above"""
+    c = model("bf16", sd)
+    lens = [17, 40]
+    g = torch.Generator().manual_seed(78)
+    mel_tm = torch.randn(sum(lens), 80, generator=g) * 2 - 5
+    noise = torch.randn(sum(lens) * 480, 9, generator=g)
+    wav_tc, src_tc = c.hift_inference(mel_tm, lens, noise)
+    c.set_option("use_tc", 0)
+    try:
+        wav_cc, src_cc = c.hift_inference(mel_tm, lens, noise)
+    finally:
+        c.set_option("use_tc", 1)
+    d = maxdiff(wav_cc, wav_tc)
+    print(f"[hift inference, bf16 context, CUDA cores vs wgmma] max |d| {d:.3g}")
+    assert maxdiff(src_cc, src_tc) < 2e-3       # the source path runs fp32 in both
+    assert d < 4e-3, d
+
+
 def test_cache_source_golden(sd, golden):
     g = golden("hift_cache_source")
     melx, noise, _ = cases.hift_case()

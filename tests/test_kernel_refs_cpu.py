@@ -1,11 +1,12 @@
-"""CPU: the fp64 references of test_kernel_edges_gpu.py (tests/kernel_refs.py) against independent formulations - torch's
-scaled_dot_product_attention with an explicit mask and expanded K/V heads, and one KV-cached step of the oracle Qwen2 LM."""
+"""CPU: the fp64 references of test_kernel_edges_gpu.py and test_kernel_epilogues_gpu.py (tests/kernel_refs.py) against independent
+formulations - torch's scaled_dot_product_attention with an explicit mask and expanded K/V heads, one KV-cached step of the oracle
+Qwen2 LM, F.conv1d with torch's activations, and the oracle conformer layer's relative-position attention."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 import kernel_refs as kr
-from oracle import lm as olm
+from oracle import flow as oflow, hift as ohift, lm as olm
 
 
 @pytest.mark.parametrize("H,kvh,chunk", [(14, 2, 1), (8, 8, 50), (16, 16, 0), (14, 2, 25)])
@@ -98,3 +99,103 @@ def test_bf16_helpers():
     x = torch.tensor([1.0, 1.0 + 2 ** -8, 1.0 + 2 ** -9, -3.0, 1e-3], dtype=torch.float64)
     assert torch.equal(kr.bf16_ulp(x), torch.tensor([2 ** -7, 2 ** -7, 2 ** -7, 2 ** -6, 2.0 ** (-10 - 7)], dtype=torch.float64))
     assert kr.near_bf16_tie(x, 1e-12).tolist() == [False, True, False, False, False]     # 1 + 2^-8 is a midpoint
+
+
+TORCH_ACTS = {
+    "none": lambda x, a: x,
+    "gelu": lambda x, a: F.gelu(x),
+    "gelu_tanh": lambda x, a: F.gelu(x, approximate="tanh"),
+    "silu": lambda x, a: F.silu(x),
+    "mish": lambda x, a: F.mish(x),
+    "elu": lambda x, a: F.elu(x),
+    "lrelu": lambda x, a: F.leaky_relu(x, 0.1),
+    "snake": lambda x, a: ohift.snake(x.t()[None], a)[0].t(),       # oracle vocoder Snake, channel-major
+    "tanh": lambda x, a: torch.tanh(x),
+    "abs": lambda x, a: x.abs(),
+}
+
+
+@pytest.mark.parametrize("act", list(TORCH_ACTS))
+@pytest.mark.parametrize("taps,dil,shift0", [(1, 1, 0), (3, 1, -1), (7, 3, -9), (31, 1, -30)])
+def test_conv_ref_equals_conv1d(taps, dil, shift0, act):
+    """conv_rows + conv_epilogue on a packed matrix with gap rows == per-sequence F.conv1d (zero padding) + the torch activation;
+    resid, accumulate and the second output follow the epilogue order"""
+    g = torch.Generator().manual_seed(taps * 31 + dil)
+    K, N = 12, 10
+    lens, gap = [17, 1, 40], max(-shift0, shift0 + (taps - 1) * dil)
+    starts, r = [], gap
+    for L in lens:
+        starts.append(r)
+        r += L + gap
+    rows = r
+    x = torch.zeros(rows, K, dtype=torch.float64)
+    valid = torch.zeros(rows, dtype=torch.bool)
+    for s, L in zip(starts, lens):
+        x[s:s + L] = torch.randn(L, K, generator=g, dtype=torch.float64) * 2
+        valid[s:s + L] = True
+    w = torch.randn(N, K, taps, generator=g, dtype=torch.float64) * (K * taps) ** -0.5
+    bias = torch.randn(N, generator=g, dtype=torch.float64)
+    alpha = torch.rand(N, generator=g, dtype=torch.float64) * 2 + 0.2
+    resid = torch.randn(rows, N, generator=g, dtype=torch.float64)
+    init = torch.randn(rows, N, generator=g, dtype=torch.float64)
+    acc = kr.conv_rows(x, w, dil, shift0)
+    out, out2 = kr.conv_epilogue(acc, valid, bias, act, 0.1, alpha, resid=resid, out_init=init, accumulate=True, act2=act,
+                                 act2_param=0.1, alpha2=alpha.flip(0))
+    plain, _ = kr.conv_epilogue(acc, valid, bias, act, 0.1, alpha)
+    for s, L in zip(starts, lens):
+        xs = x[s:s + L].t()[None]
+        y = F.conv1d(F.pad(xs, (-shift0, shift0 + (taps - 1) * dil)), w, bias, dilation=dil)[0].t()
+        y = TORCH_ACTS[act](y, alpha)
+        assert (plain[s:s + L] - y).abs().max().item() < 1e-12
+        v = init[s:s + L] + y + resid[s:s + L]
+        assert (out[s:s + L] - v).abs().max().item() < 1e-12
+        assert (out2[s:s + L] - TORCH_ACTS[act](v, alpha.flip(0))).abs().max().item() < 1e-12
+    # gap rows: no output (the accumulate input comes back unchanged), no second output, whatever resid holds there
+    assert torch.equal(plain[~valid], torch.zeros_like(plain[~valid]))
+    assert torch.equal(out[~valid], init[~valid]) and torch.equal(out2[~valid], torch.zeros_like(out2[~valid]))
+
+
+def _oracle_enc_layer_attention(x, qkv_w, qkv_b, pos_emb, u, v, chunk):
+    """the attention term of oracle.flow._enc_layer: with linear_out = I, linear_pos = I and a zero feed-forward output the layer
+    returns x + attention(x)"""
+    D, H = oflow.D_ENC, oflow.H_ENC
+    p, a = "L", "L.self_attn"
+    sd = {p + ".norm_mha.weight": torch.ones(D), p + ".norm_mha.bias": torch.zeros(D),
+          p + ".norm_ff.weight": torch.ones(D), p + ".norm_ff.bias": torch.zeros(D),
+          a + ".linear_out.weight": torch.eye(D), a + ".linear_out.bias": torch.zeros(D), a + ".linear_pos.weight": torch.eye(D),
+          a + ".pos_bias_u": u.view(H, 64), a + ".pos_bias_v": v.view(H, 64),
+          p + ".feed_forward.w_1.weight": torch.zeros(4, D), p + ".feed_forward.w_1.bias": torch.zeros(4),
+          p + ".feed_forward.w_2.weight": torch.zeros(D, 4), p + ".feed_forward.w_2.bias": torch.zeros(D)}
+    for i, n in enumerate("qkv"):
+        sd[f"{a}.linear_{n}.weight"] = qkv_w[i]
+        sd[f"{a}.linear_{n}.bias"] = qkv_b[i]
+    T = x.shape[0]
+    mask = oflow.chunk_attention_mask(T, chunk).unsqueeze(0)
+    return oflow._enc_layer(sd, p, x[None], mask, pos_emb[None])[0] - x
+
+
+@pytest.mark.parametrize("chunk", [0, 25])
+@pytest.mark.parametrize("extra", [0, 37])
+def test_relpos_ref_equals_oracle_layer(extra, chunk):
+    """kr.relpos_attention == the oracle conformer layer's attention for one sequence of length L, with the table the oracle builds
+    (center = L-1) and with a larger table (center = L-1+extra) whose central 2L-1 rows are the oracle's"""
+    D, H = oflow.D_ENC, oflow.H_ENC
+    g = torch.Generator().manual_seed(extra + chunk)
+    L = 70
+    x = torch.randn(L, D, generator=g)
+    qkv_w = torch.randn(3, D, D, generator=g) * D ** -0.5
+    qkv_b = torch.randn(3, D, generator=g) * 0.1
+    u, v = torch.randn(D, generator=g) * 0.5, torch.randn(D, generator=g) * 0.5
+    center = L - 1 + extra
+    pos = torch.randn(2 * center + 1, D, generator=g)
+    att = _oracle_enc_layer_attention(x, qkv_w, qkv_b, pos[extra:extra + 2 * L - 1], u, v, chunk)
+    xn = F.layer_norm(x, (D,), torch.ones(D), torch.zeros(D), 1e-12)
+    q, k, vv = (F.linear(xn, qkv_w[i], qkv_b[i]) for i in range(3))
+    ref = kr.relpos_attention(q, k, vv, pos, center, u, v, [L], H, chunk, 0.125)
+    # the oracle runs in fp32: its scores (|s| ~ 10) carry ~1e-6 absolute rounding, the output ~1e-6 relative
+    assert (att.double() - ref).abs().max().item() < 1e-4
+
+
+def test_f16_rounding_saturates():
+    x = torch.tensor([1.0, 1.0 + 2 ** -11, 65504.0, 65519.0, 1e6, -1e6, 2.0 ** -25], dtype=torch.float64)
+    assert kr.f16(x).tolist() == [1.0, 1.0, 65504.0, 65504.0, 65504.0, -65504.0, 0.0]
