@@ -9,8 +9,9 @@ normalisation, no tokenizer (those stay with the reference's frontend and server
 ``model.tts``).
 
 Admission policy: a batch is closed when ``max_batch`` requests are waiting or ``max_wait_ms`` have passed since the first one
-arrived; requests are never reordered inside a batch (the model's RNG streams are consumed in input order, so a fixed arrival
-order gives fixed results).  One worker thread owns the model; ``tts_batch`` itself is ragged, so no padding or bucketing is
+arrived.  Requests that were queued while the previous batch ran (a backlog) have already waited through that batch: the next batch
+takes them at once, up to ``max_batch``, instead of holding a partial remainder for the wait budget.  Requests are never reordered
+inside a batch (the model's RNG streams are consumed in input order, so a fixed arrival order gives fixed results).  One worker thread owns the model; ``tts_batch`` itself is ragged, so no padding or bucketing is
 needed here.
 
 Streaming requests (``submit_stream`` / ``submit_stream_pcm``) are served by ``tts_stream_batch``, which hands out every request's
@@ -127,12 +128,14 @@ class TtsBatcher:
 
     # ------------------------------------------------------------------ worker
     def _take_batch(self):
+        free_at = time.monotonic()         # the previous batch (if any) has just finished
         with self._cv:
             while not self._q and not self._closed:
                 self._cv.wait()
             if not self._q:
                 return None
-            deadline = self._q[0][3] + self.max_wait
+            # a head queued while the previous batch ran is a backlog: no further wait for company
+            deadline = self._q[0][3] + self.max_wait if self._q[0][3] >= free_at else free_at
             while self._run_length() < self.max_batch and self._run_length() == len(self._q) and not self._closed:
                 left = deadline - time.monotonic()
                 if left <= 0:

@@ -45,6 +45,10 @@ void llm_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* hist
                     const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, cudaStream_t st);
 void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
                              const int* ctx_len_host, int max_ctx, float* out, cudaStream_t st);
+void llm_sample_step_op(cvk_ctx* ctx, float* logits, int B, int V, const float* uniforms, const int32_t* min_len, const int32_t* max_len,
+                        int32_t* out_ids, int out_ld, int32_t* out_count, int32_t* done, int* ctx_len, const int* base_len, int* live,
+                        const float* speech_emb, float* next_x, const float* gamma, float* xn, cudaStream_t st);
+void llm_log_softmax_op(cvk_ctx* ctx, float* x, int rows, int V, cudaStream_t st);
 void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int fmax_hz, float* mel, cudaStream_t st);
 void mel_init(cvk_ctx* ctx);
 void prompt_feat_init(cvk_ctx* ctx);
@@ -731,8 +735,35 @@ int cvk_lm_last_logits(cvk_ctx* ctx, cvk_lm_session* s, float* logits, void* str
 int cvk_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* history, int hist_ld, const int32_t* hist_count,
                    const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, void* stream) {
   CVK_API_BEGIN
-  CVK_REQUIRE(logp && history && hist_count && uniforms && ignore_eos && out_ids && B > 0 && V > 0, "cvk_ras_sample: bad arguments");
+  CVK_REQUIRE(logp && history && hist_count && uniforms && ignore_eos && out_ids && B > 0 && V > 0 && hist_ld >= 0,
+              "cvk_ras_sample: bad arguments");
   llm_ras_sample(ctx, logp, B, V, history, hist_ld, hist_count, uniforms, ignore_eos, out_ids, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_op_sample_step(cvk_ctx* ctx, float* logits, int B, int V, const float* uniforms, int steps, const int32_t* min_len,
+                       const int32_t* max_len, int32_t* out_ids, int out_ld, int32_t* out_count, int32_t* done, int* ctx_len,
+                       const int* base_len, int* live, const float* speech_emb, float* next_x, const float* gamma, float* xn, void* stream) {
+  CVK_API_BEGIN
+  cudaStream_t st = (cudaStream_t)stream;
+  CVK_REQUIRE(logits && uniforms && min_len && max_len && out_ids && out_count && done && ctx_len && base_len && live && speech_emb &&
+                  next_x && !gamma == !xn && B >= 1 && steps >= 1 && out_ld >= 1,
+              "cvk_op_sample_step: bad arguments");
+  CVK_REQUIRE(V >= 6564 && V <= 6912, "cvk_op_sample_step: vocabulary size out of range (6564 .. 6912 supported)");
+  // a live row reads uniforms[count] and, unless it stops, writes out_ids[count]: both must lie inside the caller's buffers
+  std::vector<int32_t> cnt(B), dn(B);
+  CVK_CHECK_CUDA(cudaMemcpyAsync(cnt.data(), out_count, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+  CVK_CHECK_CUDA(cudaMemcpyAsync(dn.data(), done, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+  CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b)
+    CVK_REQUIRE(dn[b] || (cnt[b] >= 0 && cnt[b] < steps && cnt[b] < out_ld), "cvk_op_sample_step: a live row's count is outside [0, min(steps, out_ld))");
+  llm_sample_step_op(ctx, logits, B, V, uniforms, min_len, max_len, out_ids, out_ld, out_count, done, ctx_len, base_len, live, speech_emb,
+                     next_x, gamma, xn, st);
+  CVK_API_END
+}
+int cvk_op_log_softmax(cvk_ctx* ctx, float* x, int rows, int V, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(x && rows >= 1 && V >= 1, "cvk_op_log_softmax: bad arguments");
+  llm_log_softmax_op(ctx, x, rows, V, (cudaStream_t)stream);
   CVK_API_END
 }
 

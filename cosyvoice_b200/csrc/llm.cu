@@ -615,23 +615,26 @@ ras_sampler_kernel(float* __restrict__ scores, int V, int from_logits, const flo
       float thr = u2 * pre;
       float acc = 0.f;
       int segi = -1, lastseg = -1;
-      float segbase = 0.f;
+      float segbase = 0.f, lastbase = 0.f;
       for (int i = 0; i < SAMPLER_THREADS; ++i) {
         if (part[i] > 0.f) {
           lastseg = i;
+          lastbase = acc;
           if (acc + part[i] > thr) { segi = i; segbase = acc; break; }
         }
         acc += part[i];
       }
-      // walk (the oracle keeps scanning later segments if rounding leaves the chosen one without a hit)
+      // walk (the oracle keeps scanning later segments if rounding leaves the chosen one without a hit).  Every segment the walk
+      // enters starts from its own prefix sum, as draw_index does: the element-by-element running sum can end a few ulps below the
+      // segment prefix, and carried over it would let a tiny first entry of the next segment fail the threshold.
       int pick = -1, last = -1;
-      if (segi < 0) segi = lastseg;
-      float a = segbase;
-      for (int sg = segi; sg < SAMPLER_THREADS && pick < 0; ++sg) {
-        if (sg > segi) {
-          if (!(part[sg] > 0.f)) continue;
-          // prefix[sg+1] > thr holds trivially once an earlier segment already exceeded it
-        }
+      if (segi < 0) { segi = lastseg; segbase = lastbase; }
+      float sgbase = segbase;              // prefix sum of segment sg (part[] summed in order)
+      for (int sg = segi; sg >= 0 && sg < SAMPLER_THREADS && pick < 0; ++sg) {
+        const float a0 = sgbase;
+        sgbase += part[sg];
+        if (sg > segi && !(part[sg] > 0.f)) continue;   // prefix[sg+1] > thr holds once an earlier segment exceeded it
+        float a = a0;
         int l2 = sg * per, h2 = min(l2 + per, V);
         for (int i = l2; i < h2; ++i) {
           if (sp[i] > 0.f) last = i;
@@ -1341,6 +1344,35 @@ void llm_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* hist
   ras_sampler_kernel<<<B, SAMPLER_THREADS, sampler_smem(V), st>>>(logp, V, 0, uniforms, B, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
                                                                     nullptr, nullptr, nullptr, nullptr, history, hist_ld, hist_count, ignore_eos,
                                                                     out_ids, nullptr, nullptr, nullptr, nullptr);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+}
+
+// One decode-graph sampler step on caller data, without a loaded LM (cvk_op_sample_step): the kernel the decode step launches,
+// with from_logits = 1 and the caller's state buffers.  With gamma, the fused layer-0 RMSNorm goes to a bf16 copy of xn that is
+// widened back into the caller's fp32 xn (rows the kernel does not write come back rounded to bf16).
+void llm_sample_step_op(cvk_ctx* ctx, float* logits, int B, int V, const float* uniforms, const int32_t* min_len, const int32_t* max_len,
+                        int32_t* out_ids, int out_ld, int32_t* out_count, int32_t* done, int* ctx_len, const int* base_len, int* live,
+                        const float* speech_emb, float* next_x, const float* gamma, float* xn, cudaStream_t st) {
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(ras_sampler_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sampler_smem(V > VOUT3_PAD ? V : VOUT3_PAD)));   // per function, never lowered
+  ctx->arena.reset();
+  Mat xn16;
+  if (gamma) {
+    xn16 = arena_mat(ctx, DT_BF16, B, D, D);
+    convert_mat(ctx, st, Mat(xn, DT_F32, B, D, D), xn16);
+  }
+  ras_sampler_kernel<<<B, SAMPLER_THREADS, sampler_smem(V), st>>>(logits, V, 1, uniforms, B, min_len, max_len, out_ids, out_ld, out_count,
+                                                                    done, ctx_len, base_len, live, speech_emb, next_x, nullptr, 0, nullptr,
+                                                                    nullptr, nullptr, gamma, gamma ? xn16.b16() : nullptr, nullptr, nullptr);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+  if (gamma) convert_mat(ctx, st, xn16, Mat(xn, DT_F32, B, D, D));
+}
+
+// log_softmax of rows [rows][V] in place with the kernel of cvk_lm_next_logp / cvk_lm_forward_logp (cvk_op_log_softmax)
+void llm_log_softmax_op(cvk_ctx* ctx, float* x, int rows, int V, cudaStream_t st) {
+  logsoftmax_rows_kernel<<<rows, SAMPLER_THREADS, 0, st>>>(x, V);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }

@@ -88,6 +88,9 @@ SIGNATURES = {
     "cvk_lm_feed": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp]),
     "cvk_lm_next_logp": (ctypes.c_int, [_vp, _vp, _vp, _vp]),
     "cvk_ras_sample": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "cvk_op_sample_step": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                          _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cvk_op_log_softmax": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp]),
     "cvk_mel_spectrogram": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_mel_spectrogram_ex": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_whisper_log_mel": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
@@ -520,6 +523,8 @@ class Context:
         return out
 
     def lm_last_logits(self, sess, B):
+        """the row the last decode step sampled from: log-probs with the sampler's -inf marks (masked eos, repeated id of a
+        fallback draw); rows done before that step hold the raw head logits"""
         out = torch.empty(B, self.lm_vocab(), device=self.device)
         self._check(self.lib.cvk_lm_last_logits(self.h, sess, _ptr(out), _stream()))
         return out
@@ -534,6 +539,23 @@ class Context:
         self._check(self.lib.cvk_ras_sample(self.h, _ptr(logp), logp.shape[0], logp.shape[1], _ptr(history), history.shape[1],
                                             _ptr(hist_count), _ptr(uniforms), _ptr(ignore_eos), _ptr(out), _stream()))
         return out
+
+    def sample_step(self, logits, uniforms, min_len, max_len, out_ids, out_count, done, ctx_len, base_len, live, speech_emb, next_x,
+                    gamma=None, xn=None):
+        """one decode-graph sampler step (cvk_op_sample_step) on device tensors, updated in place: logits [B,V] fp32, uniforms
+        [steps,B,2] fp32, min_len / max_len / out_count / done / ctx_len / base_len [B] int32, out_ids [B,out_ld] int32, live [1] int32,
+        speech_emb [V,896], next_x [B,896] fp32; gamma [896] and xn [B,896] fp32 both or neither (fused layer-0 RMSNorm)."""
+        B, V = logits.shape
+        self._check(self.lib.cvk_op_sample_step(
+            self.h, _ptr(logits), B, V, _ptr(uniforms), uniforms.shape[0], _ptr(min_len), _ptr(max_len), _ptr(out_ids), out_ids.shape[1],
+            _ptr(out_count), _ptr(done), _ptr(ctx_len), _ptr(base_len), _ptr(live), _ptr(speech_emb), _ptr(next_x), _ptr(gamma), _ptr(xn),
+            _stream()))
+
+    def log_softmax(self, x):
+        """log_softmax of every row of x [rows, V] with the LM's log-prob kernel (cvk_op_log_softmax); returns a new tensor"""
+        x = _f32(x, self.device).clone()
+        self._check(self.lib.cvk_op_log_softmax(self.h, _ptr(x), x.shape[0], x.shape[1], _stream()))
+        return x
 
     # ------------------------------------------------------------------ mel
     def whisper_log_mel(self, wav, lens):

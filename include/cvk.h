@@ -296,13 +296,30 @@ int cvk_lm_vocab(cvk_ctx* ctx);
 int cvk_lm_begin(cvk_ctx* ctx, cvk_lm_session* s, int B, void* stream);
 int cvk_lm_feed(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* ids_host, const int32_t* kinds_host, int n, void* stream);
 int cvk_lm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, void* stream);
-/* parity tests: the head logits [B][V] (llm_decoder output, llm.py:542, before log_softmax) that the most recent decode step
- * sampled from, copied to `logits` (device) */
+/* parity tests: the row the most recent decode step sampled from, copied to `logits` [B][V] (device): the log-probs
+ * log_softmax(llm_decoder output) (llm.py:542) with the sampler's in-place marks, -inf at the eos id while it was masked (min_len) and
+ * at the repeated id when the repetition fallback fired.  Rows already done before that step are not sampled and hold the raw head
+ * logits. */
 int cvk_lm_last_logits(cvk_ctx* ctx, cvk_lm_session* s, float* logits, void* stream);
 /* utils/common.py:138-167 + llm.py:150-160 as one kernel.  logp [B,V] (modified in place like the reference),
- * history [B, hist_ld] with hist_count [B] valid entries, uniforms [B,2], ignore_eos [B]; out ids [B]. */
+ * history [B, hist_ld] (hist_ld >= 0) with hist_count [B] valid entries, uniforms [B,2], ignore_eos [B]; out ids [B]; 6564 <= V <= 6912. */
 int cvk_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* history, int hist_ld, const int32_t* hist_count,
                    const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, void* stream);
+/* One decode-graph sampler step on caller data, without a loaded LM (tests): the kernel cvk_lm_decode runs after the head, with
+ * log_softmax of the logits first.  All pointers are device memory.  logits [B][V] in / out (receives the log-probs with the sampler's
+ * -inf marks, as cvk_lm_last_logits shows them); uniforms [steps][B][2] indexed by each row's count; min_len, max_len [B]; out_ids
+ * [B][out_ld], out_count [B], done [B], ctx_len [B] (= base_len + count after an accepted id), base_len [B], live [1] as in a session.
+ * A row with done != 0 is skipped.  speech_emb [V][896] fp32; next_x [B][896] receives the embedding row of an accepted id.  gamma [896]
+ * or NULL: with gamma, xn [B][896] fp32 in / out receives RMSNorm(next_x) * gamma as the bf16 the decode step stores (rows the kernel
+ * does not write come back rounded to bf16); gamma and xn are both NULL or both given.  Requires 6564 <= V <= 6912, B >= 1,
+ * steps >= 1, out_ld >= 1 and, for every row not done, 0 <= count < min(steps, out_ld) (read back before the launch).  Any other
+ * argument is refused with CVK_ERR_INVALID before the sampler runs.  Either precision of context. */
+int cvk_op_sample_step(cvk_ctx* ctx, float* logits, int B, int V, const float* uniforms, int steps, const int32_t* min_len,
+                       const int32_t* max_len, int32_t* out_ids, int out_ld, int32_t* out_count, int32_t* done, int* ctx_len,
+                       const int* base_len, int* live, const float* speech_emb, float* next_x, const float* gamma, float* xn, void* stream);
+/* x [rows][V] (device) <- log_softmax(x) per row, in place, with the kernel of cvk_lm_next_logp / cvk_lm_forward_logp (tests):
+ * (x - max) - log(sum exp(x - max)), the sum in the sampler's segment order.  rows, V >= 1. */
+int cvk_op_log_softmax(cvk_ctx* ctx, float* x, int rows, int V, void* stream);
 
 /* ---------------------------------------------------------------------------------------------- mel frontend
  * replaces third_party/Matcha-TTS/matcha/utils/audio.py:45-82 with cosyvoice2.yaml:150-158 parameters (n_fft 1920, hop 480,
