@@ -41,6 +41,11 @@ int llm_vocab(cvk_ctx* ctx);
 void llm_session_begin(cvk_ctx* ctx, cvk_lm_session* s, int B, cudaStream_t st);
 void llm_feed(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* ids, const int32_t* kinds, int n, cudaStream_t st);
 void llm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, cudaStream_t st);
+void llm_feed_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows, const int* counts, const int32_t* ids, const int32_t* kinds,
+                   cudaStream_t st);
+void llm_ragged_attention_op(cvk_ctx* ctx, const float* q, const float* k_cache, const float* v_cache, int cache_rows, int max_ctx,
+                             const int* rowpos, int M, float* out, cudaStream_t st);
+void llm_next_logp_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows, float* logp, cudaStream_t st);
 void llm_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* history, int hist_ld, const int32_t* hist_count,
                     const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, cudaStream_t st);
 void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
@@ -392,6 +397,15 @@ int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int 
   CVK_API_END
 }
 
+int cvk_op_ragged_attention(cvk_ctx* ctx, const float* q, const float* k_cache, const float* v_cache, int cache_rows, int max_ctx,
+                            const int* rowpos_host, int M, float* out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(q && k_cache && v_cache && rowpos_host && out && M >= 1 && cache_rows >= 1 && max_ctx >= 1 && ctx->precision == CVK_PREC_BF16,
+              "cvk_op_ragged_attention: bad arguments (bf16 context)");
+  llm_ragged_attention_op(ctx, q, k_cache, v_cache, cache_rows, max_ctx, rowpos_host, M, out, (cudaStream_t)stream);
+  CVK_API_END
+}
+
 int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, int operand, const int* seq_start, const int* seq_len, int B,
                      const float* w, const float* bias, int N, int taps, int dil, int shift0, int act1, float act1_param, const float* alpha1,
                      const float* resid, int resid_ld, int resid_is_out, int accumulate, float* out, int out_dtype, int out_ld, int act2,
@@ -724,6 +738,19 @@ int cvk_lm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, void* stream)
   CVK_API_BEGIN
   CVK_REQUIRE(s && logp, "cvk_lm_next_logp: bad arguments");
   llm_next_logp(ctx, s, logp, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_lm_feed_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows_host, const int* counts_host, const int32_t* ids_host,
+                     const int32_t* kinds_host, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(s && rows_host && counts_host && ids_host && kinds_host, "cvk_lm_feed_rows: bad arguments");
+  llm_feed_rows(ctx, s, n_rows, rows_host, counts_host, ids_host, kinds_host, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_lm_next_logp_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows_host, float* logp, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(s && rows_host && logp, "cvk_lm_next_logp_rows: bad arguments");
+  llm_next_logp_rows(ctx, s, n_rows, rows_host, logp, (cudaStream_t)stream);
   CVK_API_END
 }
 int cvk_lm_last_logits(cvk_ctx* ctx, cvk_lm_session* s, float* logits, void* stream) {

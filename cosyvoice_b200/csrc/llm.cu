@@ -12,6 +12,7 @@
 // number of live rows every few steps - no .item() style host round trip per token (common.py:155-161 has several).
 #include "llm_decode_attn.cuh"
 #include <math.h>
+#include <algorithm>
 
 using namespace lm;
 
@@ -68,16 +69,19 @@ __global__ void build_input_kernel(const int32_t* __restrict__ text, const int* 
 }
 
 // half-split RoPE (modeling_qwen2.py rotate_half) on the q and k parts of a fused qkv row, in place; position =
-// pos0[seq] + t.  Also appends k, v to the cache at that position.
+// pos0[seq] + t.  Also appends k, v to the cache at that position.  With rowpos (ragged feed, rows_are_seqs = 1): qkv row
+// blockIdx.y goes to cache row rowpos[.].x at position rowpos[.].y.
 template <typename T>
 __global__ void rope_append_kernel(T* __restrict__ qkv, int ld, const int* __restrict__ start, const int* __restrict__ len,
                                    const int* __restrict__ pos0, const float* __restrict__ inv_freq, T* __restrict__ kc, T* __restrict__ vc,
-                                   int max_ctx, int rows_are_seqs) {
+                                   int max_ctx, int rows_are_seqs, const int2* __restrict__ rowpos) {
   int b = blockIdx.y;
   int L = rows_are_seqs ? 1 : len[b];
   int base = rows_are_seqs ? b : start[b];
+  const int cb = rowpos ? rowpos[b].x : b;
+  const int p0 = rowpos ? rowpos[b].y : (pos0 ? pos0[b] : 0);
   for (int t = blockIdx.x; t < L; t += gridDim.x) {
-    int pos = (pos0 ? pos0[b] : 0) + t;
+    int pos = p0 + t;
     T* row = qkv + (size_t)(base + t) * ld;
     // 16 heads to rotate (14 q + 2 k), 32 pairs each
     for (int e = threadIdx.x; e < (NH + NKV) * (HD / 2); e += blockDim.x) {
@@ -93,7 +97,7 @@ __global__ void rope_append_kernel(T* __restrict__ qkv, int ld, const int* __res
     if (pos < max_ctx) {
       for (int e = threadIdx.x; e < NKV * HD; e += blockDim.x) {
         int h = e / HD, d = e % HD;
-        size_t ci = (((size_t)b * NKV + h) * max_ctx + pos) * HD + d;
+        size_t ci = (((size_t)cb * NKV + h) * max_ctx + pos) * HD + d;
         kc[ci] = row[NH * HD + e];
         vc[ci] = row[NH * HD + NKV * HD + e];
       }
@@ -104,20 +108,22 @@ __global__ void rope_append_kernel(T* __restrict__ qkv, int ld, const int* __res
 
 // decode attention: one CTA per (row, kv head), one warp per query head of the group (7 warps).  Phase A: one key per
 // lane (full 64-dim dot product from a 128-byte cache row), scores to shared memory; softmax over the warp; phase B: one
-// pair of output dims per lane, keys streamed with coalesced 128-byte rows.  Keys 0..ctx_len[b] (new token included).
+// pair of output dims per lane, keys streamed with coalesced 128-byte rows.  Keys 0..ctx_len[b] (new token included).  With
+// rowpos (ragged feed): query row b reads cache row rowpos[b].x, keys 0..rowpos[b].y.
 template <typename T>
 __global__ void __launch_bounds__((NH / NKV) * 32)
 decode_attn_kernel(const T* __restrict__ qkv, int ld, const T* __restrict__ kc, const T* __restrict__ vc,
-                   const int* __restrict__ ctx_len, int max_ctx, T* __restrict__ out, int ldo) {
+                   const int* __restrict__ ctx_len, int max_ctx, T* __restrict__ out, int ldo, const int2* __restrict__ rowpos) {
   extern __shared__ float sc_all[];            // [7][max_ctx]
   const int b = blockIdx.x, kvh = blockIdx.y;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = kvh * (NH / NKV) + w;
-  const int L = min(ctx_len[b] + 1, max_ctx);
+  const int cb = rowpos ? rowpos[b].x : b;
+  const int L = min((rowpos ? rowpos[b].y : ctx_len[b]) + 1, max_ctx);
   float* sc = sc_all + (size_t)w * max_ctx;
   const T* q = qkv + (size_t)b * ld + h * HD;
-  const T* kb = kc + ((size_t)b * NKV + kvh) * max_ctx * HD;
-  const T* vb = vc + ((size_t)b * NKV + kvh) * max_ctx * HD;
+  const T* kb = kc + ((size_t)cb * NKV + kvh) * max_ctx * HD;
+  const T* vb = vc + ((size_t)cb * NKV + kvh) * max_ctx * HD;
   float qr[HD];
 #pragma unroll
   for (int d = 0; d < HD; ++d) qr[d] = to_f32(q[d]) * 0.125f;
@@ -288,6 +294,161 @@ __global__ void gather_last_kernel(const float* __restrict__ x, const int* __res
   int b = blockIdx.x;
   const float* src = x + (size_t)(start[b] + len[b] - 1) * D;
   for (int c = threadIdx.x; c < D; c += blockDim.x) out[(size_t)b * D + c] = src[c];
+}
+
+// ---- ragged feed kernels (cvk_lm_feed_rows / cvk_lm_next_logp_rows) -------------------------------------------------------
+// activation row m <- embedding of (kinds[m], ids[m]): 0 text (embed_tokens), 1 speech (speech_embedding), 2 llm_embedding row
+__global__ void ragged_embed_kernel(const int* __restrict__ ids, const int* __restrict__ kinds, const float* __restrict__ text_emb,
+                                    const float* __restrict__ llm_emb, const float* __restrict__ speech_emb, float* __restrict__ x) {
+  const int m = blockIdx.x, kind = kinds[m], id = ids[m];
+  const float* src = kind == 0 ? text_emb + (size_t)id * D : (kind == 1 ? speech_emb + (size_t)id * D : llm_emb + (size_t)id * D);
+  for (int c = threadIdx.x; c < D; c += blockDim.x) x[(size_t)m * D + c] = src[c];
+}
+
+// per fed row i: hidden[row] <- x[its last activation row], ctx_len[row] += its position count (sc [n][3] = row, last row, count)
+__global__ void feed_scatter_kernel(const int* __restrict__ sc, const float* __restrict__ x, float* __restrict__ hidden, int* __restrict__ ctx_len) {
+  const int i = blockIdx.x, b = sc[3 * i], ml = sc[3 * i + 1];
+  for (int c = threadIdx.x; c < D; c += blockDim.x) hidden[(size_t)b * D + c] = x[(size_t)ml * D + c];
+  if (threadIdx.x == 0) ctx_len[b] += sc[3 * i + 2];
+}
+
+// out[i] <- hidden[rows[i]]
+__global__ void gather_rows_kernel(const int* __restrict__ rows, const float* __restrict__ hidden, float* __restrict__ out) {
+  const int i = blockIdx.x;
+  for (int c = threadIdx.x; c < D; c += blockDim.x) out[(size_t)i * D + c] = hidden[(size_t)rows[i] * D + c];
+}
+
+__device__ __forceinline__ void mma_16816_full(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// Ragged cached GQA attention on tensor cores (bf16 KV).  One CTA per (tile, kv head); a tile is up to two consecutive positions
+// of one session row: tiles[t] = (first activation row, session row, its cache position, 1 or 2).  The MMA's 16 rows are the 7
+// query heads of the first position (rows 0..6) and of the second (rows 8..14), so both positions share every K / V fragment.
+// Each query attends to its row's cache up to and including its own position: the appends of the whole pass ran before this
+// kernel, so causality inside a feed is only the key bound.  The RA_WARPS warps walk interleaved 16-key blocks with an online
+// softmax in registers (the decode unit's scheme, llm_decode_attn.cuh) and merge their partial (max, sum, O) in shared memory.
+constexpr int RA_WARPS = 4;
+__global__ void __launch_bounds__(32 * RA_WARPS)
+ragged_attn_tc_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kc, const bf16* __restrict__ vc, int max_ctx,
+                      const int4* __restrict__ tiles, bf16* __restrict__ out, int ldo) {
+  constexpr int G = NH / NKV;
+  __shared__ float ml[RA_WARPS][16][2];
+  __shared__ __align__(16) float po[RA_WARPS][16][HD];
+  const int4 tl = tiles[blockIdx.x];
+  const int m0 = tl.x, b = tl.y, pos0 = tl.z, n = tl.w, kvh = blockIdx.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
+  const bf16* kb = kc + ((size_t)b * NKV + kvh) * max_ctx * HD;
+  const bf16* vb = vc + ((size_t)b * NKV + kvh) * max_ctx * HD;
+  const int L0 = pos0 + 1, L1 = pos0 + n;      // key bounds of MMA rows 0..7 and 8..15 (n == 1: rows 8..15 repeat the first query)
+  const bf16* qa_row = qkv + (size_t)m0 * ld + (kvh * G + g) * HD;
+  const bf16* qb_row = qkv + (size_t)(m0 + n - 1) * ld + (kvh * G + g) * HD;
+  auto qpair = [&](const bf16* p, int d) -> uint32_t {   // two dims of one query head, pre-scaled by 1/sqrt(64) (exact in bf16)
+    if (g >= G) return 0u;
+    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + d));
+    return pack_bf16x2(f.x * 0.125f, f.y * 0.125f);
+  };
+  uint32_t qf[4][4];
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const int d = kk * 16 + t4 * 2;
+    qf[kk][0] = qpair(qa_row, d);
+    qf[kk][1] = qpair(qb_row, d);
+    qf[kk][2] = qpair(qa_row, d + 8);
+    qf[kk][3] = qpair(qb_row, d + 8);
+  }
+  float o[4][2][4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int t = 0; t < 2; ++t)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[q][t][e] = 0.f;
+  float m_a = -INFINITY, l_a = 0.f, m_b = -INFINITY, l_b = 0.f;
+  KvFrag fr;
+  for (int j0 = warp * 16; j0 < L1; j0 += RA_WARPS * 16) {
+    decode_attn_load_block(kb, vb, j0, L1, lane, fr);
+    float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      mma_16816_full(s0, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3], fr.kf[0][kk][0], fr.kf[0][kk][1]);
+      mma_16816_full(s1, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3], fr.kf[1][kk][0], fr.kf[1][kk][1]);
+    }
+    // this lane: keys ka, ka + 1 (s0) and ka + 8, ka + 9 (s1); elements 0, 1 belong to MMA row g, elements 2, 3 to row g + 8
+    const int ka = j0 + t4 * 2;
+    const int key[4] = {ka, ka + 1, ka + 8, ka + 9};
+    const float sa[4] = {s0[0], s0[1], s1[0], s1[1]}, sb[4] = {s0[2], s0[3], s1[2], s1[3]};
+    float mxa = -INFINITY, mxb = -INFINITY;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (key[e] < L0) mxa = fmaxf(mxa, sa[e]);
+      if (key[e] < L1) mxb = fmaxf(mxb, sb[e]);
+    }
+    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 1));
+    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 2));
+    mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 1));
+    mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 2));
+    // a block can hold no key of the first query (j0 == L0 when L1 = L0 + 1): keep its state, scale by 1, add nothing
+    const float na = fmaxf(m_a, mxa), nb = fmaxf(m_b, mxb);
+    const float ua = na == -INFINITY ? 0.f : na, ub = nb == -INFINITY ? 0.f : nb;
+    const float ca = __expf(m_a - ua), cb = __expf(m_b - ub);
+    float pa[4], pb[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      pa[e] = key[e] < L0 ? __expf(sa[e] - ua) : 0.f;
+      pb[e] = key[e] < L1 ? __expf(sb[e] - ub) : 0.f;
+    }
+    l_a = l_a * ca + ((pa[0] + pa[1]) + (pa[2] + pa[3]));
+    l_b = l_b * cb + ((pb[0] + pb[1]) + (pb[2] + pb[3]));
+    m_a = na;
+    m_b = nb;
+    const uint32_t p0 = pack_bf16x2(pa[0], pa[1]), p1 = pack_bf16x2(pb[0], pb[1]), p2 = pack_bf16x2(pa[2], pa[3]), p3 = pack_bf16x2(pb[2], pb[3]);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        o[q][t][0] *= ca; o[q][t][1] *= ca;
+        o[q][t][2] *= cb; o[q][t][3] *= cb;
+      }
+      // n-tile 0: even dims of the 16-dim block, n-tile 1: odd dims (as in decode_attn_unit)
+      mma_16816_full(o[q][0], p0, p1, p2, p3, __byte_perm(fr.vw[q][0], fr.vw[q][1], 0x5410), __byte_perm(fr.vw[q][2], fr.vw[q][3], 0x5410));
+      mma_16816_full(o[q][1], p0, p1, p2, p3, __byte_perm(fr.vw[q][0], fr.vw[q][1], 0x7632), __byte_perm(fr.vw[q][2], fr.vw[q][3], 0x7632));
+    }
+  }
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+  if (g < G) {
+    if (t4 == 0) {
+      ml[warp][g][0] = m_a;
+      ml[warp][g][1] = l_a;
+      ml[warp][g + 8][0] = m_b;
+      ml[warp][g + 8][1] = l_b;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {     // dims 16 q + 4 t4 .. + 3
+      *reinterpret_cast<float4*>(&po[warp][g][q * 16 + t4 * 4]) = make_float4(o[q][0][0], o[q][1][0], o[q][0][1], o[q][1][1]);
+      *reinterpret_cast<float4*>(&po[warp][g + 8][q * 16 + t4 * 4]) = make_float4(o[q][0][2], o[q][1][2], o[q][0][3], o[q][1][3]);
+    }
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < n * G * HD; e += 32 * RA_WARPS) {
+    const int r = e / (G * HD), hq = (e / HD) % G, d = e % HD, mr = r * 8 + hq;
+    float M = -INFINITY;
+#pragma unroll
+    for (int w2 = 0; w2 < RA_WARPS; ++w2) M = fmaxf(M, ml[w2][mr][0]);
+    float num = 0.f, den = 0.f;
+#pragma unroll
+    for (int w2 = 0; w2 < RA_WARPS; ++w2) {
+      const float wgt = __expf(ml[w2][mr][0] - M);    // warps without keys: exp(-inf) = 0
+      den = fmaf(wgt, ml[w2][mr][1], den);
+      num = fmaf(wgt, po[w2][mr][d], num);
+    }
+    out[(size_t)(m0 + r) * ldo + (kvh * G + hq) * HD + d] = __float2bfloat16_rn(num / den);
+  }
 }
 
 static inline size_t sampler_smem(int V) { return (size_t)2 * ((V + 3) & ~3) * sizeof(float); }   // probabilities + scores
@@ -755,40 +916,86 @@ std::vector<int> prefix(const int* lens, int B) {
   return off;
 }
 
-// GEMM of the LM: the weight-streaming split-K kernel when there are at most 64 activation rows (decode), else the tiled kernel
-void lm_gemm(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& e, cvk_lm_session* sess) {
-  if (sess && A.dtype == DT_BF16 && ctx->use_tc && ctx->use_skinny && e.out.rows <= 64 && W.w16)
-    conv_gemm_skinny(ctx, st, A, W, e, sess->scratch, sess->scratch_floats);
+// GEMM of the LM: the weight-streaming split-K kernel when there are at most 64 activation rows (decode, small feeds) and a
+// split-K scratch is given, else the tiled kernel
+void lm_gemm(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& e, float* scratch, size_t scratch_floats) {
+  if (scratch && A.dtype == DT_BF16 && ctx->use_tc && ctx->use_skinny && e.out.rows <= 64 && W.w16)
+    conv_gemm_skinny(ctx, st, A, W, e, scratch, scratch_floats);
   else
     conv_gemm(ctx, st, A, W, e);
 }
 
+// rows [r0, r0 + n) of a row-major view
+static Mat row_slice(const Mat& a, int r0, int n) { return Mat((char*)a.p + (size_t)r0 * a.ld * a.esize(), a.dtype, n, a.cols, a.ld); }
+
+// GEMM of the ragged feed calls: every activation row gets the same arithmetic whatever rows share the call.  lm_gemm's choice
+// between the skinny and the tiled kernel (different summation orders in bf16) depends on the row count, so in bf16 the rows go
+// through the weight-streaming kernel in slices of at most 64; its split count depends only on the weight, and the scratch covers
+// that split count at 64 rows for every LM weight, so no slice falls back to fewer splits.  fp32 (SIMT GEMM) is row-independent.
+void lm_gemm_rows(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& e, float* scratch, size_t scratch_floats) {
+  if (!(scratch && A.dtype == DT_BF16 && ctx->use_tc && ctx->use_skinny && W.w16)) {
+    conv_gemm(ctx, st, A, W, e);
+    return;
+  }
+  for (int r0 = 0; r0 < e.out.rows; r0 += 64) {
+    const int n = std::min(64, e.out.rows - r0);
+    Epilogue es = e;
+    es.out = row_slice(e.out, r0, n);
+    if (e.resid.p) es.resid = row_slice(e.resid, r0, n);
+    conv_gemm_skinny(ctx, st, row_slice(A, r0, n), W, es, scratch, scratch_floats);
+  }
+}
+
+// one pass of a ragged feed: where each activation row goes in the cache, and the attention tiles over them (llm_feed_rows)
+struct RaggedPass {
+  const int2* rowpos = nullptr;   // [M] (session row, cache position)
+  const int4* tiles = nullptr;    // [ntiles] see ragged_attn_tc_kernel
+  int ntiles = 0;
+};
+
 // one transformer layer on `rows` rows.  prefill: seqs geometry + causal attention over the qkv buffer;
-// decode: rows == sequences, attention against the cache.
+// decode: rows == sequences, attention against the cache; ragged (rg != null): rows are fed positions placed by rg, attention
+// against the cache.
 void layer_forward(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, int li, const Mat& x, const Mat& xn, const Mat& qkv, const Mat& att,
-                   const Mat& gu, const Mat& ffa, const Seqs* s, cvk_lm_session* sess, bool decode) {
+                   const Mat& gu, const Mat& ffa, const Seqs* s, cvk_lm_session* sess, bool decode, const RaggedPass* rg = nullptr) {
   const LayerW& w = m->layers[li];
   const int rows = x.rows;
+  float* scr = rg ? sess->fscratch : (decode ? sess->scratch : nullptr);
+  const size_t scr_n = rg ? sess->fscratch_floats : (decode ? sess->scratch_floats : 0);
   rmsnorm(ctx, st, x, w.ln1, RMS_EPS, xn);
   {
     Epilogue e;
     e.out = qkv;
-    lm_gemm(ctx, st, xn, w.qkv, e, decode ? sess : nullptr);
+    (rg ? lm_gemm_rows : lm_gemm)(ctx, st, xn, w.qkv, e, scr, scr_n);
   }
   size_t es = qkv.dtype == DT_F32 ? 4 : 2;
   void* kc = sess ? (char*)sess->kcache + (size_t)li * sess->max_batch * NKV * sess->max_ctx * HD * es : nullptr;
   void* vc = sess ? (char*)sess->vcache + (size_t)li * sess->max_batch * NKV * sess->max_ctx * HD * es : nullptr;
-  if (decode) {
+  if (rg) {
+    if (qkv.dtype == DT_F32) {
+      rope_append_kernel<float><<<dim3(1, rows), 128, 0, st>>>(qkv.f32(), qkv.ld, nullptr, nullptr, nullptr, m->d_inv_freq, (float*)kc,
+                                                               (float*)vc, sess->max_ctx, 1, rg->rowpos);
+      decode_attn_kernel<float><<<dim3(rows, NKV), (NH / NKV) * 32, (NH / NKV) * sess->max_ctx * sizeof(float), st>>>(
+          qkv.f32(), qkv.ld, (const float*)kc, (const float*)vc, nullptr, sess->max_ctx, att.f32(), att.ld, rg->rowpos);
+    } else {
+      rope_append_kernel<bf16><<<dim3(1, rows), 128, 0, st>>>(qkv.b16(), qkv.ld, nullptr, nullptr, nullptr, m->d_inv_freq, (bf16*)kc,
+                                                              (bf16*)vc, sess->max_ctx, 1, rg->rowpos);
+      ragged_attn_tc_kernel<<<dim3(rg->ntiles, NKV), 32 * RA_WARPS, 0, st>>>(qkv.b16(), qkv.ld, (const bf16*)kc, (const bf16*)vc, sess->max_ctx,
+                                                                              rg->tiles, att.b16(), att.ld);
+    }
+    ctx->launches += 2;
+    CVK_LAUNCH_CHECK();
+  } else if (decode) {
     if (qkv.dtype == DT_F32) {
       rope_append_kernel<float><<<dim3(1, rows), 128, 0, st>>>(qkv.f32(), qkv.ld, nullptr, nullptr, sess->ctx_len, m->d_inv_freq, (float*)kc,
-                                                               (float*)vc, sess->max_ctx, 1);
+                                                               (float*)vc, sess->max_ctx, 1, nullptr);
       decode_attn_kernel<float><<<dim3(rows, NKV), (NH / NKV) * 32, (NH / NKV) * sess->max_ctx * sizeof(float), st>>>(qkv.f32(), qkv.ld, (const float*)kc, (const float*)vc, sess->ctx_len, sess->max_ctx,
-                                                          att.f32(), att.ld);
+                                                          att.f32(), att.ld, nullptr);
     } else {
       rope_append_kernel<bf16><<<dim3(1, rows), 128, 0, st>>>(qkv.b16(), qkv.ld, nullptr, nullptr, sess->ctx_len, m->d_inv_freq, (bf16*)kc,
-                                                              (bf16*)vc, sess->max_ctx, 1);
+                                                              (bf16*)vc, sess->max_ctx, 1, nullptr);
       decode_attn_kernel<bf16><<<dim3(rows, NKV), (NH / NKV) * 32, (NH / NKV) * sess->max_ctx * sizeof(float), st>>>(qkv.b16(), qkv.ld, (const bf16*)kc, (const bf16*)vc, sess->ctx_len, sess->max_ctx,
-                                                         att.b16(), att.ld);
+                                                         att.b16(), att.ld, nullptr);
     }
     ctx->launches += 2;
     CVK_LAUNCH_CHECK();
@@ -798,10 +1005,10 @@ void layer_forward(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, int li, con
     int mc = sess ? sess->max_ctx : 0;
     if (qkv.dtype == DT_F32)
       rope_append_kernel<float><<<dim3(bx, s->B), 128, 0, st>>>(qkv.f32(), qkv.ld, s->d_start, s->d_len, nullptr, m->d_inv_freq, (float*)kc,
-                                                                (float*)vc, mc, 0);
+                                                                (float*)vc, mc, 0, nullptr);
     else
       rope_append_kernel<bf16><<<dim3(bx, s->B), 128, 0, st>>>(qkv.b16(), qkv.ld, s->d_start, s->d_len, nullptr, m->d_inv_freq, (bf16*)kc,
-                                                               (bf16*)vc, mc, 0);
+                                                               (bf16*)vc, mc, 0, nullptr);
     ctx->launches++;
     CVK_LAUNCH_CHECK();
     // causal == block-causal with chunk 1; 7 query heads per kv head
@@ -812,13 +1019,13 @@ void layer_forward(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, int li, con
     Epilogue e;
     e.resid = x;
     e.out = x;
-    lm_gemm(ctx, st, att, w.o, e, decode ? sess : nullptr);
+    (rg ? lm_gemm_rows : lm_gemm)(ctx, st, att, w.o, e, scr, scr_n);
   }
   rmsnorm(ctx, st, x, w.ln2, RMS_EPS, xn);
   {
     Epilogue e;
     e.out = gu;
-    lm_gemm(ctx, st, xn, w.gate_up, e, decode ? sess : nullptr);
+    (rg ? lm_gemm_rows : lm_gemm)(ctx, st, xn, w.gate_up, e, scr, scr_n);
   }
   {
     size_t total = (size_t)rows * DFF;
@@ -833,7 +1040,7 @@ void layer_forward(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, int li, con
     Epilogue e;
     e.resid = x;
     e.out = x;
-    lm_gemm(ctx, st, ffa, w.down, e, decode ? sess : nullptr);
+    (rg ? lm_gemm_rows : lm_gemm)(ctx, st, ffa, w.down, e, scr, scr_n);
   }
 }
 
@@ -842,7 +1049,7 @@ void head_logits(cvk_ctx* ctx, cudaStream_t st, const LlmModel* m, const Mat& hi
   rmsnorm(ctx, st, hidden_f32, m->final_norm, RMS_EPS, xn_act);
   Epilogue e;
   e.out = logits;
-  lm_gemm(ctx, st, xn_act, m->head, e, sess);
+  lm_gemm(ctx, st, xn_act, m->head, e, sess ? sess->scratch : nullptr, sess ? sess->scratch_floats : 0);
 }
 
 // Let decode_attn_kernel hold the scores of max_ctx positions for its 7 query heads in shared memory.  The limit is per function,
@@ -893,15 +1100,47 @@ void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int
   } else {
     Mat qkv = arena_mat(ctx, DT_BF16, rows, QKV_N, QKV_N);
     qkv_reduce_kernel<<<ceil_div(rows * QKV_N, 256), 256, 0, st>>>(partial, splits, rows, bias, qkv.b16());
-    rope_append_kernel<bf16><<<dim3(1, rows), 128, 0, st>>>(qkv.b16(), qkv.ld, nullptr, nullptr, d_len, d_inv, kc.b16(), vc.b16(), max_ctx, 1);
+    rope_append_kernel<bf16><<<dim3(1, rows), 128, 0, st>>>(qkv.b16(), qkv.ld, nullptr, nullptr, d_len, d_inv, kc.b16(), vc.b16(), max_ctx, 1, nullptr);
     decode_attn_kernel<bf16><<<dim3(rows, NKV), (NH / NKV) * 32, (NH / NKV) * max_ctx * sizeof(float), st>>>(
-        qkv.b16(), qkv.ld, kc.b16(), vc.b16(), d_len, max_ctx, att.b16(), att.ld);
+        qkv.b16(), qkv.ld, kc.b16(), vc.b16(), d_len, max_ctx, att.b16(), att.ld, nullptr);
     ctx->launches += 3;
   }
   CVK_LAUNCH_CHECK();
   convert_mat(ctx, st, kc, k32);
   convert_mat(ctx, st, vc, v32);
   convert_mat(ctx, st, att, Mat(out, DT_F32, rows, D, D));
+  CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+}
+
+// The tensor-core attention of a ragged feed on a caller-supplied cache, without a loaded LM (cvk_op_ragged_attention): q [M][896]
+// (already rotated), caches [cache_rows][NKV][max_ctx][64], query m = (cache row rowpos[2m], position rowpos[2m+1]) attending to
+// keys 0..position.  Consecutive queries of one row at consecutive positions share a tile, as in llm_feed_rows.  Everything crosses
+// the call as fp32 and runs as bf16, as in a session.
+void llm_ragged_attention_op(cvk_ctx* ctx, const float* q, const float* k_cache, const float* v_cache, int cache_rows, int max_ctx,
+                             const int* rowpos, int M, float* out, cudaStream_t st) {
+  for (int i = 0; i < M; ++i)
+    CVK_REQUIRE(rowpos[2 * i] >= 0 && rowpos[2 * i] < cache_rows && rowpos[2 * i + 1] >= 0 && rowpos[2 * i + 1] < max_ctx,
+                "cvk_op_ragged_attention: row or position out of range");
+  std::vector<int> tiles;
+  for (int i = 0; i < M;) {
+    const int n = (i + 1 < M && rowpos[2 * i + 2] == rowpos[2 * i] && rowpos[2 * i + 3] == rowpos[2 * i + 1] + 1) ? 2 : 1;
+    tiles.insert(tiles.end(), {i, rowpos[2 * i], rowpos[2 * i + 1], n});
+    i += n;
+  }
+  ctx->arena.reset();
+  const int ntiles = (int)tiles.size() / 4;
+  int* d_tiles = upload(ctx, tiles, st);
+  const int crows = cache_rows * NKV * max_ctx;
+  Mat q16 = arena_mat(ctx, DT_BF16, M, D, D), kc = arena_mat(ctx, DT_BF16, crows, HD, HD), vc = arena_mat(ctx, DT_BF16, crows, HD, HD),
+      att = arena_mat(ctx, DT_BF16, M, D, D);
+  convert_mat(ctx, st, Mat(const_cast<float*>(q), DT_F32, M, D, D), q16);
+  convert_mat(ctx, st, Mat(const_cast<float*>(k_cache), DT_F32, crows, HD, HD), kc);
+  convert_mat(ctx, st, Mat(const_cast<float*>(v_cache), DT_F32, crows, HD, HD), vc);
+  ragged_attn_tc_kernel<<<dim3(ntiles, NKV), 32 * RA_WARPS, 0, st>>>(q16.b16(), q16.ld, kc.b16(), vc.b16(), max_ctx,
+                                                                     reinterpret_cast<const int4*>(d_tiles), att.b16(), att.ld);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+  convert_mat(ctx, st, att, Mat(out, DT_F32, M, D, D));
   CVK_CHECK_CUDA(cudaStreamSynchronize(st));
 }
 
@@ -1013,6 +1252,8 @@ cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context)
   s->ffa = alloc(es * (size_t)max_batch * DFF);
   s->scratch_floats = skinny_scratch_floats(max_batch, 2 * DFF);
   s->scratch = (float*)alloc(s->scratch_floats * sizeof(float));
+  s->sel = (int*)alloc(sizeof(int) * max_batch);
+  s->rows_fed.assign(max_batch, 0);
   lm_mega_session_init(ctx, s);
   return s;
 }
@@ -1071,6 +1312,7 @@ void llm_prefill(cvk_ctx* ctx, cvk_lm_session* sess, const int32_t* text, const 
   CVK_REQUIRE(sess->max_batch <= 1024, "max_batch > 1024");
   init_state_kernel<<<1, sess->max_batch < 32 ? 32 : round_up(sess->max_batch, 32), 0, st>>>(s.d_len, B, sess->ctx_len, sess->base_len, sess->live);
   sess->fresh = true;
+  sess->ragged = false;
   ctx->launches += 2;
   CVK_LAUNCH_CHECK();
   sess->B = B;
@@ -1164,6 +1406,7 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
   const LlmModel* m = ctx->llm;
   CVK_REQUIRE(m && s->B > 0, "cvk_lm_prefill must run before cvk_lm_decode");
   const int B = s->B;
+  s->ragged = false;   // the decode steps advance ctx_len on the device only
   const bool was_fresh = s->fresh;
   if (s->fresh) {
     CVK_CHECK_CUDA(cudaMemsetAsync(out_count, 0, sizeof(int32_t) * B, st));
@@ -1271,6 +1514,8 @@ void llm_session_begin(cvk_ctx* ctx, cvk_lm_session* s, int B, cudaStream_t st) 
   s->B = B;
   s->fresh = true;
   s->fed = 0;
+  s->ragged = true;
+  s->rows_fed.assign(s->max_batch, 0);
 }
 
 // ids / kinds: HOST arrays of n entries (kind 0 text id, 1 speech id, 2 llm_embedding row); every row of the session receives the
@@ -1294,6 +1539,7 @@ void llm_feed(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* ids, const int32_t
   }
   CVK_CHECK_CUDA(cudaMemcpyAsync(s->hidden, s->x, sizeof(float) * (size_t)B * D, cudaMemcpyDeviceToDevice, st));
   s->fed += n;
+  for (int b = 0; b < B; ++b) s->rows_fed[b] += n;
   s->fresh = false;      // the step-graph decode (cvk_lm_decode) is not mixed with host-driven feeding
 }
 
@@ -1308,6 +1554,136 @@ void llm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, cudaStream_t st
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   CVK_CHECK_CUDA(cudaMemcpyAsync(logp, s->logits, sizeof(float) * (size_t)B * m->vout, cudaMemcpyDeviceToDevice, st));
+}
+
+// ---------------------------------------------------------------------------------------------- ragged feeding
+// Several rows of one session, each with its own number of new positions, in one forward per layer over M = sum(counts) activation
+// rows (the reference pushes a request's whole lm_input in one forward, llm.py:617-621; here the rows of several requests share it).
+// Everything is checked against the host mirror rows_fed before any device work, so a refused call changes nothing.
+static constexpr int FEED_CAP = 256;   // positions per forward pass; a larger feed runs as several passes in position order
+
+static void feed_buffers(cvk_lm_session* s) {
+  if (s->feed_cap) return;
+  const size_t es = s->kv_dtype == DT_F32 ? 4 : 2, cap = FEED_CAP;
+  auto alloc = [&](size_t bytes) {
+    void* p = nullptr;
+    CVK_CHECK_CUDA(cudaMalloc(&p, bytes));
+    s->owned.push_back(p);
+    return p;
+  };
+  s->fx = (float*)alloc(sizeof(float) * cap * D);
+  s->fxn = alloc(es * cap * D);
+  s->fqkv = alloc(es * cap * QKV_N);
+  s->fatt = alloc(es * cap * D);
+  s->fgu = alloc(es * cap * 2 * DFF);
+  s->fffa = alloc(es * cap * DFF);
+  s->fidx = (int*)alloc(sizeof(int) * (8 * cap + 3 * (size_t)s->max_batch));
+  // the largest split-K partial sums of the feed GEMMs at 64 rows: the down projection (N = 896) at up to 32 splits
+  s->fscratch_floats = skinny_scratch_floats(64, D);
+  s->fscratch = (float*)alloc(s->fscratch_floats * sizeof(float));
+  s->feed_cap = FEED_CAP;
+}
+
+static void check_id(const LlmModel* m, int kind, int id, const char* what) {
+  CVK_REQUIRE((kind == 0 && id >= 0 && id < 151936) || (kind == 1 && id >= 0 && id < m->vout) || (kind == 2 && id >= 0 && id < 2), what);
+}
+
+void llm_feed_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows, const int* counts, const int32_t* ids, const int32_t* kinds,
+                   cudaStream_t st) {
+  const LlmModel* m = ctx->llm;
+  CVK_REQUIRE(m && s->B > 0 && s->ragged, "cvk_lm_begin must run before cvk_lm_feed_rows");
+  CVK_REQUIRE(n_rows >= 1 && n_rows <= s->B, "cvk_lm_feed_rows: row count out of range");
+  std::vector<char> seen(s->B, 0);
+  int64_t total = 0;
+  for (int r = 0; r < n_rows; ++r) {
+    const int b = rows[r];
+    CVK_REQUIRE(b >= 0 && b < s->B && !seen[b], "cvk_lm_feed_rows: duplicate or out-of-range row");
+    seen[b] = 1;
+    CVK_REQUIRE(counts[r] >= 1 && (int64_t)s->rows_fed[b] + counts[r] <= s->max_ctx, "cvk_lm_feed_rows: row context exhausted");
+    total += counts[r];
+  }
+  for (int64_t i = 0; i < total; ++i) check_id(m, kinds[i], ids[i], "cvk_lm_feed_rows: id or kind out of range");
+  feed_buffers(s);
+  const int adt = s->kv_dtype, cap = s->feed_cap;
+  // pass index tables, one upload per pass: ids [cap] | kinds [cap] | rowpos int2 [cap] | tiles int4 [cap] | scatter [max_batch][3]
+  std::vector<int> h((size_t)8 * cap + 3 * (size_t)s->max_batch);
+  int* h_ids = h.data();
+  int* h_kinds = h_ids + cap;
+  int* h_rowpos = h_kinds + cap;
+  int* h_tiles = h_rowpos + 2 * cap;
+  int* h_sc = h_tiles + 4 * cap;
+  const int2* d_rowpos = reinterpret_cast<const int2*>(s->fidx + 2 * cap);
+  const int4* d_tiles = reinterpret_cast<const int4*>(s->fidx + 4 * cap);
+  const int* d_sc = s->fidx + 8 * cap;
+  int r = 0, in_row = 0;           // next position to place: row index r of the call, its in_row-th position
+  int64_t off = 0;
+  while (off < total) {
+    const int M = (int)std::min<int64_t>(cap, total - off);
+    int mm = 0, ntiles = 0, nsc = 0;
+    while (mm < M) {
+      const int b = rows[r], take = std::min(counts[r] - in_row, M - mm), pos = s->rows_fed[b];
+      for (int k = 0; k < take; ++k) {
+        h_ids[mm + k] = ids[off + mm + k];
+        h_kinds[mm + k] = kinds[off + mm + k];
+        h_rowpos[2 * (mm + k)] = b;
+        h_rowpos[2 * (mm + k) + 1] = pos + k;
+      }
+      for (int k = 0; k < take; k += 2) {
+        int* t = h_tiles + 4 * ntiles++;
+        t[0] = mm + k; t[1] = b; t[2] = pos + k; t[3] = std::min(2, take - k);
+      }
+      h_sc[3 * nsc] = b; h_sc[3 * nsc + 1] = mm + take - 1; h_sc[3 * nsc + 2] = take;
+      ++nsc;
+      s->rows_fed[b] += take;
+      mm += take;
+      in_row += take;
+      if (in_row == counts[r]) { ++r; in_row = 0; }
+    }
+    CVK_CHECK_CUDA(cudaMemcpyAsync(s->fidx, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    Mat x(s->fx, DT_F32, M, D, D), xn(s->fxn, adt, M, D, D), qkv(s->fqkv, adt, M, QKV_N, QKV_N), att(s->fatt, adt, M, D, D),
+        gu(s->fgu, adt, M, 2 * DFF, 2 * DFF), ffa(s->fffa, adt, M, DFF, DFF);
+    ragged_embed_kernel<<<M, 128, 0, st>>>(s->fidx, s->fidx + cap, m->text_emb, m->llm_emb, m->speech_emb, s->fx);
+    ctx->launches++;
+    CVK_LAUNCH_CHECK();
+    RaggedPass rg;
+    rg.rowpos = d_rowpos;
+    rg.tiles = d_tiles;
+    rg.ntiles = ntiles;
+    for (int li = 0; li < m->num_layers; ++li) layer_forward(ctx, st, m, li, x, xn, qkv, att, gu, ffa, nullptr, s, true, &rg);
+    feed_scatter_kernel<<<nsc, 128, 0, st>>>(d_sc, s->fx, s->hidden, s->ctx_len);
+    ctx->launches++;
+    CVK_LAUNCH_CHECK();
+    off += M;
+  }
+  s->fed = std::max(s->fed, *std::max_element(s->rows_fed.begin(), s->rows_fed.begin() + s->B));
+  s->fresh = false;
+}
+
+// log_softmax(llm_decoder(final_norm(hidden))) of the listed rows -> logp [n_rows][V] (device)
+void llm_next_logp_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows, float* logp, cudaStream_t st) {
+  const LlmModel* m = ctx->llm;
+  CVK_REQUIRE(m && s->B > 0 && s->ragged, "cvk_lm_begin must run before cvk_lm_next_logp_rows");
+  CVK_REQUIRE(n_rows >= 1 && n_rows <= s->B, "cvk_lm_next_logp_rows: row count out of range");
+  std::vector<char> seen(s->B, 0);
+  for (int r = 0; r < n_rows; ++r) {
+    const int b = rows[r];
+    CVK_REQUIRE(b >= 0 && b < s->B && !seen[b], "cvk_lm_next_logp_rows: duplicate or out-of-range row");
+    CVK_REQUIRE(s->rows_fed[b] > 0, "cvk_lm_next_logp_rows: row has no fed position");
+    seen[b] = 1;
+  }
+  CVK_CHECK_CUDA(cudaMemcpyAsync(s->sel, rows, sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
+  gather_rows_kernel<<<n_rows, 128, 0, st>>>(s->sel, s->hidden, s->x);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+  Mat hid(s->x, DT_F32, n_rows, D, D), xn(s->xn, s->kv_dtype, n_rows, D, D), logits(s->logits, DT_F32, n_rows, m->vout, m->vout);
+  rmsnorm(ctx, st, hid, m->final_norm, RMS_EPS, xn);
+  Epilogue e;
+  e.out = logits;
+  lm_gemm_rows(ctx, st, xn, m->head, e, s->scratch, s->scratch_floats);   // at most min(64, max_batch) rows per slice: within scratch
+  logsoftmax_rows_kernel<<<n_rows, SAMPLER_THREADS, 0, st>>>(s->logits, m->vout);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+  CVK_CHECK_CUDA(cudaMemcpyAsync(logp, s->logits, sizeof(float) * (size_t)n_rows * m->vout, cudaMemcpyDeviceToDevice, st));
 }
 
 int llm_vocab(cvk_ctx* ctx) { return ctx->llm ? ctx->llm->vout : 0; }

@@ -64,6 +64,16 @@ struct cvk_lm_session {
   float* scratch = nullptr;      // split-K partial sums of the weight-streaming GEMM
   size_t scratch_floats = 0;
   void* mega_state = nullptr;    // llm_mega.cu: per-session device state of the persistent decode kernel (barrier words, layer table)
+  // ragged feeding (cvk_lm_feed_rows / cvk_lm_next_logp_rows)
+  bool ragged = false;           // set by cvk_lm_begin; rows_fed mirrors ctx_len only between a begin and the next prefill / decode
+  std::vector<int> rows_fed;     // [max_batch] host mirror of ctx_len: positions fed to each row since cvk_lm_begin
+  int* sel = nullptr;            // [max_batch] device: rows listed by cvk_lm_next_logp_rows
+  int feed_cap = 0;              // positions per forward pass of the feed buffers below (0 until the first cvk_lm_feed_rows)
+  float* fx = nullptr;           // [feed_cap][896] fp32 residual stream of the fed positions
+  void *fxn = nullptr, *fqkv = nullptr, *fatt = nullptr, *fgu = nullptr, *fffa = nullptr;   // act [feed_cap][...]
+  int* fidx = nullptr;           // device copy of a pass's index tables (see llm_feed_rows)
+  float* fscratch = nullptr;     // split-K partial sums of the weight-streaming GEMM for up to 64 fed positions
+  size_t fscratch_floats = 0;
   std::vector<void*> owned;
 };
 

@@ -47,6 +47,7 @@ SIGNATURES = {
     "cvk_op_attention_ex": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, _c_int_p, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_op_decode_attention": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
+    "cvk_op_ragged_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_op_conv_gemm": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_int_p, _c_int_p, ctypes.c_int,
                                         _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp,
                                         _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -87,6 +88,8 @@ SIGNATURES = {
     "cvk_lm_begin": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _vp]),
     "cvk_lm_feed": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp]),
     "cvk_lm_next_logp": (ctypes.c_int, [_vp, _vp, _vp, _vp]),
+    "cvk_lm_feed_rows": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _c_int_p, _c_int_p, _c_int_p, _c_int_p, _vp]),
+    "cvk_lm_next_logp_rows": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _c_int_p, _vp, _vp]),
     "cvk_ras_sample": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp]),
     "cvk_op_sample_step": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
                                           _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -271,6 +274,16 @@ class Context:
         self._check(self.lib.cvk_op_decode_attention(self.h, _ptr(partial), splits, rows, _ptr(bias), _ptr(k_cache), _ptr(v_cache),
                                                      _ints(ctx_len), k_cache.shape[2], _ptr(out), _stream()))
         return out, k_cache, v_cache
+
+    def ragged_attention(self, q, k_cache, v_cache, rowpos):
+        """the feed attention of cvk_lm_feed_rows (cvk_op_ragged_attention): q [M, 896], caches [rows, 2, max_ctx, 64], rowpos: M python
+        (cache row, position) pairs.  Returns out [M, 896]."""
+        q, k_cache, v_cache = _f32(q, self.device), _f32(k_cache, self.device), _f32(v_cache, self.device)
+        assert len(rowpos) == q.shape[0] and k_cache.shape == v_cache.shape
+        out = torch.empty(q.shape[0], 896, device=self.device)
+        self._check(self.lib.cvk_op_ragged_attention(self.h, _ptr(q), _ptr(k_cache), _ptr(v_cache), k_cache.shape[0], k_cache.shape[2],
+                                                     _ints([v for rp in rowpos for v in rp]), len(rowpos), _ptr(out), _stream()))
+        return out
 
     def conv_gemm(self, x, seq_start, seq_len, w, bias=None, dil=1, shift0=0, operand="fp32", act1="none", act1_param=0.0, alpha1=None,
                   resid=None, resid_is_out=False, accumulate=False, out=None, out_dtype="fp32", act2="none", act2_param=0.0, alpha2=None,
@@ -520,6 +533,19 @@ class Context:
     def lm_next_logp(self, sess, B=1):
         out = torch.empty(B, self.lm_vocab(), device=self.device)
         self._check(self.lib.cvk_lm_next_logp(self.h, sess, _ptr(out), _stream()))
+        return out
+
+    def lm_feed_rows(self, sess, rows, counts, ids, kinds):
+        """rows: distinct session rows; row rows[r] receives counts[r] positions; ids / kinds: python int lists of all positions,
+        concatenated in row order (kinds as in lm_feed).  One forward for every row and position (cvk_lm_feed_rows)."""
+        if len(counts) != len(rows) or len(ids) != len(kinds) or len(ids) != sum(int(c) for c in counts):
+            raise ValueError("lm_feed_rows: need len(counts) == len(rows) and len(ids) == len(kinds) == sum(counts)")
+        self._check(self.lib.cvk_lm_feed_rows(self.h, sess, len(rows), _ints(rows), _ints(counts), _ints(ids), _ints(kinds), _stream()))
+
+    def lm_next_logp_rows(self, sess, rows):
+        """log-probs [len(rows), V] of the next id of each listed row (cvk_lm_next_logp_rows)"""
+        out = torch.empty(len(rows), self.lm_vocab(), device=self.device)
+        self._check(self.lib.cvk_lm_next_logp_rows(self.h, sess, len(rows), _ints(rows), _ptr(out), _stream()))
         return out
 
     def lm_last_logits(self, sess, B):

@@ -48,6 +48,114 @@ def _state_dict(m):
     return m if isinstance(m, dict) else m.state_dict()
 
 
+def _to_device(t, device):
+    """a small host tensor on `device` without a host sync: staged in pinned memory and copied asynchronously on the current stream
+    (a plain .to() from pageable memory waits for the stream's queued work)"""
+    if device.type != "cuda" or t.device.type == "cuda":
+        return t.to(device)
+    return t.pin_memory().to(device, non_blocking=True)
+
+
+class _BistreamRow:
+    """The per-request control flow of the text-streaming LM (llm.py:551-661, Qwen2LM.inference_bistream), as a state machine that
+    lm_generate_bistream and lm_generate_bistream_batch both drive.
+
+    States: WAIT (needs the next text chunk, or the end of the text), DECODE (the inner decode loop of llm.py:614-640: every step is
+    one model call on `lm_input` and one id, forced or drawn, until a fill token sends the row back to WAIT), FINAL (llm.py:642-661:
+    decode until eos) and DONE.  A step in DECODE / FINAL is: feed `lm_input`, then, unless `forced()`, draw with
+    `ignore_eos()` from the log-probs, then `take(id)`.
+
+    `lm_input` has the reference variable's exact life cycle (list of (kind, id) positions): every model call pushes ALL of it, it is
+    replaced after a yielded id and - like the reference - left untouched when a fill token ends a decode burst, so a final phase
+    entered right after a fill token pushes that last input a second time (llm.py:634-637, 643)."""
+    WAIT, DECODE, FINAL, DONE = range(4)
+    MIX_TEXT, MIX_SPEECH = 5, 15
+    TEXT, SPEECH, LLM = 0, 1, 2
+    SPEECH_VOCAB = 6561
+
+    def __init__(self, fill_token, eos_token, eop_token, prompt_text, prompt_speech_token, max_tokens=None):
+        self.fill_token, self.eos_token, self.max_tokens = fill_token, eos_token, max_tokens
+        ptext = [int(x) for x in prompt_text.reshape(-1).tolist()]
+        lm_prefix = []
+        if eop_token is not None:
+            # llm.py:583-588: the prompt text up to and including <|endofprompt|> is fed ahead of the 5:15 interleaving
+            if eop_token not in ptext:
+                raise AssertionError("<|endofprompt|> not detected in CosyVoice3 prompt_text, check your input!")
+            eop = ptext.index(eop_token)
+            lm_prefix, ptext = [(self.TEXT, t) for t in ptext[:eop + 1]], ptext[eop + 1:]
+        self.pspeech = [int(x) for x in prompt_speech_token.reshape(-1).tolist()]
+        self.lm_input = [(self.LLM, 0)] + lm_prefix
+        self.text_cache = list(ptext)
+        self.out_tokens = []
+        self.next_fill_index = (len(self.pspeech) // self.MIX_SPEECH + 1) * self.MIX_SPEECH - len(self.pspeech)
+        self.fed = 0                       # positions pushed so far (the session's context)
+        self.state = self.WAIT
+
+    def add_text(self, ids):
+        """one chunk of the text generator (llm.py:593-613): interleave prompt speech, then enter the decode loop if possible"""
+        T, M = self.MIX_TEXT, self.MIX_SPEECH
+        self.text_cache += [int(x) for x in ids]
+        while self.pspeech:                                            # llm.py:595-604
+            if len(self.text_cache) >= T:
+                self.lm_input = self.lm_input + [(self.TEXT, t) for t in self.text_cache[:T]] + [(self.SPEECH, t) for t in self.pspeech[:M]]
+                self.text_cache, self.pspeech = self.text_cache[T:], self.pspeech[M:]
+            else:
+                break
+        if self.pspeech:
+            return
+        out = self.out_tokens                                          # llm.py:606-613
+        if (out and out[-1] == self.fill_token) or (not out and len(self.lm_input) == 1):
+            if len(self.text_cache) < T:
+                return
+            lm_text = [(self.TEXT, t) for t in self.text_cache[:T]]
+            self.lm_input = lm_text if (out and out[-1] == self.fill_token) else self.lm_input + lm_text
+            self.text_cache = self.text_cache[T:]
+        self.state = self.DECODE
+
+    def end_text(self):
+        """the text generator is exhausted (llm.py:643)"""
+        self.lm_input = self.lm_input + [(self.TEXT, t) for t in self.text_cache] + [(self.LLM, 1)]
+        self.state = self.FINAL
+        self._check_cap()
+
+    def _check_cap(self):
+        # benchmark aid (bistream_max_tokens): the final phase ends after this many ids
+        if self.state == self.FINAL and self.max_tokens is not None and len(self.out_tokens) >= self.max_tokens:
+            self.state = self.DONE
+
+    def forced(self):
+        """the id of this step is a forced fill token (llm.py:624-626); the reference still runs the model first"""
+        return self.state == self.DECODE and self.next_fill_index != -1 and len(self.out_tokens) == self.next_fill_index
+
+    def ignore_eos(self):
+        return self.state == self.DECODE
+
+    def take(self, top):
+        """the id of this step (ignored when forced); returns the id to yield, or None.  Raises ValueError like the reference."""
+        if self.state == self.DECODE:
+            if self.forced():
+                top = self.fill_token
+                self.next_fill_index += self.MIX_SPEECH + 1
+            if top == self.fill_token:
+                self.next_fill_index = len(self.out_tokens) + self.MIX_SPEECH + 1
+            self.out_tokens.append(top)
+            if top >= self.SPEECH_VOCAB:
+                if top == self.fill_token:
+                    self.state = self.WAIT
+                    return None
+                raise ValueError(f"should not get token {top}")
+        else:
+            self.out_tokens.append(top)
+            if top >= self.SPEECH_VOCAB:
+                if top == self.eos_token:
+                    self.state = self.DONE
+                    return None
+                raise ValueError(f"should not get token {top}")
+        self.lm_input = [(self.SPEECH, top)]
+        self._check_cap()
+        return top
+
+
 def cfm_rand_noise():
     """CausalConditionalCFM.rand_noise (flow/flow_matching.py:199-200): seed-0 torch.randn([1,80,15000]), time-major."""
     g = torch.Generator(device="cpu")
@@ -64,6 +172,7 @@ class B200CosyVoice2Model:
     # benchmark aid only (None = the reference's behaviour: decode "until met eos", llm.py:642-661, without any cap): random-init
     # weights cannot be made to emit eos at a chosen time, so bench.py ends the text-streaming decode after this many ids
     bistream_max_tokens = None
+    bistream_max_ctx = 4096              # positions of the text-streaming LM session (per request)
     # streaming synthesis: intermediate chunks through the cached flow session (cvk_flow_stream_*: each chunk computes only its new
     # frames) instead of the reference's prefix recompute (cli/model.py:346-363); same frames either way.  The U-Net estimator of
     # B200CosyVoice3Model uses the same sessions for its DiT.
@@ -296,105 +405,151 @@ class B200CosyVoice2Model:
         'decode until eos' phase are the reference's control flow line for line; the arithmetic runs on the device through
         cvk_lm_begin / cvk_lm_feed / cvk_lm_next_logp / cvk_ras_sample.  uniforms [n,2]: row len(out_tokens) is consumed by the
         draw that produces that token (default: drawn from the model's generator)."""
-        mix_text, mix_speech = 5, 15
-        fill_token, eos_token, speech_vocab = self.bistream_fill_token, self.bistream_eos_token, 6561
-        TEXT, SPEECH, LLM = 0, 1, 2
         d = self.device
-        ptext = [int(x) for x in prompt_text.reshape(-1).tolist()]
-        lm_prefix = []
-        if self.bistream_eop_token is not None:
-            # llm.py:583-588: the prompt text up to and including <|endofprompt|> is fed ahead of the 5:15 interleaving
-            if self.bistream_eop_token not in ptext:
-                raise AssertionError("<|endofprompt|> not detected in CosyVoice3 prompt_text, check your input!")
-            eop = ptext.index(self.bistream_eop_token)
-            lm_prefix, ptext = [(TEXT, t) for t in ptext[:eop + 1]], ptext[eop + 1:]
-        pspeech = [int(x) for x in prompt_speech_token.reshape(-1).tolist()]
-        max_ctx = 4096
+        row = self._bistream_row(prompt_text, prompt_speech_token)
+        max_ctx = self.bistream_max_ctx
         lm_stream = stream if stream is not None else self.stream
         key, sess = self._checkout_session(1, max_ctx - 8)
         with torch.cuda.stream(lm_stream):
             self.ctx.lm_begin(sess, 1)
         if uniforms is None and self.uniforms_override is not None:
             uniforms = self.uniforms_override[:, 0, :]
-        # `lm_input` has the reference variable's exact life cycle (list of (kind, id) positions): every model call pushes ALL
-        # of it, it is replaced after a yielded token and - like the reference - left untouched when a fill token ends a decode
-        # burst, so a final phase entered right after a fill token pushes that last input a second time (llm.py:634-637, 643).
-        lm_input = [(LLM, 0)] + lm_prefix
-        text_cache = list(ptext)
-        out_tokens = []
-        next_fill_index = (len(pspeech) // mix_speech + 1) * mix_speech - len(pspeech)
-        fed = [0]
 
-        def forward(want_logp):
-            """llm.py:617-622: push lm_input through the cached model; log-probs of the next id"""
+        def step():
+            """llm.py:617-627 / 648-650: push lm_input through the cached model, then the forced id or a draw (sampling_ids)"""
             with torch.cuda.stream(lm_stream):
-                fed[0] += len(lm_input)
-                if fed[0] >= max_ctx - 16:
-                    raise RuntimeError("text-streaming LM: session context exhausted")
-                self.ctx.lm_feed(sess, [i for _, i in lm_input], [k for k, _ in lm_input])
-                return self.ctx.lm_next_logp(sess, 1) if want_logp else None
-
-        def sample(logp, ignore_eos):
-            """llm.py:627 / 650 sampling_ids"""
-            with torch.cuda.stream(lm_stream):
-                i = len(out_tokens)
+                self._bistream_count_fed(row)
+                self.ctx.lm_feed(sess, [i for _, i in row.lm_input], [k for k, _ in row.lm_input])
+                if row.forced():                                      # the reference runs the model before overriding the draw
+                    return row.take(None)
+                logp = self.ctx.lm_next_logp(sess, 1)
+                i = len(row.out_tokens)
                 if uniforms is not None:
                     u = uniforms[i].reshape(1, 2)
                 else:
                     with self.lock:
                         u = torch.rand(1, 2, device=d, generator=self.generator)
-                hist = torch.tensor([out_tokens[-16:] or [0]], dtype=torch.int32)
-                top = self.ctx.ras_sample(logp, hist, torch.tensor([min(len(out_tokens), 16)], dtype=torch.int32), u,
-                                          torch.tensor([1 if ignore_eos else 0], dtype=torch.int32))
-                return int(top.item())
+                hist, cnt = self._bistream_history([row])
+                top = self.ctx.ras_sample(logp, hist, cnt, u, torch.tensor([1 if row.ignore_eos() else 0], dtype=torch.int32))
+                return row.take(int(top.item()))
 
         try:
             for this_text in text:
-                text_cache += [int(x) for x in this_text.reshape(-1).tolist()]
-                while pspeech:                                            # llm.py:595-604
-                    if len(text_cache) >= mix_text:
-                        lm_input = lm_input + [(TEXT, t) for t in text_cache[:mix_text]] + [(SPEECH, t) for t in pspeech[:mix_speech]]
-                        text_cache, pspeech = text_cache[mix_text:], pspeech[mix_speech:]
-                    else:
-                        break
-                if not pspeech:                                           # llm.py:606-640
-                    if (out_tokens and out_tokens[-1] == fill_token) or (not out_tokens and len(lm_input) == 1):
-                        if len(text_cache) >= mix_text:
-                            lm_text = [(TEXT, t) for t in text_cache[:mix_text]]
-                            lm_input = lm_text if (out_tokens and out_tokens[-1] == fill_token) else lm_input + lm_text
-                            text_cache = text_cache[mix_text:]
-                        else:
-                            continue
-                    while True:
-                        forced = next_fill_index != -1 and len(out_tokens) == next_fill_index
-                        logp = forward(want_logp=not forced)              # the reference runs the model before overriding the draw
-                        if forced:
-                            top = fill_token
-                            next_fill_index += mix_speech + 1
-                        else:
-                            top = sample(logp, ignore_eos=True)
-                        if top == fill_token:
-                            next_fill_index = len(out_tokens) + mix_speech + 1
-                        out_tokens.append(top)
-                        if top >= speech_vocab:
-                            if top == fill_token:
-                                break
-                            raise ValueError(f"should not get token {top}")
+                row.add_text(this_text.reshape(-1).tolist())
+                while row.state == row.DECODE:
+                    top = step()
+                    if top is not None:
                         yield top
-                        lm_input = [(SPEECH, top)]
-            lm_input = lm_input + [(TEXT, t) for t in text_cache] + [(LLM, 1)]       # llm.py:643
-            while True:
-                if self.bistream_max_tokens is not None and len(out_tokens) >= self.bistream_max_tokens:
-                    break
-                top = sample(forward(want_logp=True), ignore_eos=False)
-                out_tokens.append(top)
-                if top >= speech_vocab:
-                    if top == eos_token:
-                        break
-                    raise ValueError(f"should not get token {top}")
-                yield top
-                lm_input = [(SPEECH, top)]
+            row.end_text()
+            while row.state == row.FINAL:
+                top = step()
+                if top is not None:
+                    yield top
         finally:
+            if lm_stream is not None:
+                lm_stream.synchronize()
+            self._checkin_session(key, sess)
+
+    def _bistream_row(self, prompt_text, prompt_speech_token):
+        return _BistreamRow(self.bistream_fill_token, self.bistream_eos_token, self.bistream_eop_token, prompt_text, prompt_speech_token,
+                            self.bistream_max_tokens)
+
+    def _bistream_count_fed(self, row):
+        row.fed += len(row.lm_input)
+        if row.fed >= self.bistream_max_ctx - 16:
+            raise RuntimeError("text-streaming LM: session context exhausted")
+
+    @staticmethod
+    def _bistream_history(rows):
+        """the rows' last 16 ids (zero-padded) and their counts: the repetition window of sampling_ids (common.py:138-149)"""
+        hist = torch.tensor([(r.out_tokens[-16:] + [0] * 16)[:16] for r in rows], dtype=torch.int32)
+        return hist, torch.tensor([min(len(r.out_tokens), 16) for r in rows], dtype=torch.int32)
+
+    def lm_generate_bistream_batch(self, texts, prompt_texts, prompt_speech_tokens, uniforms=None, stream=None):
+        """lm_generate_bistream for several requests in one LM session: a generator of (i, id) as request i's ids are decoded.
+
+        `texts` are generators of int32 [1,k] chunks; one feeder thread per generator moves its chunks into a queue.  Every step
+        makes one cvk_lm_feed_rows call for all rows whose state machine can advance (rows waiting for text sit the step out), one
+        cvk_lm_next_logp_rows + one cvk_ras_sample call for the rows that draw (forced fill tokens do not), and one device-to-host
+        copy of the drawn ids - the step's only host sync (the sampler's small inputs go through pinned memory).  uniforms [n, B, 2]: uniforms[k, i] is row i's draw for
+        len(out_tokens) == k, as in lm_generate_bistream.  A row's ids depend only on its own chunks and uniforms, not on arrival
+        timing or on which rows share a step.  A row error (ValueError for an unexpected special id, AssertionError for a CosyVoice3
+        prompt without <|endofprompt|>) ends the whole generator; closing it stops within one step and returns the session."""
+        import queue
+        B = len(texts)
+        d = self.device
+        rows = [self._bistream_row(pt, ps) for pt, ps in zip(prompt_texts, prompt_speech_tokens)]
+        if uniforms is None and self.uniforms_override is not None:
+            uniforms = self.uniforms_override
+        lm_stream = stream if stream is not None else self.stream
+        arrivals = queue.Queue()               # (row, chunk ids) / (row, None) at the end / (row, exception)
+        pending = [[] for _ in range(B)]
+        stop = threading.Event()
+
+        def feeder(i, gen):
+            try:
+                for chunk in gen:
+                    if stop.is_set():
+                        return
+                    arrivals.put((i, chunk.reshape(-1).tolist()))
+                arrivals.put((i, None))
+            except BaseException as e:        # noqa: BLE001  (re-raised by the generator)
+                arrivals.put((i, e))
+
+        key, sess = self._checkout_session(B, self.bistream_max_ctx - 8)
+        try:
+            with torch.cuda.stream(lm_stream):
+                self.ctx.lm_begin(sess, B)
+            for i, gen in enumerate(texts):
+                threading.Thread(target=feeder, args=(i, gen), name=f"cvk-bistream-text-{i}", daemon=True).start()
+            while True:
+                # take what has arrived (and block for more when no row can advance)
+                while True:
+                    try:
+                        i, item = arrivals.get_nowait()
+                    except queue.Empty:
+                        break
+                    pending[i].append(item)
+                for i, r in enumerate(rows):
+                    while r.state == r.WAIT and pending[i]:
+                        item = pending[i].pop(0)
+                        if isinstance(item, BaseException):
+                            raise item
+                        if item is None:
+                            r.end_text()
+                        else:
+                            r.add_text(item)
+                adv = [i for i, r in enumerate(rows) if r.state in (r.DECODE, r.FINAL)]
+                if not adv:
+                    if all(r.state == r.DONE for r in rows):
+                        return
+                    i, item = arrivals.get()
+                    pending[i].append(item)
+                    continue
+                with torch.cuda.stream(lm_stream):
+                    for i in adv:
+                        self._bistream_count_fed(rows[i])
+                    self.ctx.lm_feed_rows(sess, adv, [len(rows[i].lm_input) for i in adv],
+                                          [t for i in adv for _, t in rows[i].lm_input], [k for i in adv for k, _ in rows[i].lm_input])
+                    draw = [i for i in adv if not rows[i].forced()]
+                    drawn = {}
+                    if draw:
+                        logp = self.ctx.lm_next_logp_rows(sess, draw)
+                        if uniforms is not None:
+                            u = _to_device(torch.stack([uniforms[len(rows[i].out_tokens), i] for i in draw]).reshape(len(draw), 2), d)
+                        else:
+                            with self.lock:
+                                u = torch.rand(len(draw), 2, device=d, generator=self.generator)
+                        hist, cnt = self._bistream_history([rows[i] for i in draw])
+                        ign = torch.tensor([1 if rows[i].ignore_eos() else 0 for i in draw], dtype=torch.int32)
+                        top = self.ctx.ras_sample(logp, _to_device(hist, d), _to_device(cnt, d), u, _to_device(ign, d)).cpu().tolist()
+                        drawn = dict(zip(draw, top))
+                for i in adv:
+                    top = rows[i].take(drawn.get(i))
+                    if top is not None:
+                        yield i, top
+        finally:
+            stop.set()
             if lm_stream is not None:
                 lm_stream.synchronize()
             self._checkin_session(key, sess)
@@ -711,38 +866,74 @@ class B200CosyVoice2Model:
         exception in it) gives the requests' slots back and ends the LM generation within one block of 8 decode steps."""
         for r in inputs:
             if not torch.is_tensor(r.get("text")):
-                raise ValueError("tts_stream_batch takes token tensors as text; a text generator (bi-stream LM) is served by tts()")
+                raise ValueError("tts_stream_batch takes token tensors as text; requests with a text generator go to tts_bistream_batch")
+        empty = torch.zeros(1, 0, dtype=torch.int32)
+
+        def lm_run(emit, lm_state):
+            B = len(inputs)
+            consumed = [0] * B
+
+            def progress(out_ids, out_count, live):
+                if lm_state["stop"]:
+                    raise _LmStopped()                   # the generator was closed: end the decode at the next block
+                cnt = out_count.cpu().tolist()
+                ids = out_ids.cpu()
+                for b in range(B):
+                    if cnt[b] > consumed[b]:
+                        for tok in ids[b, consumed[b]:cnt[b]].tolist():
+                            emit(b, tok)
+                        consumed[b] = cnt[b]
+            with self._lm_stream() as lm_stream:
+                self.lm_generate([r["text"] for r in inputs], [r.get("prompt_text", empty) for r in inputs],
+                                 [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms, steps_per_sync=8,
+                                 on_progress=progress, stream=lm_stream)
+        yield from self._stream_batch(inputs, lm_run, noise_fns)
+
+    def tts_bistream_batch(self, inputs, uniforms=None, noise_fns=None):
+        """tts_stream_batch for text-streaming requests: `inputs` are tts() kwargs dicts whose `text` is a generator of int32 [1,k]
+        chunks.  Same contract and rounds as tts_stream_batch - (i, {'tts_speech': ...}) with each request's tts(stream=True) chunk
+        schedule, the multi-slot flow session, vocoder caches and cross-fade - with the LM job replaced by one
+        lm_generate_bistream_batch over all requests (uniforms[k, i] for request i's k-th draw).  Closing the generator early (or an
+        exception in it) gives the requests' slots back and ends the LM generation at its next decoded id."""
+        empty = torch.zeros(1, 0, dtype=torch.int32)
+
+        def lm_run(emit, lm_state):
+            with self._lm_stream() as lm_stream:
+                gen = self.lm_generate_bistream_batch([iter(r["text"]) for r in inputs], [r.get("prompt_text", empty) for r in inputs],
+                                                      [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms,
+                                                      stream=lm_stream)
+                try:
+                    for b, tok in gen:
+                        if lm_state["stop"]:
+                            break
+                        emit(b, tok)
+                finally:
+                    gen.close()
+        yield from self._stream_batch(inputs, lm_run, noise_fns)
+
+    def _stream_batch(self, inputs, lm_run, noise_fns):
+        """the poll loop of tts_stream_batch / tts_bistream_batch.  lm_run(emit, lm_state) runs the LM job on a side thread and calls
+        emit(i, id) for every id request i decodes; it ends early once lm_state["stop"] is set."""
         B = len(inputs)
         empty = torch.zeros(1, 0, dtype=torch.int32)
         req = [dict(ptok=r.get("flow_prompt_speech_token", empty), pfeat=r.get("prompt_speech_feat", torch.zeros(1, 0, 80)),
                     emb=r.get("flow_embedding", torch.zeros(0, 192))) for r in inputs]
         toks = [[] for _ in range(B)]
         lm_state = {"end": False, "err": None, "stop": False}
-        consumed, silent = [0] * B, [0] * B
+        silent = [0] * B
 
-        def progress(out_ids, out_count, live):
-            if lm_state["stop"]:
-                raise _LmStopped()                       # the generator was closed: end the decode at the next block
-            cnt = out_count.cpu().tolist()
-            ids = out_ids.cpu()
-            for b in range(B):
-                if cnt[b] > consumed[b]:
-                    for tok in ids[b, consumed[b]:cnt[b]].tolist():
-                        if tok in self.silent_tokens:            # cli/model.py:121-127
-                            silent[b] += 1
-                            if silent[b] > 5:
-                                continue
-                        else:
-                            silent[b] = 0
-                        toks[b].append(tok)
-                    consumed[b] = cnt[b]
+        def emit(b, tok):
+            if tok in self.silent_tokens:            # cli/model.py:121-127
+                silent[b] += 1
+                if silent[b] > 5:
+                    return
+            else:
+                silent[b] = 0
+            toks[b].append(tok)
 
         def llm_job():
             try:
-                with self._lm_stream() as lm_stream:
-                    self.lm_generate([r["text"] for r in inputs], [r.get("prompt_text", empty) for r in inputs],
-                                     [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms, steps_per_sync=8,
-                                     on_progress=progress, stream=lm_stream)
+                lm_run(emit, lm_state)
             except _LmStopped:
                 pass
             except BaseException as e:                   # noqa: BLE001  (re-raised by the generator)

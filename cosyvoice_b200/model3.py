@@ -30,6 +30,11 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
         causal vocoder re-runs over all mel produced so far (cli/model.py:425-450).  The multi-slot DiT sessions exist in libcvk."""
         raise NotImplementedError("tts_stream_batch is CosyVoice2-only; stream CosyVoice3 requests with tts(stream=True)")
 
+    def tts_bistream_batch(self, inputs, uniforms=None, noise_fns=None):
+        """Not built for CosyVoice3, for the reason tts_stream_batch is not; its text-streaming LM is batched
+        (lm_generate_bistream_batch)."""
+        raise NotImplementedError("tts_bistream_batch is CosyVoice2-only; stream CosyVoice3 requests with tts(stream=True)")
+
     # ---------------------------------------------------------------- weights
     def load_state_dicts(self, llm_sd, flow_sd, hift_sd, rand_ini=None, sine_noise=None):
         """llm_sd: CosyVoice3LM, flow_sd: CausalMaskedDiffWithDiT, hift_sd: CausalHiFTGenerator state_dicts.  rand_ini [1,9] /

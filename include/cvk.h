@@ -15,7 +15,8 @@
  *    cvk_destroy - repack weights on the default stream and block until done).
  *  - Threading: calls that use the ctx workspace (cvk_lm_prefill, cvk_lm_forward_logp, every flow / vocoder / mel / op
  *    call) must be serialised by the caller.  Calls that only touch an LM session (cvk_lm_decode, cvk_lm_begin,
- *    cvk_lm_feed, cvk_lm_next_logp, cvk_lm_last_logits) and cvk_ras_sample own no shared state: they may run
+ *    cvk_lm_feed, cvk_lm_next_logp, cvk_lm_feed_rows, cvk_lm_next_logp_rows, cvk_lm_last_logits) and cvk_ras_sample own no
+ *    shared state: they may run
  *    concurrently with workspace calls and with each other on DISTINCT sessions and streams - this is the reference's
  *    own concurrency (LM side thread + side stream next to token2wav, cli/model.py:101-129, 268; several requests in
  *    flight, runtime/python/grpc/server.py:69).  One session is never used by two host threads at once.  Streaming-flow
@@ -115,6 +116,12 @@ int cvk_op_attention_ex(cvk_ctx* ctx, const float* q, const float* k, const floa
  * in / out (run as bf16, as in a session, and written back as fp32 with the new row appended); ctx_len_host[b] in [0, max_ctx) is the
  * position of the new token, i.e. the number of history rows; out [rows][896].  Option "lm_fused" selects the fused kernel of the
  * decode graph (default) or, at 0, the per-op reduction + RoPE/append + attention kernels.  max_ctx obeys the session limit. */
+/* The cached GQA attention of cvk_lm_feed_rows (tensor-core kernel) on a caller-supplied cache, bf16 context only: q [M][896]
+ * (14 query heads, already rotated), k_cache, v_cache [cache_rows][2][max_ctx][64]; query m belongs to cache row rowpos_host[2m] at
+ * position rowpos_host[2m+1] and attends to that row's keys 0..position; out [M][896].  Consecutive queries of one row at consecutive
+ * positions share a tensor-core tile, as in a feed.  Inputs cross as fp32 and run as bf16, as in a session. */
+int cvk_op_ragged_attention(cvk_ctx* ctx, const float* q, const float* k_cache, const float* v_cache, int cache_rows, int max_ctx,
+                            const int* rowpos_host, int M, float* out, void* stream);
 int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
                             const int* ctx_len_host, int max_ctx, float* out, void* stream);
 /* element types of the cvk_op_conv_gemm operand and outputs */
@@ -296,6 +303,21 @@ int cvk_lm_vocab(cvk_ctx* ctx);
 int cvk_lm_begin(cvk_ctx* ctx, cvk_lm_session* s, int B, void* stream);
 int cvk_lm_feed(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* ids_host, const int32_t* kinds_host, int n, void* stream);
 int cvk_lm_next_logp(cvk_ctx* ctx, cvk_lm_session* s, float* logp, void* stream);
+/* Ragged feeding, for several text-streaming requests in one session (one row each, after cvk_lm_begin with B rows): row
+ * rows_host[r] (n_rows distinct rows < B) receives counts_host[r] >= 1 new positions; ids_host / kinds_host hold them concatenated
+ * in row order (kinds as in cvk_lm_feed).  Every position of every listed row goes through ONE forward per layer: row b's positions
+ * take RoPE / cache positions fed_b .. fed_b + n - 1 (fed_b = positions fed to row b since cvk_lm_begin) and attend causally to
+ * that row's cache.  A row's results are bit for bit the same whatever other rows and positions share the call (or split it into
+ * passes).  Rows not listed keep their cache, context length and hidden state bit for bit.  Duplicate or out-of-range
+ * rows, ids or kinds out of range, and a row whose context would pass the session's max_context are refused with CVK_ERR_INVALID
+ * before any device work, so a refused call changes nothing.  A feed of more than 256 positions runs as several forward passes in
+ * position order.  The session owns the feed buffers (allocated on first use); like cvk_lm_feed, the call touches no workspace.
+ * cvk_lm_next_logp_rows writes the log-probs of the next id after the last fed position of each listed row (distinct rows that
+ * have been fed) to logp [n_rows][V] (device, V = cvk_lm_vocab), in list order.  After cvk_lm_prefill or cvk_lm_decode both are
+ * refused until the next cvk_lm_begin. */
+int cvk_lm_feed_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows_host, const int* counts_host, const int32_t* ids_host,
+                     const int32_t* kinds_host, void* stream);
+int cvk_lm_next_logp_rows(cvk_ctx* ctx, cvk_lm_session* s, int n_rows, const int* rows_host, float* logp, void* stream);
 /* parity tests: the row the most recent decode step sampled from, copied to `logits` [B][V] (device): the log-probs
  * log_softmax(llm_decoder output) (llm.py:542) with the sampler's in-place marks, -inf at the eos id while it was masked (min_len) and
  * at the repeated id when the repetition fallback fired.  Rows already done before that step are not sampled and hold the raw head
