@@ -141,6 +141,7 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   CVK_API_BEGIN
   std::string k(key ? key : "");
   if (k == "use_tc") ctx->use_tc = value;
+  else if (k == "flow_fused_ff") ctx->flow_fused_ff = value;
   else if (k == "tc_epi") ctx->tc_epi = value;
   else if (k == "tc_persist") ctx->tc_persist = value;
   else if (k == "op_out_bf16") ctx->op_out_bf16 = value;
@@ -493,6 +494,48 @@ int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, in
     else conv_gemm(ctx, st, a, W, e);
     convert_mat(ctx, st, o, Mat(out, DT_F32, rows, out_ld, out_ld));
     if (out2) convert_mat(ctx, st, o2, Mat(out2, DT_F32, rows, out2_ld, out2_ld));
+    CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+  } catch (...) {
+    release();
+    throw;
+  }
+  release();
+  CVK_API_END
+}
+
+int cvk_op_flow_ff(cvk_ctx* ctx, float* x, int rows, const int* seq_start, const int* seq_len, int B, const float* ln3_g, const float* ln3_b,
+                   const float* w1, const float* b1, const float* w2, const float* b2, const float* ln_g, const float* ln_b, float* out,
+                   void* stream) {
+  CVK_API_BEGIN
+  cudaStream_t st = (cudaStream_t)stream;
+  CVK_REQUIRE(x && rows >= 1 && seq_start && seq_len && B >= 1 && ln3_g && ln3_b && w1 && b1 && w2 && b2 && (!ln_g) == (!ln_b) && out &&
+                  ((uintptr_t)x & 15) == 0,
+              "cvk_op_flow_ff: bad arguments");
+  std::vector<int> row2seq(rows, -1);
+  for (int b = 0; b < B; ++b) {
+    CVK_REQUIRE(seq_len[b] >= 1 && seq_start[b] >= 0 && (long long)seq_start[b] + seq_len[b] <= rows,
+                "cvk_op_flow_ff: empty sequence or sequence outside [0, rows)");
+    for (int i = 0; i < seq_len[b]; ++i) {
+      CVK_REQUIRE(row2seq[seq_start[b] + i] < 0, "cvk_op_flow_ff: sequences overlap");
+      row2seq[seq_start[b] + i] = b;
+    }
+  }
+  ctx->arena.reset();
+  const size_t owned_mark = ctx->owned.size();
+  auto release = [&]() {      // the weight copies live only for this call
+    for (size_t i = owned_mark; i < ctx->owned.size(); ++i) cudaFree(ctx->owned[i]);
+    ctx->owned.resize(owned_mark);
+  };
+  try {
+    const ConvW W1 = make_conv(ctx, w1, b1, 1024, 256, 1, 1, 0), W2 = make_conv(ctx, w2, b2, 256, 1024, 1, 1, 0);
+    CVK_CHECK_CUDA(cudaDeviceSynchronize());   // weight repack runs on the default stream
+    int* d_row2seq = (int*)ctx->arena.alloc(sizeof(int) * (size_t)rows);
+    CVK_CHECK_CUDA(cudaMemcpyAsync(d_row2seq, row2seq.data(), sizeof(int) * (size_t)rows, cudaMemcpyHostToDevice, st));
+    const int adt = ctx->act_dtype;
+    Mat o = arena_mat(ctx, adt, rows, 256), xn = arena_mat(ctx, adt, rows, 256), hid = arena_mat(ctx, adt, rows, 1024);
+    const Mat xm(x, DT_F32, rows, 256, 256);
+    flow_ff(ctx, st, xm, d_row2seq, ln3_g, ln3_b, W1, W2, ln_g, ln_b, o, xn, hid);
+    convert_mat(ctx, st, o, Mat(out, DT_F32, rows, 256, 256));
     CVK_CHECK_CUDA(cudaStreamSynchronize(st));
   } catch (...) {
     release();

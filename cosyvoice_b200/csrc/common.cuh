@@ -255,6 +255,30 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// LayerNorm core of a 256-wide row held by one warp, lane l holding columns 4l..4l+3 (v[0..3]) and 128+4l..128+4l+3 (v[4..7]):
+// mean, biased variance, eps inside the sqrt, then the optional affine.  Every kernel that normalises the flow estimator's rows
+// goes through here, so their results agree bit for bit.
+__device__ __forceinline__ void ln256_warp(float* v, const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int c0, int c1) {
+  const float mean = warp_sum(((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]))) * (1.f / 256.f);
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    v[i] -= mean;
+    q = fmaf(v[i], v[i], q);
+  }
+  const float rstd = rsqrtf(warp_sum(q) * (1.f / 256.f) + eps);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] *= rstd;
+  if (gamma) {
+    const float4 ga = *reinterpret_cast<const float4*>(gamma + c0), gb = *reinterpret_cast<const float4*>(gamma + c1);
+    v[0] *= ga.x; v[1] *= ga.y; v[2] *= ga.z; v[3] *= ga.w; v[4] *= gb.x; v[5] *= gb.y; v[6] *= gb.z; v[7] *= gb.w;
+    if (beta) {
+      const float4 ba = *reinterpret_cast<const float4*>(beta + c0), bb = *reinterpret_cast<const float4*>(beta + c1);
+      v[0] += ba.x; v[1] += ba.y; v[2] += ba.z; v[3] += ba.w; v[4] += bb.x; v[5] += bb.y; v[6] += bb.z; v[7] += bb.w;
+    }
+  }
+}
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

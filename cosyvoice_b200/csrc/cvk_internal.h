@@ -203,6 +203,7 @@ struct cvk_ctx {
   int use_tc_attn = 1;                      // bf16 mode: wgmma attention kernel (0 = CUDA-core flash kernel)
   int use_graph = 1;                        // LM decode step replayed as a CUDA graph
   int use_tc = 1;                           // bf16 mode: route GEMMs to the wgmma kernel (0 = debug: SIMT on converted operands)
+  int flow_fused_ff = 1;                    // bf16 mode: LN3 + ff1 + ff2 (+ next LN1) of a flow-estimator block in one launch (ffn_fused)
 
   void* dmalloc(size_t bytes) {
     void* p = nullptr;
@@ -254,6 +255,15 @@ float* dev_copy_f32(cvk_ctx* ctx, const float* src_dev, size_t n);
 void conv_gemm(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_simt(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
+// flow-estimator feed-forward in one launch (gemm_tc.cu): x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0 in place (x fp32 [rows, 256],
+// ff1 256 -> 1024, ff2 1024 -> 256), then out (bf16 [rows, 256]) <- LN1 of the next block (ln_g, ln_b) or, with ln_g null, x itself
+void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& w1,
+               const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out);
+// x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0, then out <- LN(x; ln_g, ln_b) or, with ln_g null, x in out's dtype (flow.cu): the
+// feed-forward half of a flow-estimator transformer block and the first operand of the next one.  ffn_fused in the bf16 mode with
+// option "flow_fused_ff", otherwise LN3, ff1 and ff2 (+ LN) launches with xn [rows, 256] and hid [rows, 1024] (act dtype) as scratch.
+void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& ff1,
+             const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn, const Mat& hid);
 size_t skinny_scratch_floats(int rows, int maxN);
 const bf16* skinny_tiled_weights(cvk_ctx* ctx, const ConvW& W);
 void skinny_set_carveout();

@@ -278,24 +278,7 @@ __global__ void layernorm256_kernel(const float* __restrict__ x, int ldx, int ro
   } else {
     const float4 a = *reinterpret_cast<const float4*>(xp + c0), b = *reinterpret_cast<const float4*>(xp + c1);
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    const float mean = warp_sum(((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]))) * (1.f / 256.f);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      v[i] -= mean;
-      q = fmaf(v[i], v[i], q);
-    }
-    const float rstd = rsqrtf(warp_sum(q) * (1.f / 256.f) + eps);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] *= rstd;
-    if (gamma) {
-      const float4 ga = *reinterpret_cast<const float4*>(gamma + c0), gb = *reinterpret_cast<const float4*>(gamma + c1);
-      v[0] *= ga.x; v[1] *= ga.y; v[2] *= ga.z; v[3] *= ga.w; v[4] *= gb.x; v[5] *= gb.y; v[6] *= gb.z; v[7] *= gb.w;
-      if (beta) {
-        const float4 ba = *reinterpret_cast<const float4*>(beta + c0), bb = *reinterpret_cast<const float4*>(beta + c1);
-        v[0] += ba.x; v[1] += ba.y; v[2] += ba.z; v[3] += ba.w; v[4] += bb.x; v[5] += bb.y; v[6] += bb.z; v[7] += bb.w;
-      }
-    }
+    ln256_warp(v, gamma, beta, eps, c0, c1);
     if (act == ACT_MISH) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = FAST ? apply_act_fast(ACT_MISH, v[i], 0.f, 1.f) : apply_act(ACT_MISH, v[i], 0.f, 1.f);

@@ -273,6 +273,34 @@ void flow_set_noise(cvk_ctx* ctx, const float* noise_tm, int T, int on_device) {
   m->noise_T = T;
 }
 
+void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& ff1,
+             const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn, const Mat& hid) {
+  if (ctx->flow_fused_ff && ctx->act_dtype == DT_BF16 && ctx->use_tc) {
+    ffn_fused(ctx, st, x, row2seq, ln3_g, ln3_b, ff1, ff2, ln_g, ln_b, out);
+    return;
+  }
+  layernorm(ctx, st, x, ln3_g, ln3_b, 1e-5f, ACT_NONE, 1.f, row2seq, xn);
+  {
+    Epilogue e;
+    e.act1 = ACT_GELU;
+    e.row2seq = row2seq;
+    e.out = hid;
+    conv_gemm(ctx, st, xn, ff1, e);
+  }
+  {
+    Epilogue e;
+    e.resid = x;
+    e.row2seq = row2seq;
+    e.out = x;
+    if (!ln_g) {
+      e.act2 = ACT_NONE;
+      e.out2 = out;
+    }
+    conv_gemm(ctx, st, hid, ff2, e);
+  }
+  if (ln_g) layernorm(ctx, st, x, ln_g, ln_b, 1e-5f, ACT_NONE, 1.f, row2seq, out);
+}
+
 // ================================================================================================ kernels
 namespace {
 
@@ -676,8 +704,11 @@ Mat kv_cache_append(cvk_ctx* ctx, cudaStream_t st, EstInc* inc, const Mat& qkv, 
   return cache;
 }
 
-void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstBuffers& b, int chunk, const Mat* out2, EstInc* inc = nullptr) {
-  layernorm(ctx, st, b.x, t.ln1_g, t.ln1_b, 1e-5f, ACT_NONE, 1.f, s.d_row2seq, b.xn);
+// Every block's first operand is LN1(x) in b.xn; a stage's first block computes it, each later one gets it from the feed-forward
+// half of the block before (flow_ff), which in the bf16 mode is a single launch that never stores the 1024-wide hidden activation.
+void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstBuffers& b, int chunk, const Mat* out2, EstInc* inc,
+            bool first, const TBlockW* next) {
+  if (first) layernorm(ctx, st, b.x, t.ln1_g, t.ln1_b, 1e-5f, ACT_NONE, 1.f, s.d_row2seq, b.xn);
   {
     Epilogue e;
     e.row2seq = s.d_row2seq;
@@ -696,25 +727,8 @@ void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstB
     e.out = b.x;
     conv_gemm(ctx, st, b.att, t.out, e);
   }
-  layernorm(ctx, st, b.x, t.ln3_g, t.ln3_b, 1e-5f, ACT_NONE, 1.f, s.d_row2seq, b.xn);
-  {
-    Epilogue e;
-    e.act1 = ACT_GELU;
-    e.row2seq = s.d_row2seq;
-    e.out = b.ff;
-    conv_gemm(ctx, st, b.xn, t.ff1, e);
-  }
-  {
-    Epilogue e;
-    e.resid = b.x;
-    e.row2seq = s.d_row2seq;
-    e.out = b.x;
-    if (out2) {
-      e.act2 = ACT_NONE;
-      e.out2 = *out2;
-    }
-    conv_gemm(ctx, st, b.ff, t.ff2, e);
-  }
+  flow_ff(ctx, st, b.x, s.d_row2seq, t.ln3_g, t.ln3_b, t.ff1, t.ff2, next ? next->ln1_g : nullptr, next ? next->ln1_b : nullptr,
+          out2 ? *out2 : b.xn, b.xn, b.ff);
 }
 
 // resnet (matcha decoder.py:55-61 with CausalBlock1D) + n transformer blocks.  `in` = act operand [R, Cin];
@@ -745,7 +759,10 @@ void stage_forward(cvk_ctx* ctx, cudaStream_t st, const StageW& w, int stage_idx
     e.out = b.x;
     conv_gemm(ctx, st, in, w.rn.res, e);
   }
-  for (size_t j = 0; j < w.tb.size(); ++j) tblock(ctx, st, w.tb[j], s, b, chunk, j + 1 == w.tb.size() ? &out_act : nullptr, inc);
+  for (size_t j = 0; j < w.tb.size(); ++j) {
+    const bool last = j + 1 == w.tb.size();
+    tblock(ctx, st, w.tb[j], s, b, chunk, last ? &out_act : nullptr, inc, j == 0, last ? nullptr : &w.tb[j + 1]);
+  }
 }
 
 // in0: act [R,320] packed input; t: [B2] device; out: fp32 [R,80] (ld 80)

@@ -475,6 +475,190 @@ void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUten
   conv_gemm_wg_kernel<BN, NSTG><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode, ntn, ntiles);
 }
 
+// ------------------------------------------------------------------------------------------------ fused feed-forward
+// The feed-forward half of a flow-estimator transformer block in one launch (matcha transformer.py: x = x + ff(norm3(x))):
+//   x <- valid(r) ? x + b2 + GELU(LN3(x) W1^T + b1) W2^T : 0,   C = 256 channels, 1024 hidden,
+// followed by the bf16 operand the next launch reads: LN1 of the next block over the new x, or a plain bf16 copy of x (the stage's
+// output activation).  One CTA owns 128 rows; the 1024-wide hidden activation never leaves the SM: per 64-wide hidden chunk a
+// consumer warpgroup computes h = A W1c^T (wgmma, 64 x 64 fp32 in registers), adds the bias, applies the GELU and issues
+// O += h W2c^T with h taken straight from its registers (the accumulator layout is the register A-operand layout).  The producer
+// warp streams the W1 / W2 chunks through a two-stage ring.  Operations and their order are those of the unfused path
+// (layernorm256_kernel, conv_gemm_wg_kernel with the GELU and the residual epilogues: same wgmma K steps in ascending order, same
+// bf16 roundings), so the results agree bit for bit.
+constexpr int FF_C = 256, FF_HID = 1024, FF_HC = 64, FF_NCH = FF_HID / FF_HC;
+constexpr uint32_t FF_A_BYTES = TC_BM * FF_C * 2;      // LN3(x): four SWIZZLE_128B sub-tiles [128 rows][64 channels]
+constexpr uint32_t FF_W1_BYTES = FF_HC * FF_C * 2;     // W1 chunk: four sub-tiles [64 hidden][64 channels]
+constexpr uint32_t FF_W2_BYTES = FF_C * FF_HC * 2;     // W2 chunk: [256 channels][64 hidden]
+constexpr uint32_t FF_STAGE_BYTES = FF_W1_BYTES + FF_W2_BYTES;
+constexpr int FF_NSTG = 2;
+constexpr int FF_OLD = FF_C + 8;                       // pitch (floats) of the fp32 output tile staged over the operand region
+constexpr size_t FF_SMEM = FF_A_BYTES + FF_NSTG * FF_STAGE_BYTES + 1024;
+static_assert((size_t)TC_BM * FF_OLD * 4 <= FF_A_BYTES + FF_NSTG * FF_STAGE_BYTES, "output staging tile must fit the operand region");
+
+struct FfnDev {
+  float* x;                      // [rows][ldx] fp32 residual stream, in place
+  int ldx, rows;
+  const int* row2seq;
+  const float *ln3_g, *ln3_b, *b1, *b2;
+  const float *ln_g, *ln_b;      // LN1 of the next block; null: out is a bf16 copy of x
+  bf16* out;
+  int ldo;
+};
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_w2, FfnDev p) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t bar_full[FF_NSTG];
+  __shared__ __align__(8) uint64_t bar_empty[FF_NSTG];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t w_base = smem_base + FF_A_BYTES;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = blockIdx.x * TC_BM;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < FF_NSTG; ++s) {
+      mbar_init(smem_u32(&bar_full[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      for (int c = 0; c < FF_NCH; ++c) {
+        const uint32_t s = c % FF_NSTG, round = c / FF_NSTG;
+        mbar_wait(smem_u32(&bar_empty[s]), (round & 1u) ^ 1u);
+        const uint32_t sw = w_base + s * FF_STAGE_BYTES;
+        const uint32_t fb = smem_u32(&bar_full[s]);
+        mbar_expect_tx(fb, FF_STAGE_BYTES);
+#pragma unroll
+        for (int kt = 0; kt < FF_C / 64; ++kt) tma_load_2d(sw + kt * (FF_HC * 128u), &tmap_w1, fb, kt * 64, c * FF_HC);
+        tma_load_2d(sw + FF_W1_BYTES, &tmap_w2, fb, c * FF_HC, 0);
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int ct = threadIdx.x - 128;                   // consumer thread 0..255
+  const int wg = ct >> 7;                             // rows [64 wg, 64 wg + 64) of the tile
+  const int cw = ct >> 5;                             // consumer warp 0..7
+  const int c0 = lane * 4, c1 = 128 + lane * 4;       // this lane's columns in the row-per-warp phases
+
+  // LN3 prologue, one warp per row as in layernorm256_kernel: bf16 rows of the A tile (gap rows and rows past the end are zero)
+  for (int i = 0; i < 16; ++i) {
+    const int row = cw * 16 + i, r = r0 + row;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = 0.f;
+    if (r < p.rows && p.row2seq[r] >= 0) {
+      const float* xp = p.x + (size_t)r * p.ldx;
+      const float4 a = *reinterpret_cast<const float4*>(xp + c0), b = *reinterpret_cast<const float4*>(xp + c1);
+      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+      ln256_warp(v, p.ln3_g, p.ln3_b, 1e-5f, c0, c1);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = h ? c1 : c0;
+      __nv_bfloat162 lo = __floats2bfloat162_rn(v[4 * h], v[4 * h + 1]), hi = __floats2bfloat162_rn(v[4 * h + 2], v[4 * h + 3]);
+      const uint32_t addr = smem_base + (uint32_t)(c >> 6) * (TC_BM * 128u) + (uint32_t)row * 128u +
+                            ((((uint32_t)(c & 63) >> 3) ^ (uint32_t)(row & 7)) << 4) + (uint32_t)(c & 7) * 2u;
+      asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(addr), "r"(*reinterpret_cast<uint32_t*>(&lo)), "r"(*reinterpret_cast<uint32_t*>(&hi))
+                   : "memory");
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma operand reads
+  asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");     // this warpgroup's 64 rows are complete
+
+  const int q = lane & 3;
+  float o[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) o[i] = 0.f;
+  uint32_t hp[16];
+  const uint32_t a_wg = smem_base + (uint32_t)wg * (64 * 128u);
+  for (int c = 0; c < FF_NCH; ++c) {
+    const uint32_t s = c % FF_NSTG;
+    mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(c / FF_NSTG) & 1u);
+    const uint32_t sw1 = w_base + s * FF_STAGE_BYTES, sw2 = sw1 + FF_W1_BYTES;
+    float h[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) h[i] = 0.f;
+    wg_fence();
+#pragma unroll
+    for (int kt = 0; kt < FF_C / 64; ++kt) {
+      const uint64_t da = wg_desc_sw128(a_wg + kt * (TC_BM * 128u)), db = wg_desc_sw128(sw1 + kt * (FF_HC * 128u));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<64, 0>(h, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+    }
+    wg_commit();
+    wg_wait<0>();                                     // FF1 of this chunk and FF2 of the previous one have completed
+    wg_touch<32>(h);
+    __syncwarp();
+    if (c > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(c - 1) % FF_NSTG]));
+    // bias + GELU as the FF1 epilogue computes them (act16_fast), bf16 pairs in the register A-operand layout
+    const float* b1 = p.b1 + c * FF_HC + 2 * q;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 b = *reinterpret_cast<const float2*>(b1 + 8 * j);
+      h[4 * j] += b.x; h[4 * j + 1] += b.y; h[4 * j + 2] += b.x; h[4 * j + 3] += b.y;
+    }
+    gelu16_packed(h);
+    gelu16_packed(h + 16);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      __nv_bfloat162 t = __floats2bfloat162_rn(h[2 * j], h[2 * j + 1]);
+      hp[j] = *reinterpret_cast<uint32_t*>(&t);
+    }
+    const uint64_t d2 = wg_desc_sw128(sw2);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < FF_HC / 16; ++kk) wgmma_rs_m64n256(o, hp + 4 * kk, d2 + (uint64_t)(2 * kk), 1);
+    wg_commit();
+  }
+  wg_wait<0>();
+  wg_touch<128>(o);
+  asm volatile("bar.sync 1, 256;" ::: "memory");     // every MMA of the CTA has completed: the operand region is free
+
+  // O + b2 -> fp32 staging tile [128][FF_OLD] over the operand region
+  float* stg = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
+  {
+    const int rb = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int col = 8 * j + 2 * q;
+      const float2 b = *reinterpret_cast<const float2*>(p.b2 + col);
+      *reinterpret_cast<float2*>(stg + rb * FF_OLD + col) = make_float2(o[4 * j] + b.x, o[4 * j + 1] + b.y);
+      *reinterpret_cast<float2*>(stg + (rb + 8) * FF_OLD + col) = make_float2(o[4 * j + 2] + b.x, o[4 * j + 3] + b.y);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  // full rows, one warp per row: + residual, row mask, x out, then LN1 of the next block or the bf16 copy
+  for (int i = 0; i < 16; ++i) {
+    const int row = cw * 16 + i, r = r0 + row;
+    if (r >= p.rows) break;
+    const bool valid = p.row2seq[r] >= 0;
+    float* xp = p.x + (size_t)r * p.ldx;
+    const float* sp = stg + row * FF_OLD;
+    const float4 sa = *reinterpret_cast<const float4*>(sp + c0), sb = *reinterpret_cast<const float4*>(sp + c1);
+    const float4 xa = *reinterpret_cast<const float4*>(xp + c0), xb = *reinterpret_cast<const float4*>(xp + c1);
+    float v[8] = {sa.x + xa.x, sa.y + xa.y, sa.z + xa.z, sa.w + xa.w, sb.x + xb.x, sb.y + xb.y, sb.z + xb.z, sb.w + xb.w};
+    if (!valid) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = 0.f;
+    }
+    *reinterpret_cast<float4*>(xp + c0) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(xp + c1) = make_float4(v[4], v[5], v[6], v[7]);
+    if (p.ln_g && valid) ln256_warp(v, p.ln_g, p.ln_b, 1e-5f, c0, c1);
+    bf16* op = p.out + (size_t)r * p.ldo;
+    __nv_bfloat162 h0 = __floats2bfloat162_rn(v[0], v[1]), h1 = __floats2bfloat162_rn(v[2], v[3]);
+    __nv_bfloat162 h2 = __floats2bfloat162_rn(v[4], v[5]), h3 = __floats2bfloat162_rn(v[6], v[7]);
+    *reinterpret_cast<uint2*>(op + c0) = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+    *reinterpret_cast<uint2*>(op + c1) = make_uint2(*reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
+  }
+}
+
 }  // namespace
 
 void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep) {
@@ -542,6 +726,46 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   }
   if (BN == 128) launch_wg<128, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
   else launch_wg<64, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+}
+
+void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& w1,
+               const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out) {
+  CVK_REQUIRE(x.dtype == DT_F32 && x.cols == FF_C && x.ld % 4 == 0 && ((uintptr_t)x.p & 15) == 0, "ffn_fused: x must be fp32 [rows, 256], 16-byte aligned rows");
+  CVK_REQUIRE(out.dtype == DT_BF16 && out.cols == FF_C && out.rows >= x.rows && out.ld % 8 == 0 && ((uintptr_t)out.p & 15) == 0,
+              "ffn_fused: out must be bf16 [rows, 256], 16-byte aligned rows");
+  CVK_REQUIRE(w1.N == FF_HID && w1.K == FF_C && w1.taps == 1 && w1.w16 && w1.bias && w2.N == FF_C && w2.K == FF_HID && w2.taps == 1 && w2.w16 &&
+                  w2.bias && row2seq && ln3_g && ln3_b && (!ln_g || ln_b),
+              "ffn_fused: unexpected weights");
+  CVK_REQUIRE((((uintptr_t)ln3_g | (uintptr_t)ln3_b | (uintptr_t)ln_g | (uintptr_t)ln_b | (uintptr_t)w1.bias | (uintptr_t)w2.bias) & 15) == 0,
+              "ffn_fused: LayerNorm and bias vectors must be 16-byte aligned");
+  EncodeTiledFn enc = get_encode(ctx);
+  CUtensorMap t1, t2;
+  auto mk = [&](CUtensorMap* m, const bf16* w, int N, int K, int box_n) {
+    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
+    cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+    cuuint32_t box[2] = {64, (cuuint32_t)box_n};
+    cuuint32_t es[2] = {1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<bf16*>(w), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(ffn weights) failed: " + std::to_string((int)r));
+  };
+  mk(&t1, w1.w16, FF_HID, FF_C, FF_HC);
+  mk(&t2, w2.w16, FF_C, FF_HID, FF_C);
+  FfnDev p;
+  p.x = x.f32(); p.ldx = x.ld; p.rows = x.rows; p.row2seq = row2seq;
+  p.ln3_g = ln3_g; p.ln3_b = ln3_b; p.b1 = w1.bias; p.b2 = w2.bias; p.ln_g = ln_g; p.ln_b = ln_b;
+  p.out = out.b16(); p.ldo = out.ld;
+  const double flops = 4.0 * x.rows * (double)FF_C * FF_HID;
+  const double bytes = (double)x.rows * FF_C * (4 + 4 + 2) + 2.0 * FF_C * FF_HID * 2;
+  ProfScope ps(ctx, st, FAM_GEMM_TC, flops, bytes);
+  static bool attr_set = false;
+  if (!attr_set) {
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
+    attr_set = true;
+  }
+  ffn_fused_kernel<<<ceil_div(x.rows, TC_BM), TC_THREADS, FF_SMEM, st>>>(t1, t2, p);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }

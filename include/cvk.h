@@ -69,7 +69,7 @@ int cvk_debug_read(cvk_ctx* ctx, long long* out, int n);
  * the calls made so far - what a caller needs to size cvk_create for its largest batch. */
 int cvk_workspace_bytes(cvk_ctx* ctx, size_t* capacity, size_t* high_water);
 /* Test / measurement switches, NOT part of the drop-in surface (every default is the benchmarked configuration): kernel-variant
- * A/B ("use_tc", "tc_persist", "tc_epi", "use_tc_attn", "enc_tc_attn", "use_skinny",
+ * A/B ("use_tc", "tc_persist", "tc_epi", "use_tc_attn", "enc_tc_attn", "use_skinny", "flow_fused_ff",
  * "lm_fused", "lm_mega", "mega_coop", "pdl", "use_graph", "hift_f16" - the last one takes effect at the next cvk_finalize("hift")),
  * probes ("op_iters", "op_out_bf16", "chain_timeline").  Unknown keys return CVK_ERR_INVALID. */
 int cvk_set_option(cvk_ctx* ctx, const char* key, int value);
@@ -147,6 +147,16 @@ int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, in
                      float act1_param, const float* alpha1, const float* resid, int resid_ld, int resid_is_out, int accumulate,
                      float* out, int out_dtype, int out_ld, int act2, float act2_param, const float* alpha2, float* out2, int out2_dtype,
                      int out2_ld, void* stream);
+/* The feed-forward half of a flow-estimator transformer block with the first operand of the next block (tests), in place on
+ * x [rows, 256] fp32 (device):
+ *   x[r]   = valid(r) ? x[r] + b2 + GELU(LN3(x[r]) w1^T + b1) w2^T : 0,   LN3 = LayerNorm(eps 1e-5; ln3_g, ln3_b)
+ *   out[r] = valid(r) ? LayerNorm(x[r]; ln_g, ln_b) : 0   (ln_g, ln_b NULL: out = x)
+ * rounded to the activation dtype, returned as fp32 [rows, 256].  w1 [1024, 256], b1 [1024], w2 [256, 1024], b2 [256] (torch Linear).
+ * Sequence b occupies rows [seq_start_host[b], + seq_len_host[b]) (inside [0, rows), not overlapping); every other row is a gap row.
+ * bf16 context: one fused launch, or with option "flow_fused_ff" 0 the LayerNorm / GEMM launches the estimator otherwise runs. */
+int cvk_op_flow_ff(cvk_ctx* ctx, float* x, int rows, const int* seq_start_host, const int* seq_len_host, int B, const float* ln3_g,
+                   const float* ln3_b, const float* w1, const float* b1, const float* w2, const float* b2, const float* ln_g,
+                   const float* ln_b, float* out, void* stream);
 /* The conformer relative-position attention (tests): score(i, j) = ((q_i + bias_u) . k_j + (q_i + bias_v) . pos[center - (i - j)]) * scale
  * per head, block-causal when chunk > 0 (key j visible iff j < (i / chunk + 1) * chunk), softmax over the visible keys, times v.
  * q, k, v, out [sum lens, H*64] ragged; pos [2*center+1, H*64] (row t holds relative position center - t; the library pads it to a
