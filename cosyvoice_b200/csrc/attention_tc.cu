@@ -8,7 +8,8 @@ namespace {
 
 constexpr int AT_BQ = 128, AT_BK = 64, AT_HD = 64;    // 128 queries x 64-key tiles
 constexpr int AT_KVST = 3;                             // K/V stages (one key tile each)
-constexpr int AT_THREADS = 384;   // warp 0: TMA producer; warpgroups 1-2: 64 queries each (MMA + softmax)
+constexpr int AT_THREADS = 256;   // attn_wg_kernel: warpgroups 0-1, 64 queries each (MMA + softmax); thread 0 also issues the TMA loads
+constexpr int RP_THREADS = 384;   // relpos_u_kernel: warp 0 TMA producer; warpgroups 1-2 consumers
 constexpr uint32_t Q_BYTES = AT_BQ * AT_HD * 2;        // 16 KB
 constexpr uint32_t K_BYTES = AT_BK * AT_HD * 2;        // 8 KB
 constexpr uint32_t V_BYTES = AT_BK * AT_HD * 2;        // 8 KB
@@ -26,7 +27,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+// true once the phase of the given parity has completed (one bounded try, no spinning)
+__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
   uint32_t ok = 0;
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -35,17 +37,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       : "=r"(ok)
       : "r"(bar), "r"(parity)
       : "memory");
-  if (ok) return;            // fast path without clock reads
+  return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  if (mbar_test(bar, parity)) return;            // fast path without clock reads
   const long long t0 = clock64();
   for (;;) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
+    if (mbar_test(bar, parity)) return;
     if (clock64() - t0 > 4000000000ll) break;
   }
   __trap();
@@ -57,8 +55,9 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
-// One CTA = 128 queries of one (sequence, head), 384 threads: warp 0 of warpgroup 0 is the TMA producer (Q once, then K/V
-// 64-key tiles through a three-stage ring), warpgroups 1 and 2 own 64 queries each.  Per key tile a consumer warpgroup computes
+// One CTA = 128 queries of one (sequence, head), 256 threads: warpgroups 0 and 1 own 64 queries each, and thread 0 also issues
+// the TMA loads (Q once, then K/V 64-key tiles through a three-stage ring).  Without a producer warp the plain kernel fits in 128
+// registers, so two CTAs share an SM and one CTA's softmax runs under the other's MMAs.  Per key tile a consumer warpgroup computes
 // S = Q K^T (wgmma, 64 x 64 fp32 in registers), applies mask / bias and an online softmax in registers (the four threads of a
 // quad share a row: row maxima and sums are quad shuffles), rescales its O accumulator and issues O += P V with P taken straight
 // from the S registers (the accumulator layout of S is the register A-operand layout of the P V MMA) and V consumed MN-major
@@ -66,6 +65,11 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 // BIAS: an additive score term read from global memory, bias(i, j) = ubias[((s0 + i) * H + h) * ldu + ucenter - i + j]: the
 // relative-position term of the conformer attention (transformer/attention.py:249-330), where row t of U = (q + pos_bias_v) p[t]^T
 // has been produced by relpos_u_kernel and the reference's rel_shift (attention.py:225-247) is the index map (i, j) -> center - (i - j).
+// Work that cannot change a stored row is skipped: a warpgroup whose 64 rows all lie at or past L returns at once (the K/V stages
+// are then released by the 4 warps that consume), and the key mask / -inf select run only on the key tiles that reach past the
+// smallest key limit of the warp's 16 rows.  Every stored value goes through the same operations in the same order either way.
+// The row sum takes the rescale and the tile's first P in one fma, lsum = fma(lsum, f, p) + p' + ...: the rounding this kernel
+// has always had (the compiler contracted lsum * f + p), written out so that changes around it cannot move the contraction.
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h2);
@@ -80,7 +84,7 @@ __device__ __forceinline__ float quad_sum(float v) {
 }
 
 template <bool BIAS>
-__global__ void __launch_bounds__(AT_THREADS, 1)
+__global__ void __launch_bounds__(AT_THREADS, BIAS ? 1 : 2)
 attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk, const __grid_constant__ CUtensorMap tmv,
                const int* __restrict__ start, const int* __restrict__ len, int chunk, float scale_log2e, int kv_div,
                bf16* __restrict__ out, int ldo, const int* __restrict__ kstart, const int* __restrict__ klen, const int* __restrict__ qoff,
@@ -101,33 +105,42 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
   const int i_last = q0 + min(i0 + AT_BQ, L) - 1;
   const int kmax = chunk > 0 ? min(Lk, (i_last / chunk + 1) * chunk) : Lk;
   const int G = (kmax + AT_BK - 1) / AT_BK;
+  const int wg = threadIdx.x >> 7;      // warpgroup 0 always has a valid row (i0 < L); warpgroup 1 only if i0 + 64 < L
 
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(&bar_q), 1);
     for (int s = 0; s < AT_KVST; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
+      mbar_init(smem_u32(&bar_empty[s]), i0 + 64 < L ? 8 : 4);     // one arrival per consuming warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  if (i0 + wg * 64 >= L) return;        // all 64 rows padded: nothing of this warpgroup is stored
 
-  if (warp < 4) {
-    if (warp == 0 && lane == 0) {
-      mbar_expect_tx(smem_u32(&bar_q), Q_BYTES);
-      tma_load_2d(sQ, &tmq, smem_u32(&bar_q), h * AT_HD, s0 + i0);
-      for (int g = 0; g < G; ++g) {
-        const int st = g % AT_KVST;
-        mbar_wait(smem_u32(&bar_empty[st]), (uint32_t)(((g / AT_KVST) & 1) ^ 1));
-        const uint32_t fb = smem_u32(&bar_full[st]);
-        mbar_expect_tx(fb, KV_STAGE);
-        tma_load_2d(sKV + st * KV_STAGE, &tmk, fb, (h / kv_div) * AT_HD, ks0 + g * AT_BK);
-        tma_load_2d(sKV + st * KV_STAGE + K_BYTES, &tmv, fb, (h / kv_div) * AT_HD, ks0 + g * AT_BK);
+  // Thread 0 produces: Q once, then K/V tile t into stage t % AT_KVST once every consuming warp has released the tile t - AT_KVST
+  // that used it.  It blocks on that release only when the consumers need tile t now (t == g); otherwise it tries again later.
+  int nx = 0;                           // next K/V tile to load (thread 0)
+  auto produce = [&](int g) {
+    for (; nx < G && nx < g + AT_KVST; ++nx) {
+      const int st = nx % AT_KVST;
+      const uint32_t eb = smem_u32(&bar_empty[st]), par = (uint32_t)(((nx / AT_KVST) & 1) ^ 1);
+      if (nx > g) {
+        if (!mbar_test(eb, par)) break;
+      } else {
+        mbar_wait(eb, par);
       }
+      const uint32_t fb = smem_u32(&bar_full[st]);
+      mbar_expect_tx(fb, KV_STAGE);
+      tma_load_2d(sKV + st * KV_STAGE, &tmk, fb, (h / kv_div) * AT_HD, ks0 + nx * AT_BK);
+      tma_load_2d(sKV + st * KV_STAGE + K_BYTES, &tmv, fb, (h / kv_div) * AT_HD, ks0 + nx * AT_BK);
     }
-    return;
+  };
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(smem_u32(&bar_q), Q_BYTES);
+    tma_load_2d(sQ, &tmq, smem_u32(&bar_q), h * AT_HD, s0 + i0);
   }
-  const int wg = (threadIdx.x - 128) >> 7;
+
   const int q = lane & 3;
   const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // tile rows rbase (h = 0) and rbase + 8 (h = 1)
   int ii[2], klim[2];
@@ -136,6 +149,8 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
     ii[hh] = i0 + rbase + 8 * hh;
     klim[hh] = ii[hh] < L ? (chunk > 0 ? min(Lk, ((q0 + ii[hh]) / chunk + 1) * chunk) : Lk) : 0;
   }
+  // key tiles that end at or before the smallest key limit of the warp's 16 rows need no mask (warp-uniform)
+  const int kfree = __reduce_min_sync(0xffffffffu, min(klim[0], klim[1]));
   const uint64_t dq = wg_desc_sw128(sQ + (uint32_t)wg * (Q_BYTES / 2));
   float o[32], m_run[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
 #pragma unroll
@@ -144,6 +159,9 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
   for (int g = 0; g < G; ++g) {
     const int st = g % AT_KVST;
     const int j0 = g * AT_BK;
+    const bool masked = j0 + AT_BK > kfree;
+    if (threadIdx.x == 0) produce(g);
+    __syncwarp();
     float bia[BIAS ? 32 : 1];
     if (BIAS) {       // issued before the score MMA: the two latencies overlap
 #pragma unroll
@@ -163,16 +181,27 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
 #pragma unroll
     for (int k = 0; k < AT_HD / 16; ++k) wgmma_ss<64, 0>(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), 1);
     wg_commit();
+    if (threadIdx.x == 0) produce(g);    // stages released meanwhile: never blocks here (tile g is already loaded)
+    __syncwarp();
     wg_wait<0>();
     wg_touch<32>(s);
     // s[e]: row rbase + 8 ((e >> 1) & 1), key j0 + 8 (e >> 2) + 2 q + (e & 1)
     float tm[2] = {-INFINITY, -INFINITY};
+    if (masked) {
 #pragma unroll
-    for (int e = 0; e < 32; ++e) {
-      const int hh = (e >> 1) & 1, j = j0 + 8 * (e >> 2) + 2 * q + (e & 1);
-      if (BIAS) s[e] += bia[e];
-      if (j >= klim[hh]) s[e] = -INFINITY;
-      tm[hh] = fmaxf(tm[hh], s[e]);
+      for (int e = 0; e < 32; ++e) {
+        const int hh = (e >> 1) & 1, j = j0 + 8 * (e >> 2) + 2 * q + (e & 1);
+        if (BIAS) s[e] += bia[e];
+        if (j >= klim[hh]) s[e] = -INFINITY;
+        tm[hh] = fmaxf(tm[hh], s[e]);
+      }
+    } else {
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        const int hh = (e >> 1) & 1;
+        if (BIAS) s[e] += bia[e];
+        tm[hh] = fmaxf(tm[hh], s[e]);
+      }
     }
     float f[2], mneg[2];
 #pragma unroll
@@ -182,15 +211,25 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
       f[hh] = m_run[hh] == -INFINITY ? 1.f : fast_ex2(m_run[hh] - mn);   // nothing accumulated yet: o and lsum are 0
       m_run[hh] = mn;
       mneg[hh] = mn == -INFINITY ? 0.f : -mn;
-      lsum[hh] *= f[hh];
     }
+    if (masked) {
 #pragma unroll
-    for (int e = 0; e < 32; ++e) {
-      const int hh = (e >> 1) & 1;
-      const float p = s[e] == -INFINITY ? 0.f : fast_ex2(fmaf(s[e], scale_log2e, mneg[hh]));
-      s[e] = p;
-      lsum[hh] += p;
-      o[e] *= f[hh];
+      for (int e = 0; e < 32; ++e) {
+        const int hh = (e >> 1) & 1;
+        const float p = s[e] == -INFINITY ? 0.f : fast_ex2(fmaf(s[e], scale_log2e, mneg[hh]));
+        s[e] = p;
+        lsum[hh] = e < 4 && !(e & 1) ? fmaf(lsum[hh], f[hh], p) : lsum[hh] + p;   // rescale fused into the row's first add
+        o[e] *= f[hh];
+      }
+    } else {      // no -inf from the mask here (an overflowed score of -inf still gives ex2(-inf) = +0)
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        const int hh = (e >> 1) & 1;
+        const float p = fast_ex2(fmaf(s[e], scale_log2e, mneg[hh]));
+        s[e] = p;
+        lsum[hh] = e < 4 && !(e & 1) ? fmaf(lsum[hh], f[hh], p) : lsum[hh] + p;   // rescale fused into the row's first add
+        o[e] *= f[hh];
+      }
     }
     uint32_t pa[4][4];      // P as the A operand of 4 K16 steps: rows rbase / rbase + 8, keys 16 kk + 2 q (+8)
 #pragma unroll
@@ -227,7 +266,7 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ 
 // U[(s0 + i) * H + h][t] = (q_i + pos_bias_v)_h . p[t]_h for the table rows t that query tile i0 can address (t = center - (i - j),
 // j < L): one CTA per (query tile, head, sequence), 64-row tiles of the position table through the same TMA / wgmma pipeline as
 // the score MMA of the attention kernel; each consumer warpgroup writes the fp32 rows of its 64 queries.
-__global__ void __launch_bounds__(AT_THREADS, 1)
+__global__ void __launch_bounds__(RP_THREADS, 1)
 relpos_u_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmp, const int* __restrict__ start,
                 const int* __restrict__ len, int center, int pos_rows, float* __restrict__ U, int ldu) {
   extern __shared__ uint8_t smem_raw[];
@@ -336,6 +375,11 @@ void attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& q, const Mat& k,
   static bool attr = false;
   if (!attr) {
     CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+    // the kernel relies on two co-resident CTAs per SM to hide its serial MMA -> softmax -> MMA chain: a register or shared
+    // memory increase that loses the second CTA is an error, not a silent slowdown
+    int per_sm = 0;
+    CVK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_wg_kernel<false>, AT_THREADS, AT_SMEM));
+    CVK_REQUIRE(per_sm >= 2, "attn_wg_kernel: " + std::to_string(per_sm) + " CTA(s) per SM, laid out for 2");
     attr = true;
   }
   dim3 grid(ceil_div(s.max_len, AT_BQ), H, s.B);
@@ -368,7 +412,7 @@ void relpos_attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& qu, const
     attr = true;
   }
   dim3 grid(ceil_div(s.max_len, AT_BQ), H, s.B);
-  relpos_u_kernel<<<grid, AT_THREADS, AT_SMEM, st>>>(tqv, tp, s.d_start, s.d_len, pos_center, pos_rows, U.f32(), U.ld);
+  relpos_u_kernel<<<grid, RP_THREADS, AT_SMEM, st>>>(tqv, tp, s.d_start, s.d_len, pos_center, pos_rows, U.f32(), U.ld);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   attn_wg_kernel<true><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, 1, out.b16(), out.ld,
