@@ -50,6 +50,8 @@ void llm_ras_sample(cvk_ctx* ctx, float* logp, int B, int V, const int32_t* hist
                     const float* uniforms, const int32_t* ignore_eos, int32_t* out_ids, cudaStream_t st);
 void llm_decode_attention_op(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
                              const int* ctx_len_host, int max_ctx, float* out, cudaStream_t st);
+void llm_decode_layers_op(cvk_ctx* ctx, int B, const int* ctx_len_host, int max_ctx, float* x, float* k_cache, float* v_cache,
+                          float* xn_out, float* att_out, float* ffa_out, cudaStream_t st);
 void llm_sample_step_op(cvk_ctx* ctx, float* logits, int B, int V, const float* uniforms, const int32_t* min_len, const int32_t* max_len,
                         int32_t* out_ids, int out_ld, int32_t* out_count, int32_t* done, int* ctx_len, const int* base_len, int* live,
                         const float* speech_emb, float* next_x, const float* gamma, float* xn, cudaStream_t st);
@@ -395,6 +397,20 @@ int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int 
               "cvk_op_decode_attention: bad arguments (bf16 context)");
   for (int b = 0; b < rows; ++b) CVK_REQUIRE(ctx_len[b] >= 0 && ctx_len[b] < max_ctx, "cvk_op_decode_attention: ctx_len outside [0, max_ctx)");
   llm_decode_attention_op(ctx, partial, splits, rows, bias, k_cache, v_cache, ctx_len, max_ctx, out, (cudaStream_t)stream);
+  CVK_API_END
+}
+
+int cvk_op_lm_decode_layers(cvk_ctx* ctx, int B, const int* ctx_len_host, int max_ctx, float* x, float* k_cache, float* v_cache,
+                            float* xn_out, float* att_out, float* ffa_out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(ctx_len_host && x && k_cache && v_cache && xn_out && ctx->precision == CVK_PREC_BF16,
+              "cvk_op_lm_decode_layers: bad arguments (bf16 context)");
+  CVK_REQUIRE(ctx->llm, "cvk_op_lm_decode_layers: llm stage not finalised");
+  CVK_REQUIRE(B >= 1 && B <= 64, "cvk_op_lm_decode_layers: B outside [1, 64]");
+  // the decode attention kernel holds the scores of max_ctx positions for its 7 query heads in shared memory (decode_attn_allow_ctx)
+  CVK_REQUIRE(max_ctx >= 1 && 7 * (size_t)max_ctx * sizeof(float) <= 200 * 1024, "cvk_op_lm_decode_layers: max_ctx beyond the decode attention limit");
+  for (int b = 0; b < B; ++b) CVK_REQUIRE(ctx_len_host[b] >= 0 && ctx_len_host[b] < max_ctx, "cvk_op_lm_decode_layers: ctx_len outside [0, max_ctx)");
+  llm_decode_layers_op(ctx, B, ctx_len_host, max_ctx, x, k_cache, v_cache, xn_out, att_out, ffa_out, (cudaStream_t)stream);
   CVK_API_END
 }
 

@@ -1326,39 +1326,25 @@ static bool lm_fused_path(cvk_ctx* ctx, cvk_lm_session* s) {
   return s->kv_dtype == DT_BF16 && ctx->use_tc && ctx->use_skinny && ctx->lm_fused && s->g_B <= 64;
 }
 
-// bf16 decode step with fused kernels: 2 + 7 launches per layer instead of 2 + 12
-static void decode_step_fused(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) {
+// The layers of a bf16 decode step on the fused path: x (residual stream) and xn = RMSNorm(x) ln1[0] in -> x, xn = the final-normed
+// hidden state out; every layer appends its K / V row at ctx_len.  Persistent kernel when it can run, else the PDL chain of 7
+// launches per layer.  decode_step_fused runs it after the sampler, cvk_op_lm_decode_layers on caller state.
+static void decode_layers_fused(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) {
   const LlmModel* m = ctx->llm;
   const int B = s->g_B;
-  const bool fused = true;
-  ctx->tl_seq = 0;
-  Mat x(s->x, DT_F32, B, D, D), xn(s->xn, DT_BF16, B, D, D), att(s->att, DT_BF16, B, D, D), ffa(s->ffa, DT_BF16, B, DFF, DFF),
-      logits(s->logits, DT_F32, B, m->vout, m->vout);
-  {
-    Epilogue e;
-    e.out = logits;
-    conv_gemm_skinny_ex(ctx, st, xn, m->head, e, s->scratch, s->scratch_floats, 0);
-  }
-  const bool pdl = ctx->pdl != 0;
-  launch_ex(ras_sampler_kernel, dim3(B), dim3(SAMPLER_THREADS), sampler_smem(m->vout), st, pdl, s->logits, m->vout, 1, s->g_uniforms, B, s->g_min,
-            s->g_max, s->g_out_ids, s->g_out_ld, s->g_out_count, s->g_done, s->ctx_len, (const int*)s->base_len, s->live,
-            (const float*)m->speech_emb, s->x, (const int32_t*)nullptr, 0, (const int32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr,
-            (const float*)(fused ? m->layers[0].ln1 : nullptr), fused ? (bf16*)s->xn : (bf16*)nullptr, ctx->tl_next(),
-            ctx->tl ? (long long*)ctx->tl + 1024 : (long long*)nullptr);
-  ctx->launches++;
-  CVK_LAUNCH_CHECK();
   if (lm_mega_usable(ctx, s, B)) {     // all layers in one persistent cooperative kernel (llm_mega.cu)
     lm_mega_layers(ctx, st, s, B);
     return;
   }
-  const size_t attn_smem = ((NH / NKV + 2) * HD + AF_WARPS * 8 * 2 + AF_WARPS * (NH / NKV) * HD) * sizeof(float);
+  const bool pdl = ctx->pdl != 0;
+  Mat xn(s->xn, DT_BF16, B, D, D), att(s->att, DT_BF16, B, D, D), ffa(s->ffa, DT_BF16, B, DFF, DFF);
   for (int li = 0; li < m->num_layers; ++li) {
     const LayerW& w = m->layers[li];
     bf16* kc = (bf16*)s->kcache + (size_t)li * s->max_batch * NKV * s->max_ctx * HD;
     bf16* vc = (bf16*)s->vcache + (size_t)li * s->max_batch * NKV * s->max_ctx * HD;
     Epilogue none;
     int sp = conv_gemm_skinny_ex(ctx, st, xn, w.qkv, none, s->scratch, s->scratch_floats, 1);
-    launch_ex(attn_fused_kernel, dim3(B, NKV), dim3(32 * AF_WARPS), attn_smem, st, pdl, (const float*)s->scratch, sp, B,
+    launch_ex(attn_fused_kernel, dim3(B, NKV), dim3(32 * AF_WARPS), ATTN_FUSED_SMEM, st, pdl, (const float*)s->scratch, sp, B,
               (const float*)w.qkv.bias, kc, vc, (const int*)s->ctx_len, s->max_ctx, (const float*)m->d_inv_freq, att.b16(), att.ld, ctx->tl_next());
     ctx->launches++;
     CVK_LAUNCH_CHECK();
@@ -1377,6 +1363,29 @@ static void decode_step_fused(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) 
     ctx->launches++;
     CVK_LAUNCH_CHECK();
   }
+}
+
+// bf16 decode step with fused kernels: 2 + 7 launches per layer instead of 2 + 12
+static void decode_step_fused(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) {
+  const LlmModel* m = ctx->llm;
+  const int B = s->g_B;
+  const bool fused = true;
+  ctx->tl_seq = 0;
+  Mat xn(s->xn, DT_BF16, B, D, D), logits(s->logits, DT_F32, B, m->vout, m->vout);
+  {
+    Epilogue e;
+    e.out = logits;
+    conv_gemm_skinny_ex(ctx, st, xn, m->head, e, s->scratch, s->scratch_floats, 0);
+  }
+  const bool pdl = ctx->pdl != 0;
+  launch_ex(ras_sampler_kernel, dim3(B), dim3(SAMPLER_THREADS), sampler_smem(m->vout), st, pdl, s->logits, m->vout, 1, s->g_uniforms, B, s->g_min,
+            s->g_max, s->g_out_ids, s->g_out_ld, s->g_out_count, s->g_done, s->ctx_len, (const int*)s->base_len, s->live,
+            (const float*)m->speech_emb, s->x, (const int32_t*)nullptr, 0, (const int32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr,
+            (const float*)(fused ? m->layers[0].ln1 : nullptr), fused ? (bf16*)s->xn : (bf16*)nullptr, ctx->tl_next(),
+            ctx->tl ? (long long*)ctx->tl + 1024 : (long long*)nullptr);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+  decode_layers_fused(ctx, st, s);
 }
 
 static void decode_step(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) {
@@ -1474,6 +1483,54 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
     CVK_CHECK_CUDA(cudaMemcpyAsync(live_host, s->live, sizeof(int), cudaMemcpyDeviceToHost, st));
     CVK_CHECK_CUDA(cudaStreamSynchronize(st));
   }
+}
+
+// The layers of one decode step on caller state (cvk_op_lm_decode_layers), on a temporary session of B rows x max_ctx positions:
+// the layer loop cvk_lm_decode runs after the sampler, on the path the step would take (decode_step: the fused chain or the persistent
+// kernel, else the per-op loop).  x [B][896] fp32 in / out; the caches [layers][B][2][max_ctx][64] cross the call as fp32 and run as
+// bf16, each layer appending its row at ctx_len_host[b]; xn_out [B][896] the bf16 final-normed row the step hands to the head;
+// att_out [B][896] / ffa_out [B][4864] (nullable) the last layer's o_proj / down_proj operands, which every path leaves in the session's
+// att / ffa buffers.  The entry xn = RMSNorm(x) ln1[0], which the sampler computes in a step, comes from the path's own norm kernel.
+void llm_decode_layers_op(cvk_ctx* ctx, int B, const int* ctx_len_host, int max_ctx, float* x, float* k_cache, float* v_cache,
+                          float* xn_out, float* att_out, float* ffa_out, cudaStream_t st) {
+  const LlmModel* m = ctx->llm;
+  ctx->arena.reset();
+  cvk_lm_session* s = llm_session_create(ctx, B, max_ctx);
+  try {
+    s->B = s->g_B = B;
+    const int cache_rows = m->num_layers * B * NKV * max_ctx;
+    Mat k32(k_cache, DT_F32, cache_rows, HD, HD), v32(v_cache, DT_F32, cache_rows, HD, HD);
+    Mat kc(s->kcache, DT_BF16, cache_rows, HD, HD), vc(s->vcache, DT_BF16, cache_rows, HD, HD);
+    Mat xs(s->x, DT_F32, B, D, D), xn(s->xn, DT_BF16, B, D, D), att(s->att, DT_BF16, B, D, D), ffa(s->ffa, DT_BF16, B, DFF, DFF);
+    CVK_CHECK_CUDA(cudaMemcpyAsync(s->ctx_len, ctx_len_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+    CVK_CHECK_CUDA(cudaMemcpyAsync(s->x, x, sizeof(float) * (size_t)B * D, cudaMemcpyDeviceToDevice, st));
+    convert_mat(ctx, st, k32, kc);
+    convert_mat(ctx, st, v32, vc);
+    if (lm_fused_path(ctx, s)) {
+      // no split to add: finish_rms_kernel is the plain RMSNorm of x
+      launch_ex(finish_rms_kernel, dim3(B), dim3(D), 0, st, ctx->pdl != 0, (const float*)s->scratch, 0, B, s->x, (const float*)m->layers[0].ln1,
+                xn.b16(), (long long*)nullptr);
+      ctx->launches++;
+      CVK_LAUNCH_CHECK();
+      decode_layers_fused(ctx, st, s);
+    } else {
+      Mat qkv(s->qkv, DT_BF16, B, QKV_N, QKV_N), gu(s->gu, DT_BF16, B, 2 * DFF, 2 * DFF);
+      for (int li = 0; li < m->num_layers; ++li) layer_forward(ctx, st, m, li, xs, xn, qkv, att, gu, ffa, nullptr, s, true);
+      rmsnorm(ctx, st, xs, m->final_norm, RMS_EPS, xn);     // what head_logits does at the next step
+    }
+    CVK_CHECK_CUDA(cudaMemcpyAsync(x, s->x, sizeof(float) * (size_t)B * D, cudaMemcpyDeviceToDevice, st));
+    convert_mat(ctx, st, kc, k32);
+    convert_mat(ctx, st, vc, v32);
+    convert_mat(ctx, st, xn, Mat(xn_out, DT_F32, B, D, D));
+    if (att_out) convert_mat(ctx, st, att, Mat(att_out, DT_F32, B, D, D));
+    if (ffa_out) convert_mat(ctx, st, ffa, Mat(ffa_out, DT_F32, B, DFF, DFF));
+    CVK_CHECK_CUDA(cudaStreamSynchronize(st));
+  } catch (...) {
+    cudaStreamSynchronize(st);
+    llm_session_destroy(ctx, s);
+    throw;
+  }
+  llm_session_destroy(ctx, s);
 }
 
 // ---------------------------------------------------------------------------------------------- incremental feeding

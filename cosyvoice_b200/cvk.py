@@ -48,6 +48,7 @@ SIGNATURES = {
                                            ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_op_decode_attention": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_op_ragged_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _c_int_p, ctypes.c_int, _vp, _vp]),
+    "cvk_op_lm_decode_layers": (ctypes.c_int, [_vp, ctypes.c_int, _c_int_p, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cvk_op_conv_gemm": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_int_p, _c_int_p, ctypes.c_int,
                                         _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp,
                                         _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -276,6 +277,21 @@ class Context:
         self._check(self.lib.cvk_op_decode_attention(self.h, _ptr(partial), splits, rows, _ptr(bias), _ptr(k_cache), _ptr(v_cache),
                                                      _ints(ctx_len), k_cache.shape[2], _ptr(out), _stream()))
         return out, k_cache, v_cache
+
+    def lm_decode_layers(self, x, k_cache, v_cache, ctx_len):
+        """every layer of the loaded LM for one decode step (cvk_op_lm_decode_layers): x [B, 896] residual stream, caches
+        [layers, B, 2, max_ctx, 64], ctx_len [B] (python ints, the new row's position).  Returns copies (x, k_cache, v_cache) updated
+        by the step and (xn [B, 896], att [B, 896], ffa [B, 4864]): the final-normed row and the last layer's o_proj / down_proj
+        operands."""
+        x = _f32(x, self.device).clone()
+        k_cache, v_cache = _f32(k_cache, self.device).clone(), _f32(v_cache, self.device).clone()
+        B = x.shape[0]
+        xn = torch.empty(B, 896, device=self.device)
+        att = torch.empty(B, 896, device=self.device)
+        ffa = torch.empty(B, 4864, device=self.device)
+        self._check(self.lib.cvk_op_lm_decode_layers(self.h, B, _ints(ctx_len), k_cache.shape[3], _ptr(x), _ptr(k_cache), _ptr(v_cache),
+                                                     _ptr(xn), _ptr(att), _ptr(ffa), _stream()))
+        return x, k_cache, v_cache, (xn, att, ffa)
 
     def ragged_attention(self, q, k_cache, v_cache, rowpos):
         """the feed attention of cvk_lm_feed_rows (cvk_op_ragged_attention): q [M, 896], caches [rows, 2, max_ctx, 64], rowpos: M python

@@ -124,6 +124,17 @@ int cvk_op_ragged_attention(cvk_ctx* ctx, const float* q, const float* k_cache, 
                             const int* rowpos_host, int M, float* out, void* stream);
 int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int rows, const float* bias, float* k_cache, float* v_cache,
                             const int* ctx_len_host, int max_ctx, float* out, void* stream);
+/* Every layer of the finalised "llm" stage for one decode step on caller state, bf16 context only: the layer loop cvk_lm_decode runs
+ * after the sampler, on a temporary session of B x max_ctx.  x [B][896] fp32 residual stream, in / out; k_cache, v_cache
+ * [layers][B][2][max_ctx][64] fp32, in / out (run as bf16, as in a session; layer l appends row b at position ctx_len_host[b]);
+ * xn_out [B][896] the bf16 final-normed row the step hands to the head; att_out [B][896] and ffa_out [B][4864] (nullable) the last
+ * layer's attention output and SwiGLU output, the bf16 operands of its o_proj and down_proj.  The options choose the path as in
+ * cvk_lm_decode: "lm_fused" 1 the fused chain ("lm_mega" 1: the persistent kernel), "lm_fused" 0 the per-op chain ("use_skinny" 0: the
+ * tiled GEMMs); "pdl" is honoured.  The entry xn = RMSNorm(x) ln1[0] comes from the path's own norm kernel.  An fp32 context, an
+ * unfinalised stage, B outside [1, 64], ctx_len outside [0, max_ctx) and max_ctx beyond the decode-attention limit are refused with
+ * CVK_ERR_INVALID before any device work. */
+int cvk_op_lm_decode_layers(cvk_ctx* ctx, int B, const int* ctx_len_host, int max_ctx, float* x, float* k_cache, float* v_cache,
+                            float* xn_out, float* att_out, float* ffa_out, void* stream);
 /* element types of the cvk_op_conv_gemm operand and outputs */
 #define CVK_DT_F32 0
 #define CVK_DT_BF16 1

@@ -104,6 +104,57 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, ctx_len):
     return out
 
 
+# ------------------------------------------------------------------------------------------------ LM decode layer
+LM_D, LM_DFF = olm.D, olm.D_FF              # 896, 4864
+LAYER_ROUNDING = {
+    # where a decode path stores a bf16 value that the next stage reads: the fused chain and the persistent kernel keep the qkv and
+    # gate/up projections in fp32 (split-K partial sums reduced by the attention unit, SwiGLU in the GEMM epilogue); the per-op chain
+    # stores both as bf16 first
+    None: (),
+    "fused": ("xn", "qkv_rot", "att", "ffa"),
+    "per-op": ("xn", "qkv", "qkv_rot", "att", "gu", "ffa"),
+}
+
+
+def rms_norm(x, g):
+    """RMSNorm (eps 1e-6) of the rows of x times g, in fp64"""
+    x = x.double()
+    return g.double() * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + olm.RMS_EPS))
+
+
+def layer_weights(sd, i):
+    """layer i of an oracle-style LM state dict, in the kernels' grouping: ln1, wqkv [1152, 896], bqkv, wo, ln2, wg, wu, wd"""
+    p = f"llm.model.model.layers.{i}"
+    return dict(ln1=sd[p + ".input_layernorm.weight"], ln2=sd[p + ".post_attention_layernorm.weight"],
+                wqkv=torch.cat([sd[f"{p}.self_attn.{n}_proj.weight"] for n in "qkv"]),
+                bqkv=torch.cat([sd[f"{p}.self_attn.{n}_proj.bias"] for n in "qkv"]),
+                wo=sd[p + ".self_attn.o_proj.weight"], wg=sd[p + ".mlp.gate_proj.weight"], wu=sd[p + ".mlp.up_proj.weight"],
+                wd=sd[p + ".mlp.down_proj.weight"])
+
+
+def decode_layer(w, x, k_cache, v_cache, ctx_len, rounding=None):
+    """One Qwen2 decoder layer (modeling_qwen2.py: RMSNorm -> q/k/v + bias -> RoPE -> GQA attention over the cache and the new row ->
+    o_proj + residual -> RMSNorm -> SwiGLU -> down_proj + residual) for one decode step of `rows` independent rows, in fp64.
+    w: layer_weights(...) (the kernels hold the weights as bf16: give bf16-representable ones); x [rows, 896] the residual stream;
+    caches [rows, 2, max_ctx, 64] holding ctx_len[b] history rows (not modified: the new rows are returned); the new token sits at
+    position ctx_len[b].  rounding: None (exact), "fused" or "per-op": the values that path stores as bf16 before the next stage reads
+    them are rounded here too (LAYER_ROUNDING).  Returns every stage: xn, qkv, q, k, v (rotated; k, v are the cache rows), att, x_mid,
+    xn_mid, g, u, ffa, x_out."""
+    r = LAYER_ROUNDING[rounding]
+    rd = lambda t, what: bf16(t) if what in r else t
+    W = {k: v.double() for k, v in w.items()}
+    xn = rd(rms_norm(x, W["ln1"]), "xn")
+    qkv = rd(xn @ W["wqkv"].t() + W["bqkv"][None], "qkv")
+    q, k, v = decode_qkv(qkv[None], torch.zeros(QKV_N, dtype=torch.float64), ctx_len, round_bf16="qkv_rot" in r)
+    att = rd(decode_attention(q, k, v, k_cache, v_cache, ctx_len), "att")
+    x_mid = x.double() + att @ W["wo"].t()
+    xn_mid = rd(rms_norm(x_mid, W["ln2"]), "xn")
+    g, u = rd(xn_mid @ W["wg"].t(), "gu"), rd(xn_mid @ W["wu"].t(), "gu")
+    ffa = rd(g / (1.0 + torch.exp(-g)) * u, "ffa")
+    x_out = x_mid + ffa @ W["wd"].t()
+    return dict(xn=xn, qkv=qkv, q=q, k=k, v=v, att=att, x_mid=x_mid, xn_mid=xn_mid, g=g, u=u, ffa=ffa, x_out=x_out)
+
+
 # ------------------------------------------------------------------------------------------------ conv-GEMM and its epilogue
 def act(name, x, param=0.0, alpha=None):
     """the epilogue activations in x's dtype, written from their definitions: GELU with erf, GELU's tanh form

@@ -78,6 +78,60 @@ def test_decode_ref_equals_oracle_step(past_len):
     assert (hid[0].double() - want).abs().max().item() < 1e-4
 
 
+@pytest.mark.parametrize("num_layers", [1, 2])
+@pytest.mark.parametrize("past_len", [0, 5, 40])
+def test_decode_layer_ref_equals_oracle_step(num_layers, past_len):
+    """kr.decode_layer (rounding off), layer after layer, then the final RMSNorm == one KV-cached step of oracle.lm.qwen2_forward: the
+    final-normed hidden state and every layer's new K / V row"""
+    g = torch.Generator().manual_seed(num_layers * 100 + past_len)
+    sd = {}
+    for name, shape in olm.param_shapes(num_layers, with_lm_head=False).items():
+        if name.startswith("llm.model.model.layers."):
+            fan_in = shape[-1] if len(shape) == 2 else 1
+            sd[name] = kr.bf16(torch.randn(*shape, generator=g) * (fan_in ** -0.5 if len(shape) == 2 else 0.1))
+            if name.endswith("layernorm.weight"):
+                sd[name] = 1.0 + 0.1 * torch.randn(*shape, generator=g)
+    sd["llm.model.model.norm.weight"] = 1.0 + 0.1 * torch.randn(olm.D, generator=g)
+    x = torch.randn(1, 1, olm.D, generator=g)
+    past = [(torch.randn(1, olm.N_KV, past_len, 64, generator=g), torch.randn(1, olm.N_KV, past_len, 64, generator=g))
+            for _ in range(num_layers)]
+    hid, new_past = olm.qwen2_forward(sd, x, past if past_len else None, num_layers=num_layers)
+    h = x[0].double()
+    for i in range(num_layers):
+        kc = torch.zeros(1, olm.N_KV, 64, 64, dtype=torch.float64)
+        vc = torch.zeros_like(kc)
+        kc[0, :, :past_len], vc[0, :, :past_len] = past[i][0][0].double(), past[i][1][0].double()
+        st = kr.decode_layer(kr.layer_weights(sd, i), h, kc, vc, [past_len])
+        # the oracle runs in fp32: ~1e-6 relative on O(1) values
+        assert (new_past[i][0][0, :, past_len].double() - st["k"][0]).abs().max().item() < 1e-4, i
+        assert (new_past[i][1][0, :, past_len].double() - st["v"][0]).abs().max().item() < 1e-4, i
+        h = st["x_out"]
+    want = kr.rms_norm(h, sd["llm.model.model.norm.weight"])
+    assert (hid[0].double() - want).abs().max().item() < 1e-4
+
+
+def test_decode_layer_rounding_points():
+    """rounding "fused" / "per-op" rounds exactly the stored stages: every one of them is bf16-representable, the exact reference's
+    fp32-kept stages are not (the per-op qkv and g / u), and without rounding nothing is"""
+    g = torch.Generator().manual_seed(11)
+    sd = {}
+    for name, shape in olm.param_shapes(1, with_lm_head=False).items():
+        if name.startswith("llm.model.model.layers."):
+            sd[name] = kr.bf16(torch.randn(*shape, generator=g) * (shape[-1] ** -0.5 if len(shape) == 2 else 0.1))
+    w = kr.layer_weights(sd, 0)
+    x = torch.randn(3, olm.D, generator=g, dtype=torch.float64)
+    kc = kr.bf16(torch.randn(3, olm.N_KV, 32, 64, generator=g, dtype=torch.float64))
+    vc = kr.bf16(torch.randn(3, olm.N_KV, 32, 64, generator=g, dtype=torch.float64))
+    is_b = lambda t: torch.equal(t, kr.bf16(t))
+    for rounding, stored in [("fused", ("xn", "q", "k", "v", "att", "xn_mid", "ffa")),
+                             ("per-op", ("xn", "qkv", "q", "k", "v", "att", "xn_mid", "g", "u", "ffa"))]:
+        st = kr.decode_layer(w, x, kc, vc, [0, 7, 31], rounding)
+        assert all(is_b(st[n]) for n in stored), rounding
+        assert not any(is_b(st[n]) for n in set(("qkv", "g", "u", "x_mid", "x_out")) - set(stored)), rounding
+    st = kr.decode_layer(w, x, kc, vc, [0, 7, 31])
+    assert not any(is_b(st[n]) for n in ("xn", "qkv", "q", "k", "v", "att", "xn_mid", "g", "u", "ffa", "x_out"))
+
+
 def test_rope_phase_table_matches_libm():
     """The LM kernels rotate by cosf / sinf of fp32(pos * inv_freq[i]) with inv_freq = 1 / powf(1e6, 2i / 64) (llm.cu
     lm_rope_inv_freq); oracle.lm.rope builds the same fp32 table, so the decode-attention bound of test_kernel_edges_gpu.py needs
