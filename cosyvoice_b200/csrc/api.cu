@@ -144,6 +144,7 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   std::string k(key ? key : "");
   if (k == "use_tc") ctx->use_tc = value;
   else if (k == "flow_fused_ff") ctx->flow_fused_ff = value;
+  else if (k == "flow_qkv_panel") ctx->flow_qkv_panel = value;
   else if (k == "tc_epi") ctx->tc_epi = value;
   else if (k == "tc_persist") ctx->tc_persist = value;
   else if (k == "op_out_bf16") ctx->op_out_bf16 = value;

@@ -204,6 +204,9 @@ struct cvk_ctx {
   int use_graph = 1;                        // LM decode step replayed as a CUDA graph
   int use_tc = 1;                           // bf16 mode: route GEMMs to the wgmma kernel (0 = debug: SIMT on converted operands)
   int flow_fused_ff = 1;                    // bf16 mode: LN3 + ff1 + ff2 (+ next LN1) of a flow-estimator block in one launch (ffn_fused)
+  int flow_qkv_panel = 1;                   // wgmma GEMM with one tap, K = 256, N >= 512 in 128-column chunks, 16-bit output (the estimator's qkv
+                                            // projection): row-panel kernel (qkv_panel_kernel) from 25 panels of 128 rows up; 2 = at any row
+                                            // count, 0 = conv_gemm_wg_kernel
 
   void* dmalloc(size_t bytes) {
     void* p = nullptr;

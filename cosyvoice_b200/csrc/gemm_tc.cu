@@ -475,6 +475,215 @@ void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUten
   conv_gemm_wg_kernel<BN, NSTG><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode, ntn, ntiles);
 }
 
+// ------------------------------------------------------------------------------------------------ row-panel GEMM, K = 256
+// out[r, n] = epilogue(sum_k A[r + shift0, k] W[n][k]) for one tap, K = 256 and a wide N (the qkv projection of the flow estimator's
+// transformer blocks: 256 -> 1536 on ~40 k rows; option "flow_qkv_panel").  At K = 256 a 128 x 128 tile of conv_gemm_wg_kernel has
+// only four ring stages of work, refills 128 KB of operands for it, and nothing runs on the tensor cores under its epilogue.  Here a
+// CTA keeps the 128 x 256 activation panel resident (64 KB, four SWIZZLE_128B sub-tiles [128 rows][64 channels], loaded once per
+// work unit) and walks 128-column chunks of W ([128][256], 64 KB, all of K) that the producer thread streams through a two-stage ring.
+// The two consumer warpgroups own 64 rows each and never wait for one another: each has two accumulator sets (setmaxnreg gives the
+// consumers 232 registers), commits the 16 wgmma of chunk c + 1 into one set and runs the epilogue of chunk c from the other while
+// they execute, stages its 64 x 128 tile in its own half of the staging region and issues its own TMA store, ordered by a
+// 128-thread named barrier of its own.
+// Shared memory: A 64 KB + 2 x 64 KB of W + 32 KB of staging = 224 KB (+ 1 KB alignment).  128-column chunks keep the generic
+// kernel's m64n128k16 instruction and leave room for exactly two W stages; that suffices because a stage is released as soon as the
+// chunk's MMAs complete, before its epilogue, so the refill has the whole epilogue to land.  64-column chunks would allow deeper
+// rings but halve the work per wgmma and double the barrier traffic.  Staging 64 x 128 of a 16-bit type per warpgroup: 16-bit outputs only.
+// A work unit is (panel, column group): group fastest, so the CTAs running together read the same W chunks from L2, and the CTA
+// walks units blockIdx.x, blockIdx.x + gridDim.x, ...  The next unit's first W chunk is requested before its A panel; the panel load
+// itself waits for the unit's last MMAs and lands under the last epilogue.
+// Per output the MMAs are those of conv_gemm_wg_kernel (K sub-tiles ascending, four k16 steps each, one fp32 accumulator from zero)
+// and the epilogue is its epi_math16p / stage_store16, so the results agree bit for bit.
+constexpr int QP_K = 256, QP_BN = 128, QP_NSTG = 2;
+constexpr uint32_t QP_A_BYTES = TC_BM * QP_K * 2;
+constexpr uint32_t QP_W_BYTES = QP_BN * QP_K * 2;
+constexpr uint32_t QP_STG_BYTES = TC_BM * QP_BN * 2;
+constexpr size_t QP_SMEM = QP_A_BYTES + QP_NSTG * QP_W_BYTES + QP_STG_BYTES + 1024;
+// fewest panels the dispatch sends here: 3200 rows x 256 -> 1536, the smallest size timed, took 15.5 us against 21.5 us on the generic
+// kernel (H100 80GB HBM3, 700 W); smaller launches, the streaming sessions' 50-frame chunks among them, have not been timed and stay there
+constexpr int QP_MIN_PANELS = 25;
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ CUtensorMap tmap_o, int shift0, int rowsOut, EpiDev ep, int ngroups, int cpu, int nunits) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t bar_full[QP_NSTG];
+  __shared__ __align__(8) uint64_t bar_empty[QP_NSTG];
+  __shared__ __align__(8) uint64_t bar_a_full, bar_a_empty;
+  __shared__ __align__(16) float s_bias_all[2 * QP_BN];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t w_base = smem_base + QP_A_BYTES;
+  const uint32_t stg_base = w_base + QP_NSTG * QP_W_BYTES;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < QP_NSTG; ++s) {
+      mbar_init(smem_u32(&bar_full[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);     // one arrival per consumer warp
+    }
+    mbar_init(smem_u32(&bar_a_full), 1);
+    mbar_init(smem_u32(&bar_a_empty), 8);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      uint32_t it = 0, ui = 0;
+      for (int u = blockIdx.x; u < nunits; u += gridDim.x, ++ui) {
+        const int r0 = (u / ngroups) * TC_BM, c0 = (u % ngroups) * cpu;
+        for (int c = 0; c < cpu; ++c, ++it) {
+          const uint32_t s = it % QP_NSTG, round = it / QP_NSTG;
+          mbar_wait(smem_u32(&bar_empty[s]), (round & 1u) ^ 1u);
+          const uint32_t sw = w_base + s * QP_W_BYTES;
+          const uint32_t fb = smem_u32(&bar_full[s]);
+          mbar_expect_tx(fb, QP_W_BYTES);
+#pragma unroll
+          for (int kt = 0; kt < QP_K / TC_BK; ++kt) tma_load_3d(sw + kt * (QP_BN * 128u), &tmap_w, fb, kt * TC_BK, 0, (c0 + c) * QP_BN);
+          if (c == 0) {     // the panel, once the previous unit's MMAs have read theirs
+            mbar_wait(smem_u32(&bar_a_empty), (ui & 1u) ^ 1u);
+            const uint32_t fa = smem_u32(&bar_a_full);
+            mbar_expect_tx(fa, QP_A_BYTES);
+#pragma unroll
+            for (int kt = 0; kt < QP_K / TC_BK; ++kt) tma_load_2d(smem_base + kt * (TC_BM * 128u), &tmap_a, fa, kt * TC_BK, r0 + shift0);
+          }
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int ct = threadIdx.x - 128;                   // consumer thread 0..255
+  const int wg = ct >> 7;                             // rows [64 wg, 64 wg + 64) of the panel
+  const int wt = ct & 127;                            // thread of the warpgroup
+  const int q = lane & 3;
+  const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);   // the panel row this thread's epilogue owns
+  const int cq = 16 * (q >> 1);                       // ... and its 16 columns of every 32
+  const uint32_t a_wg = smem_base + (uint32_t)wg * (64 * 128u);
+  float* s_bias = s_bias_all + wg * QP_BN;
+  EpiDev e = ep;
+  e.out2 = nullptr;                                   // no second output on this path: its epilogue code folds away
+
+  int r0 = 0, r = 0, seq = 0;
+  bool rin = false, valid = false;
+  // the 16 MMAs of one chunk: K sub-tiles ascending, four k16 steps each, into a zeroed accumulator
+  auto issue = [&](float* acc, uint32_t it) {
+    const uint32_t s = it % QP_NSTG;
+    mbar_wait(smem_u32(&bar_full[s]), (it / QP_NSTG) & 1u);
+    const uint32_t sw = w_base + s * QP_W_BYTES;
+#pragma unroll
+    for (int i = 0; i < QP_BN / 2; ++i) acc[i] = 0.f;
+    wg_fence();
+#pragma unroll
+    for (int kt = 0; kt < QP_K / TC_BK; ++kt) {
+      const uint64_t da = wg_desc_sw128(a_wg + kt * (TC_BM * 128u)), db = wg_desc_sw128(sw + kt * (QP_BN * 128u));
+      if (e.ab_f16) {
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) wgmma_ss<QP_BN, 1>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      } else {
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) wgmma_ss<QP_BN, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      }
+    }
+    wg_commit();
+  };
+  // chunk `it` has completed: free its W stage (and the panel after a unit's last chunk)
+  auto release = [&](uint32_t it, bool last) {
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(smem_u32(&bar_empty[it % QP_NSTG]));
+      if (last) mbar_arrive(smem_u32(&bar_a_empty));
+    }
+  };
+  // this warpgroup's 64 x 128 tile of columns [n0, n0 + 128): epilogue math, staging, one TMA store per 64 columns
+  auto epilogue = [&](float* acc, int n0, float bv) {
+    if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous store has read the staging tile
+    s_bias[wt] = bv;
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+#pragma unroll
+    for (int cb = 0; cb < QP_BN; cb += 32) {
+      float a16[16], v[16], w2[16];
+      wg_frag_rows16(acc + cb / 2, lane, a16);
+      const int c = cb + cq;
+      epi_math16p(e, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
+      stage_store16(stg_base, e.out_dtype, row, c, v);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if (wt == 0) {
+#pragma unroll
+      for (int sb = 0; sb < QP_BN / 64; ++sb)
+        tma_store_2d(&tmap_o, stg_base + sb * 16384u + (uint32_t)wg * 8192u, n0 + sb * 64, r0 + wg * 64);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+  };
+
+  float acc0[QP_BN / 2], acc1[QP_BN / 2];
+  uint32_t it = 0, ui = 0;
+  for (int u = blockIdx.x; u < nunits; u += gridDim.x, ++ui) {
+    r0 = (u / ngroups) * TC_BM;
+    const int nb = (u % ngroups) * cpu * QP_BN;
+    r = r0 + row;
+    rin = r < rowsOut;
+    seq = 0;
+    if (rin && e.row2seq) seq = e.row2seq[r];
+    valid = rin && (!e.row2seq || seq >= 0);
+    mbar_wait(smem_u32(&bar_a_full), ui & 1u);
+    issue(acc0, it);
+    for (int c = 0; c < cpu; c += 2) {
+      // chunk c is in flight in acc0
+      float bv = e.bias ? e.bias[nb + c * QP_BN + wt] : 0.f;
+      if (c + 1 < cpu) {
+        issue(acc1, it + 1);
+        wg_wait<1>();
+      } else {
+        wg_wait<0>();
+      }
+      wg_touch<QP_BN / 2>(acc0);
+      release(it, c + 1 == cpu);
+      epilogue(acc0, nb + c * QP_BN, bv);
+      ++it;
+      if (c + 1 == cpu) break;
+      // chunk c + 1 is in flight in acc1
+      bv = e.bias ? e.bias[nb + (c + 1) * QP_BN + wt] : 0.f;
+      if (c + 2 < cpu) {
+        issue(acc0, it + 1);
+        wg_wait<1>();
+      } else {
+        wg_wait<0>();
+      }
+      wg_touch<QP_BN / 2>(acc1);
+      release(it, c + 2 == cpu);
+      epilogue(acc1, nb + (c + 1) * QP_BN, bv);
+      ++it;
+    }
+  }
+  if (wt == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+void launch_panel(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const ConvW& W, int rowsOut,
+                  const EpiDev& e) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(qkv_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QP_SMEM));
+    attr_set = true;
+  }
+  // Column groups per panel: whole panels leave the last wave of CTAs partly idle (313 panels on 132 SMs: 3 waves of 12 chunks
+  // where 2.4 are needed), more groups reload the panel more often.  Take the split with the fewest chunk times on the busiest SM,
+  // a unit's panel load and its unpipelined first chunk counted as one more.
+  const int panels = ceil_div(rowsOut, TC_BM), nch = W.N / QP_BN;
+  int ngroups = 1;
+  long best = -1;
+  for (int g = 1; g <= 4; ++g) {
+    if (nch % g) continue;
+    const long cost = (long)ceil_div(panels * g, ctx->num_sms) * (nch / g + 1);
+    if (best < 0 || cost < best) { best = cost; ngroups = g; }
+  }
+  const int nunits = panels * ngroups;
+  qkv_panel_kernel<<<std::min(nunits, ctx->num_sms), TC_THREADS, QP_SMEM, st>>>(ta, tw, to, W.shift0, rowsOut, e, ngroups, nch / ngroups, nunits);
+}
+
 // ------------------------------------------------------------------------------------------------ fused feed-forward
 // The feed-forward half of a flow-estimator transformer block in one launch (matcha transformer.py: x = x + ff(norm3(x))):
 //   x <- valid(r) ? x + b2 + GELU(LN3(x) W1^T + b1) W2^T : 0,   C = 256 channels, 1024 hidden,
@@ -711,11 +920,15 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
     const bool whole16 = (W.N * ep.out.esize()) % 16 == 0 && (!ep.out2.p || (W.N * ep.out2.esize()) % 16 == 0);
     if (ep.accumulate || need > TC_STG_BYTES || !whole16) epi_mode = 0;
   }
+  // the row-panel kernel: one tap, K = 256, wide N in whole 128-column chunks, one 16-bit output through the staged stores, and at
+  // least QP_MIN_PANELS 128-row panels (option 2: any row count)
+  const bool panel = ctx->flow_qkv_panel && epi_mode == 2 && W.taps == 1 && W.K == QP_K && W.N % QP_BN == 0 && W.N >= 512 && !ep.out2.p &&
+                     ep.out.esize() == 2 && (ctx->flow_qkv_panel == 2 || ceil_div(rowsOut, TC_BM) >= QP_MIN_PANELS);
   if (epi_mode == 2) {
     auto mk = [&](CUtensorMap* m, const Mat& o) {
       cuuint64_t dims[2] = {(cuuint64_t)W.N, (cuuint64_t)rowsOut};
       cuuint64_t strides[1] = {(cuuint64_t)o.ld * o.esize()};
-      cuuint32_t box[2] = {(cuuint32_t)(o.dtype == DT_F32 ? 32 : 64), TC_BM};
+      cuuint32_t box[2] = {(cuuint32_t)(o.dtype == DT_F32 ? 32 : 64), (cuuint32_t)(panel ? TC_BM / 2 : TC_BM)};   // panel: a store per warpgroup
       cuuint32_t es[2] = {1, 1};
       CUresult r = enc(m, o.dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, o.p, dims, strides, box, es,
                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -724,7 +937,8 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
     mk(&to, ep.out);
     if (ep.out2.p) mk(&to2, ep.out2);
   }
-  if (BN == 128) launch_wg<128, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+  if (panel) launch_panel(ctx, st, ta, tw, to, W, rowsOut, e);
+  else if (BN == 128) launch_wg<128, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
   else launch_wg<64, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
   ctx->launches++;
   CVK_LAUNCH_CHECK();

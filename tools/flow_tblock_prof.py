@@ -2,7 +2,7 @@
 
 Writes <out>/flow_kernels_<opt><value>.md: per kernel name the time and launch count of one flow_batch, then the
 time of the estimator's transformer-block launches by role.  Roles come from the launch order inside a block: the attention kernel
-is preceded by the qkv GEMM (and, for the first block of a stage, LN1) and followed by the out GEMM, then either LN3, the ff1 and the
+is preceded by the qkv GEMM (the generic kernel or the row-panel one; and, for the first block of a stage, LN1) and followed by the out GEMM, then either LN3, the ff1 and the
 ff2 GEMMs (and the next block's LN1), or the fused feed-forward kernel.  Not a bench: the profiler slows the host.
 
   python tools/flow_tblock_prof.py --opt flow_fused_ff --values 0,1 --out /tmp/flow_prof
@@ -57,7 +57,7 @@ def roles(kern):
     for i, n in enumerate(names):
         if "attn_wg_kernel" not in n or i < 1 or i + 2 >= len(names):
             continue
-        if "conv_gemm_wg_kernel" not in names[i - 1] or "conv_gemm_wg_kernel" not in names[i + 1]:
+        if not ("conv_gemm_wg_kernel" in names[i - 1] or "qkv_panel_kernel" in names[i - 1]) or "conv_gemm_wg_kernel" not in names[i + 1]:
             continue
         if not (is_ln(names[i + 2]) or "ffn_fused_kernel" in names[i + 2]):
             continue      # the conformer encoder's layers continue otherwise
