@@ -74,6 +74,20 @@ void prompt_feat_init(cvk_ctx* ctx);
     return CVK_ERR_INVALID;                          \
   }
 
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+void encode_tma_map(cvk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                    const cuuint32_t* box, int dtype, CUtensorMapL2promotion l2, const char* what) {
+  CVK_REQUIRE(rank == 2 || rank == 3, std::string("tensor map ") + what + ": rank 2 or 3");
+  const cuuint32_t es[3] = {1, 1, 1};
+  CUresult r = ((EncodeTiledFn)ctx->encode_tiled)(map, dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
+                                                  const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                                  CU_TENSOR_MAP_SWIZZLE_128B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CVK_REQUIRE(r == CUDA_SUCCESS, std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)r));
+}
+
 extern "C" {
 
 const char* cvk_version(void) { return "libcvk 0.1 (sm_90a)"; }
@@ -88,11 +102,24 @@ int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out)
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return CVK_ERR_CUDA;
   if (prop.major != 9) return CVK_ERR_CUDA;    // sm_90a only: the wgmma/TMA kernels have no other code path
+  void* encode = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &encode, cudaEnableDefault, &qres) != cudaSuccess ||
+      qres != cudaDriverEntryPointSuccess || !encode)
+    return CVK_ERR_CUDA;
+  try {
+    gemm_tc_setup();
+    attention_tc_setup();
+    skinny_setup();
+  } catch (const std::exception&) {
+    return CVK_ERR_CUDA;
+  }
   cvk_ctx* ctx = new cvk_ctx();
   ctx->device = device;
   ctx->precision = precision;
   ctx->act_dtype = precision == CVK_PREC_BF16 ? DT_BF16 : DT_F32;
   ctx->num_sms = prop.multiProcessorCount;
+  ctx->encode_tiled = encode;
   if (workspace_bytes == 0) workspace_bytes = (size_t)4 << 30;
   void* p = nullptr;
   if (cudaMalloc(&p, workspace_bytes) != cudaSuccess) {

@@ -3,6 +3,7 @@
 // relative-position attention of the encoder.
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "tma.cuh"
 
 namespace {
 
@@ -16,44 +17,6 @@ constexpr uint32_t V_BYTES = AT_BK * AT_HD * 2;        // 8 KB
 constexpr uint32_t KV_STAGE = K_BYTES + V_BYTES;       // 16 KB
 
 constexpr uint32_t AT_SMEM = Q_BYTES + AT_KVST * KV_STAGE + 1024;   // 65 KB
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// true once the phase of the given parity has completed (one bounded try, no spinning)
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_test(bar, parity)) return;            // fast path without clock reads
-  const long long t0 = clock64();
-  for (;;) {
-    if (mbar_test(bar, parity)) return;
-    if (clock64() - t0 > 4000000000ll) break;
-  }
-  __trap();
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
 
 // One CTA = 128 queries of one (sequence, head), 256 threads: warpgroups 0 and 1 own 64 queries each, and thread 0 also issues
 // the TMA loads (Q once, then K/V 64-key tiles through a three-stage ring).  Without a producer warp the plain kernel fits in 128
@@ -338,30 +301,26 @@ relpos_u_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
   }
 }
 
-
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
+// bf16 operand [rows, cols]: 64-column boxes of box_rows rows
 void make_map(cvk_ctx* ctx, CUtensorMap* m, const Mat& x, int box_rows) {
-  if (!ctx->encode_tiled) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    CVK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    CVK_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
-    ctx->encode_tiled = fn;
-  }
-  cuuint64_t dims[2] = {(cuuint64_t)x.cols, (cuuint64_t)x.rows};
-  cuuint64_t strides[1] = {(cuuint64_t)x.ld * 2};
-  cuuint32_t box[2] = {AT_HD, (cuuint32_t)box_rows};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = ((EncodeTiledFn)ctx->encode_tiled)(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(attention) failed: " + std::to_string((int)r));
+  const cuuint64_t dims[2] = {(cuuint64_t)x.cols, (cuuint64_t)x.rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)x.ld * 2};
+  const cuuint32_t box[2] = {AT_HD, (cuuint32_t)box_rows};
+  encode_tma_map(ctx, m, x.p, 2, dims, strides, box, DT_BF16, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "attention");
 }
 
 }  // namespace
+
+void attention_tc_setup() {
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(relpos_u_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
+  // the kernel relies on two co-resident CTAs per SM to hide its serial MMA -> softmax -> MMA chain: a register or shared
+  // memory increase that loses the second CTA is an error, not a silent slowdown
+  int per_sm = 0;
+  CVK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_wg_kernel<false>, AT_THREADS, AT_SMEM));
+  CVK_REQUIRE(per_sm >= 2, "attn_wg_kernel: " + std::to_string(per_sm) + " CTA(s) per SM, laid out for 2");
+}
 
 void attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& q, const Mat& k, const Mat& v, const Seqs& s, int H, int chunk,
                       float scale, const Mat& out, int kv_div, const KvGeom* kg) {
@@ -372,16 +331,6 @@ void attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& q, const Mat& k,
   make_map(ctx, &tq, q, AT_BQ);
   make_map(ctx, &tk, k, AT_BK);
   make_map(ctx, &tv, v, AT_BK);
-  static bool attr = false;
-  if (!attr) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    // the kernel relies on two co-resident CTAs per SM to hide its serial MMA -> softmax -> MMA chain: a register or shared
-    // memory increase that loses the second CTA is an error, not a silent slowdown
-    int per_sm = 0;
-    CVK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_wg_kernel<false>, AT_THREADS, AT_SMEM));
-    CVK_REQUIRE(per_sm >= 2, "attn_wg_kernel: " + std::to_string(per_sm) + " CTA(s) per SM, laid out for 2");
-    attr = true;
-  }
   dim3 grid(ceil_div(s.max_len, AT_BQ), H, s.B);
   attn_wg_kernel<false><<<grid, AT_THREADS, AT_SMEM, st>>>(tq, tk, tv, s.d_start, s.d_len, chunk, scale * 1.4426950408889634f, kv_div, out.b16(), out.ld,
                                                            kg ? kg->d_kstart : nullptr, kg ? kg->d_klen : nullptr, kg ? kg->d_qoff : nullptr,
@@ -405,12 +354,6 @@ void relpos_attention_fwd_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& qu, const
   make_map(ctx, &tk, k, AT_BK);
   make_map(ctx, &tv, v, AT_BK);
   make_map(ctx, &tp, pos, AT_BK);
-  static bool attr = false;
-  if (!attr) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(relpos_u_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AT_SMEM));
-    attr = true;
-  }
   dim3 grid(ceil_div(s.max_len, AT_BQ), H, s.B);
   relpos_u_kernel<<<grid, RP_THREADS, AT_SMEM, st>>>(tqv, tp, s.d_start, s.d_len, pos_center, pos_rows, U.f32(), U.ld);
   ctx->launches++;

@@ -172,7 +172,7 @@ struct cvk_ctx {
   LlmModel* llm = nullptr;
   void* mel_model = nullptr;
   void* prompt_feat_model = nullptr;      // prompt_feat.cu (whisper log-mel / kaldi fbank constants), built on first use
-  void* encode_tiled = nullptr;             // cuTensorMapEncodeTiled entry point
+  void* encode_tiled = nullptr;             // cuTensorMapEncodeTiled entry point (fetched by cvk_create)
   std::atomic<int64_t> launches{0};         // kernels launched by this library (bench.py gpu_launches); LM-session calls and workspace calls may run on two threads
   int op_out_bf16 = 0;                      // cvk_op_conv1d: bf16 output matrix (the estimator's usual epilogue) instead of fp32
   int op_iters = 0;                         // cvk_op_conv1d: repeat the GEMM launch this many times and time it
@@ -240,6 +240,19 @@ inline void launch_ex(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem
   CVK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...));
 }
 
+// ------------------------------------------------------------------------------------------------ Hopper kernel set-up (api.cu)
+// Tiled TMA map over a row-major tensor of rank 2 or 3 at `base`: dims and box innermost first, byte strides of dims 1 .. rank - 1,
+// SWIZZLE_128B boxes; elements outside the tensor load as zero and are not stored.  dtype DT_F32 is encoded as FLOAT32, the 16-bit
+// types (bf16 and IEEE half alike: TMA moves their bytes unchanged) as BFLOAT16.  Throws CvkError naming `what` if the driver
+// rejects the map.
+void encode_tma_map(cvk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                    const cuuint32_t* box, int dtype, CUtensorMapL2promotion l2, const char* what);
+// Kernel attributes of the current device (maximum dynamic shared memory, carveouts) and the checks that depend on them; cvk_create
+// runs them once per context.  Throw CvkError on failure.
+void gemm_tc_setup();
+void attention_tc_setup();
+void skinny_setup();
+
 // ------------------------------------------------------------------------------------------------ shared ops
 // geometry
 Seqs make_seqs(cvk_ctx* ctx, const int* lens, int B, int gap, int scale, int extra_front, cudaStream_t st, bool with_row2seq = true);
@@ -269,7 +282,6 @@ void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, co
              const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn, const Mat& hid);
 size_t skinny_scratch_floats(int rows, int maxN);
 const bf16* skinny_tiled_weights(cvk_ctx* ctx, const ConvW& W);
-void skinny_set_carveout();
 int conv_gemm_skinny_ex(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep, float* scratch, size_t scratch_floats,
                         int mode);
 void conv_gemm_skinny(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep, float* scratch, size_t scratch_floats);

@@ -10,6 +10,7 @@
 // (cosyvoice/llm/llm.py:244-251, 542).
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "tma.cuh"
 
 namespace {
 
@@ -18,51 +19,6 @@ constexpr int SK_BK = 64;
 constexpr int SK_STAGES = 8;
 constexpr int SK_THREADS = 384;   // warp 0: TMA producer; warpgroups 1-2: wgmma + epilogue, 64 features each
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  if (ok) return;                       // fast path: no clock reads on the MMA issuer's instruction stream
-  const long long t0 = clock64();
-  for (;;) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 4000000000ll) break;
-  }
-  __trap();
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// plain (non-tensor) bulk copy global -> shared, completion counted on an mbarrier
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
 // W [N][K] bf16 row-major -> streaming layout: [N/128 tiles][K/64 chunks] blocks of 16 KB, each block being the exact
 // shared-memory image of a K-major SWIZZLE_128B operand tile (row r, 16-byte chunk c stored at r*128 + ((c ^ (r & 7)) << 4)),
 // so that one stage is ONE contiguous 16 KB bulk copy: DRAM sees perfectly sequential reads instead of 128 strided rows.
@@ -208,20 +164,15 @@ __global__ void splitk_finish_kernel(const float* __restrict__ partial, int spli
   tl_stamp(tl, 2);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+template <int BPAD>
+constexpr size_t skinny_smem() {
+  return (size_t)SK_STAGES * (SK_BM * SK_BK * 2 + BPAD * SK_BK * 2) + 1024;
+}
 
 template <int BPAD>
 void launch(cudaStream_t st, dim3 grid, const bf16* tw, const CUtensorMap& tx, const ConvW& W, int rows, int cps, float* partial,
             const EpiDev& e, int swiglu, bool pdl, long long* tl) {
-  constexpr size_t smem = (size_t)SK_STAGES * (SK_BM * SK_BK * 2 + BPAD * SK_BK * 2) + 1024;
-  static bool attr = false;
-  if (!attr) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<BPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
-  launch_ex(skinny_gemm_kernel<BPAD>, grid, dim3(SK_THREADS), smem, st, pdl, tw, tx, W.N, W.K, rows, cps, partial, e, swiglu, tl);
+  launch_ex(skinny_gemm_kernel<BPAD>, grid, dim3(SK_THREADS), skinny_smem<BPAD>(), st, pdl, tw, tx, W.N, W.K, rows, cps, partial, e, swiglu, tl);
 }
 
 }  // namespace
@@ -252,25 +203,14 @@ int conv_gemm_skinny_ex(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW
   const int rows = mode == 1 ? A.rows : ep.out.rows;
   CVK_REQUIRE(rows <= 64 && A.rows >= rows, "conv_gemm_skinny: at most 64 rows");
   CVK_REQUIRE(W.K % 8 == 0 && A.ld % 8 == 0 && ((uintptr_t)A.p & 15) == 0, "conv_gemm_skinny: 16-byte aligned operands required");
-  if (!ctx->encode_tiled) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    CVK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    CVK_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
-    ctx->encode_tiled = fn;
-  }
-  EncodeTiledFn enc = (EncodeTiledFn)ctx->encode_tiled;
   const int BPAD = rows <= 32 ? 32 : 64;
   CUtensorMap tx;
   const bf16* tw = skinny_tiled_weights(ctx, W);
   {
-    cuuint64_t dims[2] = {(cuuint64_t)W.K, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)A.ld * 2};
-    cuuint32_t box[2] = {SK_BK, (cuuint32_t)BPAD};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(&tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, A.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(skinny x) failed: " + std::to_string((int)r));
+    const cuuint64_t dims[2] = {(cuuint64_t)W.K, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)A.ld * 2};
+    const cuuint32_t box[2] = {SK_BK, (cuuint32_t)BPAD};
+    encode_tma_map(ctx, &tx, A.p, 2, dims, strides, box, DT_BF16, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "skinny x");
   }
   const int tiles = ceil_div(W.N, SK_BM);
   const int kchunks = ceil_div(W.K, SK_BK);
@@ -312,7 +252,11 @@ void conv_gemm_skinny(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& 
   conv_gemm_skinny_ex(ctx, st, A, W, ep, scratch, scratch_floats, 0);
 }
 
-void skinny_set_carveout() {
+// dynamic shared memory of both batch widths, and the maximum shared-memory carveout that every kernel of the LM decode chain
+// keeps (see llm_session_create)
+void skinny_setup() {
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skinny_smem<32>()));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skinny_smem<64>()));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(skinny_gemm_kernel<64>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(splitk_finish_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));

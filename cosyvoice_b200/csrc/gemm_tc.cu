@@ -10,61 +10,13 @@
 // upsampling convolutions (hifigan/generator.py:110-117, 432-443).
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "tma.cuh"
 
 namespace {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;   // 64 bf16 = 128 B = one SWIZZLE_128B atom row
 constexpr int TC_THREADS = 384;   // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue, 64 rows each
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// bounded spin: a broken pipeline traps (-> CUDA error in the host API) instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  if (ok) return;            // fast path without clock reads: the wait sits on the single MMA-issuing thread's instruction stream
-  const long long t0 = clock64();
-  for (;;) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 4000000000ll) break;   // ~2 s at 2 GHz
-  }
-  __trap();
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 
 // 16 consecutive columns of one row through the fused epilogue (vector fast path + scalar tail).
 __device__ __forceinline__ void epi_store16(const EpiDev& e, int r, int n0, int N, const float* acc) {
@@ -304,9 +256,6 @@ __device__ __forceinline__ void stage_store16(uint32_t stg, int dtype, int row, 
     }
   }
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
 
 // One CTA computes 128 x BN output tiles: warp 0 (lane 0) is the TMA producer, warpgroups 1 and 2 each issue wgmma for 64 of the
 // 128 rows and run the fused epilogue on their own accumulators.  With more tiles than CTAs (persistent launch, one CTA per SM)
@@ -445,30 +394,15 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   if (ct == 0 && epi_mode == 2) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode(cvk_ctx* ctx) {
-  if (!ctx->encode_tiled) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    CVK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    CVK_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
-    ctx->encode_tiled = fn;
-  }
-  return (EncodeTiledFn)ctx->encode_tiled;
+template <int BN, int NSTG>
+constexpr size_t wg_smem() {
+  return (size_t)NSTG * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + TC_STG_BYTES + 1024;
 }
 
 template <int BN, int NSTG>
 void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const CUtensorMap& to2,
                const ConvW& W, int rowsOut, const EpiDev& e, int epi_mode) {
-  constexpr size_t smem = (size_t)NSTG * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + TC_STG_BYTES + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<BN, NSTG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  constexpr size_t smem = wg_smem<BN, NSTG>();
   const int ntn = ceil_div(W.N, BN), ntiles = ntn * ceil_div(rowsOut, TC_BM);
   // more tiles than SMs: persistent CTAs (one per SM) unless switched off
   const int grid = (ctx->tc_persist && ntiles > ctx->num_sms) ? ctx->num_sms : ntiles;
@@ -664,11 +598,6 @@ qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
 void launch_panel(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const ConvW& W, int rowsOut,
                   const EpiDev& e) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(qkv_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QP_SMEM));
-    attr_set = true;
-  }
   // Column groups per panel: whole panels leave the last wave of CTAs partly idle (313 panels on 132 SMs: 3 waves of 12 chunks
   // where 2.4 are needed), more groups reload the panel more often.  Take the split with the fewest chunk times on the busiest SM,
   // a unit's panel load and its unpipelined first chunk counted as one more.
@@ -876,26 +805,19 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   CVK_REQUIRE(A.cols >= W.K, "conv_gemm_tc: A has fewer columns than K");
   CVK_REQUIRE(W.K % 8 == 0 && A.ld % 8 == 0 && ((uintptr_t)A.p & 15) == 0, "conv_gemm_tc: operands must be 16-byte aligned");
   CVK_REQUIRE(ep.out.p != nullptr && ep.out.cols >= W.N, "conv_gemm_tc: bad output");
-  EncodeTiledFn enc = get_encode(ctx);
   const int BN = W.N > 64 ? 128 : 64;
   CUtensorMap ta, tw;
   {
-    cuuint64_t dims[2] = {(cuuint64_t)W.K, (cuuint64_t)A.rows};
-    cuuint64_t strides[1] = {(cuuint64_t)A.ld * 2};
-    cuuint32_t box[2] = {TC_BK, TC_BM};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, A.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(A) failed: " + std::to_string((int)r));
+    const cuuint64_t dims[2] = {(cuuint64_t)W.K, (cuuint64_t)A.rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)A.ld * 2};
+    const cuuint32_t box[2] = {TC_BK, TC_BM};
+    encode_tma_map(ctx, &ta, A.p, 2, dims, strides, box, A.dtype, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "A");
   }
   {
-    cuuint64_t dims[3] = {(cuuint64_t)W.K, (cuuint64_t)W.taps, (cuuint64_t)W.N};
-    cuuint64_t strides[2] = {(cuuint64_t)W.K * 2, (cuuint64_t)W.K * W.taps * 2};
-    cuuint32_t box[3] = {TC_BK, 1, (cuuint32_t)BN};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&tw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(w16p), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(W) failed: " + std::to_string((int)r));
+    const cuuint64_t dims[3] = {(cuuint64_t)W.K, (cuuint64_t)W.taps, (cuuint64_t)W.N};
+    const cuuint64_t strides[2] = {(cuuint64_t)W.K * 2, (cuuint64_t)W.K * W.taps * 2};
+    const cuuint32_t box[3] = {TC_BK, 1, (cuuint32_t)BN};
+    encode_tma_map(ctx, &tw, w16p, 3, dims, strides, box, A.dtype, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "W");
   }
   EpiDev e = to_dev(ep);
   e.ab_f16 = A.dtype == DT_F16;
@@ -926,13 +848,10 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
                      ep.out.esize() == 2 && (ctx->flow_qkv_panel == 2 || ceil_div(rowsOut, TC_BM) >= QP_MIN_PANELS);
   if (epi_mode == 2) {
     auto mk = [&](CUtensorMap* m, const Mat& o) {
-      cuuint64_t dims[2] = {(cuuint64_t)W.N, (cuuint64_t)rowsOut};
-      cuuint64_t strides[1] = {(cuuint64_t)o.ld * o.esize()};
-      cuuint32_t box[2] = {(cuuint32_t)(o.dtype == DT_F32 ? 32 : 64), (cuuint32_t)(panel ? TC_BM / 2 : TC_BM)};   // panel: a store per warpgroup
-      cuuint32_t es[2] = {1, 1};
-      CUresult r = enc(m, o.dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, o.p, dims, strides, box, es,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(out) failed: " + std::to_string((int)r));
+      const cuuint64_t dims[2] = {(cuuint64_t)W.N, (cuuint64_t)rowsOut};
+      const cuuint64_t strides[1] = {(cuuint64_t)o.ld * o.esize()};
+      const cuuint32_t box[2] = {(cuuint32_t)(o.dtype == DT_F32 ? 32 : 64), (cuuint32_t)(panel ? TC_BM / 2 : TC_BM)};   // panel: a store per warpgroup
+      encode_tma_map(ctx, m, o.p, 2, dims, strides, box, o.dtype, CU_TENSOR_MAP_L2_PROMOTION_NONE, "out");
     };
     mk(&to, ep.out);
     if (ep.out2.p) mk(&to2, ep.out2);
@@ -954,16 +873,12 @@ void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, 
               "ffn_fused: unexpected weights");
   CVK_REQUIRE((((uintptr_t)ln3_g | (uintptr_t)ln3_b | (uintptr_t)ln_g | (uintptr_t)ln_b | (uintptr_t)w1.bias | (uintptr_t)w2.bias) & 15) == 0,
               "ffn_fused: LayerNorm and bias vectors must be 16-byte aligned");
-  EncodeTiledFn enc = get_encode(ctx);
   CUtensorMap t1, t2;
   auto mk = [&](CUtensorMap* m, const bf16* w, int N, int K, int box_n) {
-    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
-    cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)box_n};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<bf16*>(w), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(ffn weights) failed: " + std::to_string((int)r));
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
+    const cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+    const cuuint32_t box[2] = {64, (cuuint32_t)box_n};
+    encode_tma_map(ctx, m, w, 2, dims, strides, box, DT_BF16, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "ffn weights");
   };
   mk(&t1, w1.w16, FF_HID, FF_C, FF_HC);
   mk(&t2, w2.w16, FF_C, FF_HID, FF_C);
@@ -974,12 +889,14 @@ void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, 
   const double flops = 4.0 * x.rows * (double)FF_C * FF_HID;
   const double bytes = (double)x.rows * FF_C * (4 + 4 + 2) + 2.0 * FF_C * FF_HID * 2;
   ProfScope ps(ctx, st, FAM_GEMM_TC, flops, bytes);
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVK_CHECK_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
-    attr_set = true;
-  }
   ffn_fused_kernel<<<ceil_div(x.rows, TC_BM), TC_THREADS, FF_SMEM, st>>>(t1, t2, p);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
+}
+
+void gemm_tc_setup() {
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<128, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<128, 4>()));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<64, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<64, 4>()));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(qkv_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QP_SMEM));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
 }

@@ -1233,11 +1233,11 @@ cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context)
   CVK_REQUIRE((NH / NKV) * max_context * sizeof(float) <= 200 * 1024, "session context too long for the decode attention kernel");
   decode_attn_allow_ctx(max_context);
   // keep every kernel of the decode step on the same (maximum) shared-memory carveout: alternating carveouts between
-  // consecutive kernels forces an SM reconfiguration (idle + several microseconds) at every boundary
+  // consecutive kernels forces an SM reconfiguration (idle + several microseconds) at every boundary (the skinny GEMM kernels'
+  // carveout is set by skinny_setup when the context is created)
   CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(finish_rms_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CVK_CHECK_CUDA(cudaFuncSetAttribute(ras_sampler_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  skinny_set_carveout();
   CVK_CHECK_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATTN_FUSED_SMEM));
   s->count = (int*)alloc(sizeof(int) * max_batch);
   s->done = (int*)alloc(sizeof(int) * max_batch);

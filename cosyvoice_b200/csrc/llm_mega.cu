@@ -22,6 +22,7 @@
 // down GEMM | +res, RMSNorm.
 #include "llm_decode_attn.cuh"
 #include "wgmma.cuh"
+#include "tma.cuh"
 #include <algorithm>
 #include <type_traits>
 
@@ -67,44 +68,6 @@ struct MegaParams {
   long long* tl;                       // optional phase timeline (CTA 0)
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  if (ok) return;                       // fast path: no clock reads on the MMA issuers' instruction stream
-  const long long t0 = clock64();
-  for (;;) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 4000000000ll) break;     // ~2 s: a protocol bug traps instead of hanging the GPU
-  }
-  __trap();
-}
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void worker_bar() { asm volatile("bar.sync 1, %0;" ::"n"(MG_WORKERS) : "memory"); }
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 2, 256;" ::: "memory"); }   // the two MMA warpgroups
 __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {

@@ -50,6 +50,8 @@ typedef enum {
 #define CVK_PREC_BF16 1 /* dense GEMM / conv operands bf16 on wgmma tensor cores, fp32 accumulate + residuals */
 
 /* ---------------------------------------------------------------------------------------------- context */
+/* Fails with CVK_ERR_CUDA when the device is not an sm_90 GPU, when the driver does not provide cuTensorMapEncodeTiled, or when the
+ * tensor-core kernels cannot be configured on the device, including when the flow attention kernel no longer fits two CTAs per SM. */
 int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out);
 void cvk_destroy(cvk_ctx* ctx);
 const char* cvk_last_error(cvk_ctx* ctx);
