@@ -111,6 +111,7 @@ int cvk_create(int device, int precision, size_t workspace_bytes, cvk_ctx** out)
     gemm_tc_setup();
     attention_tc_setup();
     skinny_setup();
+    hift3_setup();
   } catch (const std::exception&) {
     return CVK_ERR_CUDA;
   }

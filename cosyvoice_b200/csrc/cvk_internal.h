@@ -252,6 +252,7 @@ void encode_tma_map(cvk_ctx* ctx, CUtensorMap* map, const void* base, int rank, 
 void gemm_tc_setup();
 void attention_tc_setup();
 void skinny_setup();
+void hift3_setup();
 
 // ------------------------------------------------------------------------------------------------ shared ops
 // geometry

@@ -676,13 +676,13 @@ void hift_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, cons
 // The vocoder BODY is the CosyVoice2 one with different weights: every centred convolution becomes a left-padded one (a different
 // row shift of the same conv-GEMM), conv_pre looks 4 frames to the right, the transposed convolutions become nearest-neighbour
 // up-sampling + causal convolution (again a 3-tap polyphase conv-GEMM whose [R, u*C] output is the next level's [u*R, C]), and
-// the strided source_downs pad left only.  The f0 predictor runs in float64 on CUDA cores (a few GFLOP per utterance; the
-// reference insists on float64 so that streaming and offline f0 agree), the harmonic source uses nearest-neighbour phase
+// the strided source_downs pad left only.  The f0 predictor runs in float64 on the fp64 tensor cores (a few GFLOP per utterance;
+// the reference insists on float64 so that streaming and offline f0 agree), the harmonic source uses nearest-neighbour phase
 // up-sampling and the module's stored uniform noise instead of fresh Gaussian draws.
 namespace {
 
 struct F64Conv {
-  double* w = nullptr;      // [taps][K][N]  (n fastest: coalesced across the threads of a block)
+  double* w = nullptr;      // [taps][K][N]  (n fastest: 16-byte cp.async rows of the kernel's weight slabs)
   double* bias = nullptr;   // [N]
   int N = 0, K = 0, taps = 0, shift0 = 0;
 };
@@ -726,27 +726,132 @@ __global__ void f64_copy_kernel(const float* __restrict__ a, double* __restrict_
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) o[i] = (double)a[i];
 }
 
-// out[r, n] = ELU(bias[n] + sum_j sum_k A[r + shift0 + j, k] * w[j][k][n]) in float64; one block per row, rows outside every
-// sequence (row2seq < 0) stay zero so that they act as the zero padding of the next layer
-__global__ void conv_f64_kernel(const double* __restrict__ A, int K, const double* __restrict__ w, const double* __restrict__ bias, int N, int taps,
-                                int shift0, int rows, const int* __restrict__ row2seq, double* __restrict__ out) {
-  const int r = blockIdx.x;
-  const bool valid = row2seq[r] >= 0;
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    double acc = 0.0;
-    if (valid) {
-      acc = bias[n];
-      for (int j = 0; j < taps; ++j) {
-        const int rr = r + shift0 + j;
-        if (rr < 0 || rr >= rows) continue;
-        const double* a = A + (size_t)rr * K;
-        const double* wp = w + (size_t)j * K * N + n;
-        for (int k = 0; k < K; ++k) acc = fma(a[k], wp[(size_t)k * N], acc);
-      }
-      acc = acc > 0.0 ? acc : expm1(acc);
+// f0 predictor convolution on the fp64 tensor cores (mma.sync m16n8k8 f64, SASS DMMA.16x8x8):
+//   out[r, n] = ELU(bias[n] + sum_j sum_k A[r + shift0 + j, k] * w[j][k][n])
+// One CTA computes an F0_BM x F0_BN output tile.  Per F0_BK-wide K slab it stages the tile's A rows plus the taps-1 halo rows
+// once (tap j reads them at row offset j) and the taps' F0_BK x F0_BN weight slabs, in a cp.async ring of F0Stages slabs, so
+// the weights are read once per row tile.  Every output sums its products in the same (slab, tap, k) order whatever tile or
+// row it sits in, with no split-K, and rows outside [0, rows) read as zero like the zero gap rows between sequences: an
+// utterance's f0 is bit-identical alone, in any ragged batch and as the prefix of a streaming call (the reason the reference
+// runs this predictor in float64).  Rows outside every sequence (row2seq < 0) are written as zero: they are the zero padding
+// (gap rows, streaming look-ahead rows) of the next layer.
+constexpr int F0_BM = 128, F0_BN = 128, F0_BK = 16, F0_THREADS = 256;
+constexpr int F0_LDA = F0_BK + 4, F0_LDW = F0_BN + 4;   // pitches of 4 mod 16 doubles: conflict-free fragment loads
+template <int TAPS> struct F0Tile {
+  static constexpr int kStages = TAPS == 3 ? 3 : 2;
+  static constexpr int kArows = F0_BM + TAPS - 1;
+  static constexpr int kStage = kArows * F0_LDA + TAPS * F0_BK * F0_LDW;   // doubles per stage (even: 16-byte aligned)
+  static constexpr size_t kSmem = (size_t)kStages * kStage * sizeof(double);
+};
+
+__device__ __forceinline__ void cp_async16(void* dst, const void* src, bool ok) {
+  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void dmma16x8x8(double (&c)[4], const double (&a)[4], const double (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+
+// A [rows][K], w [TAPS][K][N], out [rows][N]; K % F0_BK == 0, N % F0_BN == 0.  Grid (N / F0_BN, ceil(rows / F0_BM)): the
+// column tiles of one row tile run side by side and share its A rows in L2.
+template <int TAPS>
+__global__ void __launch_bounds__(F0_THREADS, 1)
+f0_conv_dmma_kernel(const double* __restrict__ A, int K, const double* __restrict__ w, const double* __restrict__ bias, int N, int shift0,
+                    int rows, const int* __restrict__ row2seq, double* __restrict__ out) {
+  using T = F0Tile<TAPS>;
+  extern __shared__ __align__(16) double f0_smem[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const int wm = (warp >> 2) * 64, wn = (warp & 3) * 32;     // 2 x 4 warps, 64 x 32 each
+  const int n0 = blockIdx.x * F0_BN, r0 = blockIdx.y * F0_BM;
+  const int nk = K / F0_BK;
+
+  auto load = [&](int ks, int s) {
+    double* sa = f0_smem + (size_t)s * T::kStage;
+    double* sw = sa + T::kArows * F0_LDA;
+    const int k0 = ks * F0_BK;
+    for (int c = tid; c < T::kArows * (F0_BK / 2); c += F0_THREADS) {
+      const int i = c / (F0_BK / 2), q = c % (F0_BK / 2);
+      const int rr = r0 + shift0 + i;
+      const bool ok = rr >= 0 && rr < rows;
+      cp_async16(sa + i * F0_LDA + 2 * q, ok ? A + (size_t)rr * K + k0 + 2 * q : A, ok);
     }
-    out[(size_t)r * N + n] = acc;
+    for (int c = tid; c < TAPS * F0_BK * (F0_BN / 2); c += F0_THREADS) {
+      const int q = c % (F0_BN / 2), kk = (c / (F0_BN / 2)) % F0_BK, j = c / (F0_BK * (F0_BN / 2));
+      cp_async16(sw + (j * F0_BK + kk) * F0_LDW + 2 * q, w + ((size_t)j * K + k0 + kk) * N + n0 + 2 * q, true);
+    }
+  };
+
+  double acc[4][4][4];
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[mt][nt][i] = 0.0;
+
+#pragma unroll
+  for (int s = 0; s < T::kStages - 1; ++s) {
+    if (s < nk) load(s, s);
+    asm volatile("cp.async.commit_group;" ::: "memory");
   }
+  for (int ks = 0; ks < nk; ++ks) {
+    asm volatile("cp.async.wait_group %0;" ::"n"(T::kStages - 2) : "memory");
+    __syncthreads();                                        // slab ks landed for all threads; slab ks-1's buffer is free
+    if (ks + T::kStages - 1 < nk) load(ks + T::kStages - 1, (ks + T::kStages - 1) % T::kStages);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    const double* sa = f0_smem + (size_t)(ks % T::kStages) * T::kStage;
+    const double* sw = sa + T::kArows * F0_LDA;
+#pragma unroll
+    for (int j = 0; j < TAPS; ++j) {
+#pragma unroll
+      for (int kk = 0; kk < F0_BK; kk += 8) {
+        double a[4][4], b[4][2];
+#pragma unroll
+        for (int mt = 0; mt < 4; ++mt) {
+          const double* p = sa + (wm + mt * 16 + g + j) * F0_LDA + kk + t;
+          a[mt][0] = p[0];
+          a[mt][1] = p[8 * F0_LDA];
+          a[mt][2] = p[4];
+          a[mt][3] = p[8 * F0_LDA + 4];
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const double* p = sw + (j * F0_BK + kk + t) * F0_LDW + wn + nt * 8 + g;
+          b[nt][0] = p[0];
+          b[nt][1] = p[4 * F0_LDW];
+        }
+#pragma unroll
+        for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) dmma16x8x8(acc[mt][nt], a[mt], b[nt]);
+      }
+    }
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + wm + mt * 16 + g + 8 * h;
+      if (r >= rows) continue;
+      const bool valid = row2seq[r] >= 0;
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) {
+        const int n = n0 + wn + nt * 8 + 2 * t;
+        double2 v = make_double2(0.0, 0.0);
+        if (valid) {
+          v.x = acc[mt][nt][2 * h] + bias[n];
+          v.y = acc[mt][nt][2 * h + 1] + bias[n + 1];
+          v.x = v.x > 0.0 ? v.x : expm1(v.x);
+          v.y = v.y > 0.0 ? v.y : expm1(v.y);
+        }
+        *reinterpret_cast<double2*>(out + (size_t)r * N + n) = v;
+      }
+    }
 }
 // f0 = |x . w + b| (f0_predictor.py:103), written as float32
 __global__ void f0_head_f64_kernel(const double* __restrict__ x, const double* __restrict__ w, double b, int rows, const int* __restrict__ row2seq,
@@ -808,6 +913,7 @@ void hift3_build(cvk_ctx* ctx) {
     CVK_CHECK_CUDA(cudaDeviceSynchronize());
     F64Conv& f = x->conv[i];
     f.N = c.N; f.K = c.K; f.taps = c.taps; f.shift0 = c.shift0;
+    CVK_REQUIRE(f.K % F0_BK == 0 && f.N % F0_BN == 0 && f.taps == (i == 0 ? 4 : 3), "unexpected f0 predictor convolution shape");
     f.w = (double*)ctx->dmalloc((size_t)c.N * c.taps * c.K * sizeof(double));
     f.bias = (double*)ctx->dmalloc((size_t)c.N * sizeof(double));
     f64_weight_kernel<<<256, 256>>>(c.w32, f.w, c.N, c.taps, c.K);
@@ -879,6 +985,11 @@ void hift3_build(cvk_ctx* ctx) {
   ctx->hift3_extra = x;
 }
 
+void hift3_setup() {
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(f0_conv_dmma_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F0Tile<3>::kSmem));
+  CVK_CHECK_CUDA(cudaFuncSetAttribute(f0_conv_dmma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F0Tile<4>::kSmem));
+}
+
 // SineGen2.rand_ini [9] and SineGen2.sine_waves [n][9] (generator.py:223-226): module attributes, not state_dict entries
 void hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_noise, long long n, int on_device) {
   Hift3Extra* x = ctx->hift3_extra ? (Hift3Extra*)ctx->hift3_extra : new Hift3Extra();
@@ -931,7 +1042,11 @@ void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, int
   for (int i = 0; i < 5; ++i) {
     const F64Conv& f = x->conv[i];
     double* o = (i & 1) ? bb : a;
-    conv_f64_kernel<<<s0.R, 128, 0, st>>>(cur, f.K, f.w, f.bias, f.N, f.taps, f.shift0, s0.R, s0.d_row2seq, o);
+    const dim3 grid(f.N / F0_BN, ceil_div(s0.R, F0_BM));
+    if (f.taps == 4)
+      f0_conv_dmma_kernel<4><<<grid, F0_THREADS, F0Tile<4>::kSmem, st>>>(cur, f.K, f.w, f.bias, f.N, f.shift0, s0.R, s0.d_row2seq, o);
+    else
+      f0_conv_dmma_kernel<3><<<grid, F0_THREADS, F0Tile<3>::kSmem, st>>>(cur, f.K, f.w, f.bias, f.N, f.shift0, s0.R, s0.d_row2seq, o);
     ctx->launches++;
     CVK_LAUNCH_CHECK();
     cur = o;

@@ -23,6 +23,28 @@ PRE_LOOKAHEAD = 3            # cosyvoice2.yaml:46
 SAMPLES_PER_FRAME = 480
 
 
+class SilentTokenFilter:
+    """The silent-token rule of the reference's LM job (cli/model.py:102, 121-127) for one request: a silent token is dropped once
+    more than MAX_RUN of them have come in a row.  CosyVoice2's list of silent tokens is empty, so it never drops anything."""
+    MAX_RUN = 5
+
+    def __init__(self, silent_tokens):
+        self.silent_tokens = silent_tokens
+        self.run = 0
+
+    def keep(self, tok):
+        """feed the request's next id: whether it is kept"""
+        if tok in self.silent_tokens:
+            self.run += 1
+            return self.run <= self.MAX_RUN
+        self.run = 0
+        return True
+
+    def filter(self, ids):
+        """the kept ids of a whole sequence"""
+        return [t for t in ids if self.keep(t)]
+
+
 class _LmStopped(Exception):
     """raised into a batched LM generation whose consumer has gone away"""
 
@@ -585,6 +607,7 @@ class B200CosyVoice2Model:
             ev[0].record()
         ids = self.lm_generate([i["text"] for i in inputs], [i["prompt_text"] for i in inputs],
                                [i["llm_prompt_speech_token"] for i in inputs], uniforms)
+        ids = [SilentTokenFilter(self.silent_tokens).filter(x) for x in ids]      # what tts() keeps of each request's ids
         with torch.cuda.stream(self.stream):
             ev[1].record()
         toks = [torch.tensor(x, dtype=torch.int32).unsqueeze(0) for x in ids]
@@ -719,32 +742,23 @@ class B200CosyVoice2Model:
         """cli/model.py:101-129 (non-generator text).  Tokens are appended to the session list as they arrive."""
         if hasattr(text, "__next__") or (hasattr(text, "__iter__") and not torch.is_tensor(text)):
             # cli/model.py:113-123: text generator -> bi-stream decoding, tokens appended one by one
-            cur_silent, max_silent = 0, 5                  # cli/model.py:102,121-127 (silent_tokens is empty for CosyVoice2)
+            silent = SilentTokenFilter(self.silent_tokens)
             with self._lm_stream() as lm_stream:
                 for tok in self.lm_generate_bistream(iter(text), prompt_text, llm_prompt_speech_token, stream=lm_stream):
-                    if tok in self.silent_tokens:
-                        cur_silent += 1
-                        if cur_silent > max_silent:
-                            continue
-                    else:
-                        cur_silent = 0
-                    self.tts_speech_token_dict[uuid].append(tok)
+                    if silent.keep(tok):
+                        self.tts_speech_token_dict[uuid].append(tok)
             self.llm_end_dict[uuid] = True
             return
 
-        st = {"consumed": 0, "silent": 0}
+        st = {"consumed": 0}
+        silent = SilentTokenFilter(self.silent_tokens)
 
         def progress(out_ids, out_count, live):
             n = int(out_count[0].item())
             if n > st["consumed"]:
                 for tok in out_ids[0, st["consumed"]:n].tolist():
-                    if tok in self.silent_tokens:            # cli/model.py:121-127 (empty list for CosyVoice2: never taken)
-                        st["silent"] += 1
-                        if st["silent"] > 5:
-                            continue
-                    else:
-                        st["silent"] = 0
-                    self.tts_speech_token_dict[uuid].append(tok)
+                    if silent.keep(tok):
+                        self.tts_speech_token_dict[uuid].append(tok)
                 st["consumed"] = n
         # the LM job decodes on its own stream (cli/model.py:103: `with self.llm_context`, a side stream) while token2wav runs on
         # the model's stream
@@ -920,16 +934,11 @@ class B200CosyVoice2Model:
                     emb=r.get("flow_embedding", torch.zeros(0, 192))) for r in inputs]
         toks = [[] for _ in range(B)]
         lm_state = {"end": False, "err": None, "stop": False}
-        silent = [0] * B
+        silent = [SilentTokenFilter(self.silent_tokens) for _ in range(B)]
 
         def emit(b, tok):
-            if tok in self.silent_tokens:            # cli/model.py:121-127
-                silent[b] += 1
-                if silent[b] > 5:
-                    return
-            else:
-                silent[b] = 0
-            toks[b].append(tok)
+            if silent[b].keep(tok):
+                toks[b].append(tok)
 
         def llm_job():
             try:

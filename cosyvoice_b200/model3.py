@@ -5,9 +5,15 @@ tokens) and replaces token2wav: the flow is the DiT one (stage "flow3"), the voc
 of the CosyVoice2 mel / source / speech caches with a cross-fade it keeps ALL mel frames produced so far, re-runs the causal vocoder
 over them and emits the samples beyond ``speech_offset``.  This class follows that bookkeeping literally.
 
-Status (end of round 1): the flow stage is parity-green on the GPU; the LM variant and the vocoder (offline and streaming call)
-are written but had their first GPU run only at the round-end test pass.  The class itself is checked on the CPU against the reference's own
-CosyVoice3Model.tts with the device primitives faked by the oracle (tests/test_host_logic_cpu.py)."""
+Offline requests also batch: the inherited ``tts_batch`` / ``tts_batch_device`` run the LM, the DiT flow and the causal vocoder
+(``hift_batch`` below) once for the whole batch, and ``TtsBatcher`` serves CosyVoice3 offline requests through them.  Each request
+gets what ``tts()`` gives it alone: the causal vocoder reads its stored noise from each utterance's start and its float64 f0
+predictor sums in an order that does not depend on the batch.  Batched streaming (``tts_stream_batch`` / ``tts_bistream_batch``)
+is not built.
+
+The class is checked on the CPU against the reference's own CosyVoice3Model.tts with the device primitives faked by the oracle
+(tests/test_host_logic_cpu.py, tests/test_tts3_batch_cpu.py) and on the GPU against the reference's waveform
+(tests/test_zz_model3_gpu.py, tests/test_zz_tts3_batch_gpu.py)."""
 import torch
 
 from .model import B200CosyVoice2Model, TOKEN_MEL_RATIO, _count
@@ -64,6 +70,16 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
             pf = torch.cat([f[0].to(d) for f in prompt_feats], 0) if sum(pl) else None
             emb = torch.cat([e.reshape(1, -1).to(d) for e in embeddings], 0)
             return self.ctx.flow3_inference(toks, tl, pf, pl, emb, n_timesteps=self.n_timesteps, streaming=streaming, finalize=finalize)
+
+    def hift_batch(self, mel_tm, lens, cache_source=None, cache_lens=None, noise=None):
+        """The causal vocoder over a ragged batch (finalize=True): mel [sum T, 80] -> (wav [sum 480 T], source [sum 480 T]), the pair
+        the inherited tts_batch_device takes.  Its source noise is the module's stored sine_waves indexed from each utterance's start
+        (generator.py:303-307), so a noise tensor or a source cache from the caller has no meaning here."""
+        if noise is not None or cache_source is not None:
+            raise ValueError("the causal vocoder draws its noise from its stored sine_waves: noise= and cache_source= are not accepted")
+        with torch.cuda.stream(self.stream), self.ctx.lock:
+            wav, _, src = self.ctx.hift3_inference(mel_tm, lens, finalize=True)
+        return wav, src
 
     def token2wav(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream=False, finalize=False, speed=1.0):
         """cli/model.py:425-450"""
