@@ -15,7 +15,8 @@ inside a batch (the model's RNG streams are consumed in input order, so a fixed 
 needed here.
 
 Streaming requests (``submit_stream`` / ``submit_stream_pcm``) are served by ``tts_stream_batch``, which hands out every request's
-chunks as they become ready.  A batch is either all streaming or all offline: it is the run of requests of the same kind at the
+chunks as they become ready; it exists for CosyVoice2 (``B200CosyVoice2Model``) and CosyVoice3 (``B200CosyVoice3Model``) models
+alike, so the queue serves both families' offline and streaming requests.  A batch is either all streaming or all offline: it is the run of requests of the same kind at the
 head of the queue, so it also closes early when a request of the other kind is waiting behind it, and no request is ever moved
 ahead of an earlier one of the other kind.
 """
@@ -76,7 +77,9 @@ class TtsBatcher:
     ``submit_pcm`` -> Future of the int16 PCM bytes.  ``submit_stream`` / ``submit_stream_pcm`` -> iterator over the request's
     chunks (what ``tts`` yields for stream=True: float [1, n] tensors, or their int16 PCM bytes).  ``tts_kwargs`` are the keyword
     arguments of ``CosyVoice2Model.tts`` that the batched pipeline consumes: text, prompt_text, llm_prompt_speech_token,
-    flow_prompt_speech_token, prompt_speech_feat, flow_embedding."""
+    flow_prompt_speech_token, prompt_speech_feat, flow_embedding.  ``model`` is a ``B200CosyVoice2Model`` or a
+    ``B200CosyVoice3Model``: both serve offline (``tts_batch``) and streaming (``tts_stream_batch``) batches, and a streaming
+    request gets the chunk schedule ``tts(stream=True)`` gives it alone."""
 
     def __init__(self, model, max_batch=32, max_wait_ms=10.0):
         assert max_batch >= 1

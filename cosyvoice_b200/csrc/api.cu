@@ -24,8 +24,8 @@ cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context)
 void llm_session_destroy(cvk_ctx* ctx, cvk_lm_session* s);
 void hift3_build(cvk_ctx* ctx);
 void hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_noise, long long n, int on_device);
-void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, int finalize, float* wav, float* f0_out, float* source_out,
-                     cudaStream_t st);
+void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int* finalize, int B, float* wav, float* f0_out,
+                     float* source_out, cudaStream_t st);
 void dit_build(cvk_ctx* ctx, const int* cfg, int ncfg);
 void dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
                    int B, int streaming, float* out, cudaStream_t st);
@@ -759,7 +759,15 @@ int cvk_hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens_host, in
                         float* source_out, void* stream) {
   CVK_API_BEGIN
   CVK_REQUIRE(mel && lens_host && wav && B > 0, "cvk_hift3_inference: bad arguments");
-  hift3_inference(ctx, mel, lens_host, B, finalize, wav, f0_out, source_out, (cudaStream_t)stream);
+  const std::vector<int> flags(B, finalize);
+  hift3_inference(ctx, mel, lens_host, flags.data(), B, wav, f0_out, source_out, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_hift3_inference_rows(cvk_ctx* ctx, const float* mel, const int* lens_host, const int* finalize_host, int B, float* wav,
+                             float* f0_out, float* source_out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(mel && lens_host && finalize_host && wav && B > 0, "cvk_hift3_inference_rows: bad arguments");
+  hift3_inference(ctx, mel, lens_host, finalize_host, B, wav, f0_out, source_out, (cudaStream_t)stream);
   CVK_API_END
 }
 int cvk_dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,

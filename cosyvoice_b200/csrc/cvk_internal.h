@@ -294,6 +294,7 @@ void layernorm(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const float* gamma, 
                float post_scale, const int* row2seq, const Mat& out, const float* rowvec = nullptr, int rowvec_ld = 0);
 void unpack_rows_skip(cvk_ctx* ctx, cudaStream_t st, const Mat& in, const Seqs& s, const int* skip_host, float* dense, int C);
 Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& s, int drop_tail, cudaStream_t st);
+Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& s, const int* drop_tail_host /*[s.B]*/, cudaStream_t st);
 Seqs subseqs(cvk_ctx* ctx, const Seqs& s, const int* skip_host, cudaStream_t st);
 void rmsnorm(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const float* gamma, float eps, const Mat& out);
 void act_copy(cvk_ctx* ctx, cudaStream_t st, const Mat& x, int act, float param, const float* alpha, const int* row2seq,

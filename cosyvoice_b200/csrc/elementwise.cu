@@ -65,14 +65,15 @@ Seqs scale_seqs(cvk_ctx* ctx, const Seqs& b, int scale, int extra_front, cudaStr
   return s;
 }
 
-// same rows, every sequence shortened by drop_tail rows at its end (flow look-ahead context, flow/flow.py:259-261)
-Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& b, int drop_tail, cudaStream_t st) {
+// same rows, sequence i shortened by drop_tail[i] rows at its end (look-ahead context per sequence: the CosyVoice3 vocoder's
+// streaming and final utterances in one call)
+Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& b, const int* drop_tail, cudaStream_t st) {
   Seqs s;
   s.B = b.B;
   s.start = b.start;
   s.len.resize(b.B);
   for (int i = 0; i < b.B; ++i) {
-    s.len[i] = b.len[i] - drop_tail;
+    s.len[i] = b.len[i] - drop_tail[i];
     CVK_REQUIRE(s.len[i] > 0, "sequence shorter than the look-ahead context");
     if (s.len[i] > s.max_len) s.max_len = s.len[i];
     s.sum_len += s.len[i];
@@ -80,6 +81,12 @@ Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& b, int drop_tail, cudaStream_t st) {
   s.R = b.R;
   upload_seqs(ctx, s, st, true);
   return s;
+}
+
+// same rows, every sequence shortened by drop_tail rows at its end (flow look-ahead context, flow/flow.py:259-261)
+Seqs shrink_seqs(cvk_ctx* ctx, const Seqs& b, int drop_tail, cudaStream_t st) {
+  const std::vector<int> d(b.B, drop_tail);
+  return shrink_seqs(ctx, b, d.data(), st);
 }
 
 // same rows, sequence b restricted to its first skip[b] rows (prompt part)

@@ -153,7 +153,8 @@ template <typename TO>
 __global__ void stft16_kernel(const float* __restrict__ src, const int* __restrict__ start0, const int* __restrict__ len0,
                               const int* __restrict__ start3, TO* __restrict__ out, int ldo, const int* __restrict__ len_sig = nullptr) {
   int b = blockIdx.y;
-  // len_sig (CosyVoice3 streaming call): the source is len_sig frames long, only the first len0*120 + 1 STFT frames are kept
+  // len_sig (CosyVoice3 vocoder): sequence b's source is len_sig[b] frames long, only the first len0[b]*120 + 1 STFT frames are
+  // kept.  A final utterance passes len_sig[b] == len0[b], which is the nullptr case.
   int L = (len_sig ? len_sig[b] : len0[b]) * kUpscale;
   int F = len_sig ? len0[b] * 120 + 1 : L / 4 + 1;
   const float* x = src + (size_t)start0[b] * kUpscale;
@@ -188,11 +189,13 @@ __global__ void stft16_kernel(const float* __restrict__ src, const int* __restri
 // overlap-add / window-envelope, trim 8, clamp +-0.99 (generator.py:533-538, torch.istft center=True).
 // Block: 512 output samples, which need frames f_base-1 .. f_base+129.
 __global__ void istft16_kernel(const float* __restrict__ xp, int ldx, const int* __restrict__ start3, const int* __restrict__ len0,
-                               const int* __restrict__ out_off, float* __restrict__ wav, float limit, int drop_tail = 0) {
+                               const int* __restrict__ out_off, float* __restrict__ wav, float limit,
+                               const int* __restrict__ drop_tail = nullptr) {
   __shared__ float fr[131][17];   // frames f_base-1 .. f_base+129
   int b = blockIdx.y;
   int L = len0[b] * kUpscale;
   int F = L / 4 + 1;
+  const int L_out = L - (drop_tail ? drop_tail[b] : 0);
   int f_base = blockIdx.x * 128;          // first frame whose leading 4 samples this block emits
   if (f_base * 4 >= L) return;
   for (int i = threadIdx.x; i < 131; i += blockDim.x) {
@@ -226,7 +229,7 @@ __global__ void istft16_kernel(const float* __restrict__ xp, int ldx, const int*
   // output sample n (after trimming 8) lives at padded position p = n + 8; frames f with 4f <= p < 4f + 16
   for (int i = threadIdx.x; i < 512; i += blockDim.x) {
     int n = f_base * 4 + i;
-    if (n >= L - drop_tail) break;        // drop_tail: samples of the last look-ahead frame are not emitted (generator.py:709-710)
+    if (n >= L_out) break;        // drop_tail[b]: samples of the last look-ahead frame are not emitted (generator.py:709-710)
     int p = n + 8;
     int f_hi = p >> 2;
     float acc = 0.f, env = 0.f;
@@ -550,13 +553,14 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
   return xp;
 }
 
-// lens: frames per utterance that define the OUTPUT offsets (sum 480*lens samples); drop_tail samples at the end of every utterance
-// are not written (0 except for the CosyVoice3 streaming call)
-static void hift_istft(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const int* lens, const Mat& xp, float* wav_dense, int drop_tail = 0) {
+// lens: frames per utterance that define the OUTPUT offsets (sum 480*lens samples); d_drop_tail[b] samples at the end of utterance
+// b are not written (device array; nullptr = none, 480 for a CosyVoice3 streaming utterance)
+static void hift_istft(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const int* lens, const Mat& xp, float* wav_dense,
+                       const int* d_drop_tail = nullptr) {
   const Seqs& s0 = g.s0;
   int* ooff = upload_ints(ctx, prefix_offsets(lens, s0.B), st);
   int bx = ceil_div(s0.max_len * kUpscale, 512);
-  istft16_kernel<<<dim3(bx, s0.B), 128, 0, st>>>(xp.f32(), xp.ld, g.lv[2].d_start, s0.d_len, ooff, wav_dense, 0.99f, drop_tail);
+  istft16_kernel<<<dim3(bx, s0.B), 128, 0, st>>>(xp.f32(), xp.ld, g.lv[2].d_start, s0.d_len, ooff, wav_dense, 0.99f, d_drop_tail);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }
@@ -1002,34 +1006,42 @@ void hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_nois
   ctx->hift3_extra = x;
 }
 
-// generator.py:714-726.  mel dense [sum T, 80].  finalize: wav [sum 480 T], f0_out [sum T], source_out [sum 480 T] (optional);
-// streaming call (finalize = 0): wav [sum 480 (T-8)], f0_out [sum (T-3)], source_out [sum 480 (T-3)]
-void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, int finalize, float* wav, float* f0_out, float* source_out,
-                     cudaStream_t st) {
+// generator.py:714-726 with a finalize flag per utterance.  mel dense [sum T, 80]; utterance b's outputs, back to back:
+// finalize[b] != 0: wav 480 T, f0_out T, source_out 480 T (f0_out / source_out optional);
+// finalize[b] == 0 (streaming): wav 480 (T-8), f0_out T-3, source_out 480 (T-3)
+void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int* finalize, int B, float* wav, float* f0_out,
+                     float* source_out, cudaStream_t st) {
   const HiftModel* m = ctx->hift3;
   Hift3Extra* x = (Hift3Extra*)ctx->hift3_extra;
   CVK_REQUIRE(m && x && x->conv[0].w, "hift3 stage not finalised");
   CVK_REQUIRE(x->noise != nullptr, "cvk_hift3_set_noise has not been called");
+  // Geometry.  A final utterance has one geometry of T frames.  A streaming utterance (generator.py:676-683, 709-710, 722-725;
+  // f0_predictor.py:99-100): the f0 predictor consumes 3 frames of look-ahead (f0 / source have T-3 frames), conv_pre 4 more
+  // (the body runs on T-7 frames, the source STFT is cut to its first 120(T-7)+1 frames) and the last 480 samples are dropped
+  // (480(T-8) returned).  All geometries share the row starts of the T-frame one, so the look-ahead rows are simply read by the
+  // right-looking convs, and each utterance's look-ahead is its own: one call serves streaming and final utterances together.
+  std::vector<int> la_f0(B), la_body(B), drop(B), lens_src(B), lens_out(B);
+  bool any_stream = false;
+  for (int b = 0; b < B; ++b) {
+    const bool fin = finalize[b] != 0;
+    CVK_REQUIRE(lens[b] > 0, "cvk_hift3_inference: an utterance of 0 mel frames");
+    CVK_REQUIRE(fin || lens[b] >= 9, "cvk_hift3_inference: a streaming utterance needs at least 9 mel frames");
+    any_stream |= !fin;
+    la_f0[b] = fin ? 0 : 3;
+    la_body[b] = fin ? 0 : 3 + 4;
+    drop[b] = fin ? 0 : kUpscale;
+    lens_src[b] = lens[b] - la_f0[b];
+    lens_out[b] = fin ? lens[b] : lens[b] - 8;
+    CVK_REQUIRE((long long)lens_src[b] * kUpscale <= x->noise_n, "stored source noise shorter than the utterance");
+  }
   ctx->arena.reset();
-  // Geometry.  Offline: one geometry of T frames.  Streaming call (generator.py:676-683, 709-710, 722-725; f0_predictor.py:99-100):
-  // the f0 predictor consumes 3 frames of look-ahead (f0 / source have T-3 frames), conv_pre 4 more (the body runs on T-7
-  // frames, the source STFT is cut to its first 120(T-7)+1 frames) and the last 480 samples are dropped (480(T-8) returned).
-  // All geometries share the row starts of the T-frame one, so the look-ahead rows are simply read by the right-looking convs.
-  const int la_f0 = finalize ? 0 : 3, la_pre = finalize ? 0 : 4;
   HiftGeom g;
-  Seqs sF = make_seqs(ctx, lens, B, 8, 1, 0, st);                         // all frames
-  Seqs s0 = la_f0 ? shrink_seqs(ctx, sF, la_f0, st) : sF;                 // f0 / source frames
-  g.s0 = la_f0 ? shrink_seqs(ctx, sF, la_f0 + la_pre, st) : sF;           // body frames
+  Seqs sF = make_seqs(ctx, lens, B, 8, 1, 0, st);                             // all frames
+  Seqs s0 = any_stream ? shrink_seqs(ctx, sF, la_f0.data(), st) : sF;         // f0 / source frames
+  g.s0 = any_stream ? shrink_seqs(ctx, sF, la_body.data(), st) : sF;          // body frames
   g.lv[0] = scale_seqs(ctx, g.s0, 8, 0, st);
   g.lv[1] = scale_seqs(ctx, g.s0, 40, 0, st);
   g.lv[2] = scale_seqs(ctx, g.s0, 120, 1, st);
-  std::vector<int> lens_src(B), lens_out(B);
-  for (int b = 0; b < B; ++b) {
-    CVK_REQUIRE(finalize || lens[b] >= 9, "cvk_hift3_inference: a streaming call needs at least 9 mel frames");
-    lens_src[b] = lens[b] - la_f0;
-    lens_out[b] = finalize ? lens[b] : lens[b] - 8;
-    CVK_REQUIRE((long long)lens_src[b] * kUpscale <= x->noise_n, "stored source noise shorter than the utterance");
-  }
   Mat mel32 = pack_mel(ctx, st, sF, mel);
   // ---- f0 predictor in float64
   double* a = (double*)ctx->arena.alloc(sizeof(double) * (size_t)s0.R * 512);
@@ -1079,6 +1091,7 @@ void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, int
     CVK_LAUNCH_CHECK();
   }
   // ---- vocoder body (shared with CosyVoice2) + ISTFT
-  Mat xp = hift_body(ctx, st, g, mel32, src, m, finalize ? nullptr : s0.d_len);
-  hift_istft(ctx, st, g, lens_out.data(), xp, wav, finalize ? 0 : kUpscale);
+  // per utterance: the source length the STFT reads and the samples the ISTFT drops (nullptr when every utterance is final)
+  Mat xp = hift_body(ctx, st, g, mel32, src, m, any_stream ? s0.d_len : nullptr);
+  hift_istft(ctx, st, g, lens_out.data(), xp, wav, any_stream ? upload_ints(ctx, drop, st) : nullptr);
 }

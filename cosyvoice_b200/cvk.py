@@ -79,6 +79,7 @@ SIGNATURES = {
     "cvk_cfm_set_noise": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int]),
     "cvk_hift3_set_noise": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_longlong, ctypes.c_int]),
     "cvk_hift3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]),
+    "cvk_hift3_inference_rows": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp, _vp, _vp, _vp]),
     "cvk_dit_estimator": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_flow3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, _vp, _c_int_p, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_lm_session_create": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp)]),
@@ -420,6 +421,23 @@ class Context:
         src = torch.empty(n_src * 480, device=self.device)
         self._check(self.lib.cvk_hift3_inference(self.h, _ptr(mel), _ints(lens), len(lens), int(finalize), _ptr(wav), _ptr(f0), _ptr(src),
                                                  _stream()))
+        return wav, f0, src
+
+    def hift3_inference_rows(self, mel, lens, finalize):
+        """hift3_inference with a finalize flag per utterance: mel [sum T, 80] -> (wav, f0, src), utterance b's parts back to back,
+        480 T / T / 480 T samples when finalize[b] and 480 (T-8) / T-3 / 480 (T-3) when not (streaming, T >= 9).  Each utterance
+        gets exactly what hift3_inference gives it alone with its own flag; one launch sequence serves the whole call."""
+        if len(finalize) != len(lens):
+            raise ValueError("hift3_inference_rows: one finalize flag per utterance")
+        mel = _f32(mel, self.device)
+        fin = [bool(f) for f in finalize]
+        n_src = sum(int(l) - (0 if f else 3) for l, f in zip(lens, fin))
+        n_out = sum(int(l) - (0 if f else 8) for l, f in zip(lens, fin))
+        wav = torch.empty(max(n_out, 0) * 480, device=self.device)
+        f0 = torch.empty(max(n_src, 0), device=self.device)
+        src = torch.empty(max(n_src, 0) * 480, device=self.device)
+        self._check(self.lib.cvk_hift3_inference_rows(self.h, _ptr(mel), _ints(lens), _ints([int(f) for f in fin]), len(lens), _ptr(wav),
+                                                      _ptr(f0), _ptr(src), _stream()))
         return wav, f0, src
 
     def dit_estimator(self, x, mu, t, spks, cond, lens, streaming=False):

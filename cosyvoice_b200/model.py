@@ -987,9 +987,56 @@ class B200CosyVoice2Model:
             if self.stream is not None:
                 self.stream.synchronize()
 
+    def _stream_vocode(self, voc, mels, st, finishing, noise_fns):
+        """the vocoder step of a poll round: requests `voc` (in order) with their new mel frames mels[i], in one vocoder call, each
+        with its own cached mel / source and token2wav's cross-fade (cli/model.py:292-326); requests in `finishing` make their
+        final call.  Returns {i: float32 CPU [n]}, copied to the host in one D2H for the round."""
+        outs = {}
+        with torch.cuda.stream(self.stream):
+            tts_mel, lens, cache_src, cache_lens, noise = [], [], [], [], []
+            for i in voc:
+                c = st[i]["cache"]
+                m_i = torch.cat([c["mel"], mels[i]], 0) if c is not None else mels[i]
+                tts_mel.append(m_i)
+                lens.append(int(m_i.shape[0]))
+                cache_lens.append(int(c["source"].shape[0]) if c is not None else 0)
+                if c is not None:
+                    cache_src.append(c["source"])
+                noise.append(self._noise_for(i, lens[-1] * SAMPLES_PER_FRAME, noise_fns))
+            with self.ctx.lock:
+                wav, src = self.ctx.hift_inference(torch.cat(tts_mel, 0), lens, torch.cat(noise, 0),
+                                                   torch.cat(cache_src) if cache_src else None, cache_lens if cache_src else None)
+            o = 0
+            for i, m_i, n in zip(voc, tts_mel, lens):
+                w, s_ = wav[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME], src[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME]
+                o += n
+                c = st[i]["cache"]
+                if c is not None:
+                    w = self._fade_in_out(w, c["speech"])
+                if i in finishing:
+                    outs[i] = w
+                else:
+                    st[i]["cache"] = {"mel": m_i[-self.mel_cache_len:].clone(), "source": s_[-self.source_cache_len:].clone(),
+                                      "speech": w[-self.source_cache_len:].clone()}
+                    outs[i] = w[:-self.source_cache_len]
+            flat = torch.cat([outs[i] for i in voc]).cpu()       # one D2H for the round
+        if self.stream is not None:
+            self.stream.synchronize()
+        return self._split_host(voc, outs, flat)
+
+    @staticmethod
+    def _split_host(voc, outs, flat):
+        """the host copy `flat` of the device tensors outs[i] (concatenated in voc order), split back per request"""
+        host, o = {}, 0
+        for i in voc:
+            n = int(outs[i].shape[0])
+            host[i] = flat[o:o + n]
+            o += n
+        return host
+
     def _stream_round(self, req, st, toks, ready, finishing, noise_fns):
-        """one poll round of tts_stream_batch: flow for every ready / finishing request (at most three calls), one vocoder call,
-        then token2wav's cache and cross-fade bookkeeping per request (cli/model.py:292-326)"""
+        """one poll round of tts_stream_batch: flow for every ready / finishing request (at most three calls), then one vocoder call
+        with the model's token2wav bookkeeping per request (_stream_vocode)"""
         d = self.device
         slot_grp, prefix_grp = [], []
         for i, this_hop in ready:
@@ -1037,53 +1084,16 @@ class B200CosyVoice2Model:
             for (i, _, _), n in zip(grp, lens):
                 mels[i] = mel[o + st[i]["offset"] * TOKEN_MEL_RATIO:o + n]
                 o += n
-        # vocoder: every request of the round in one call, each with its own cached mel / source
+        # vocoder: every request of the round in one call
         order = [i for i, _ in ready] + finishing
-        outs = {}
         voc = [i for i in order if i in mels]
-        if voc:
-            with torch.cuda.stream(self.stream):
-                tts_mel, lens, cache_src, cache_lens, noise = [], [], [], [], []
-                for i in voc:
-                    c = st[i]["cache"]
-                    m_i = torch.cat([c["mel"], mels[i]], 0) if c is not None else mels[i]
-                    tts_mel.append(m_i)
-                    lens.append(int(m_i.shape[0]))
-                    cache_lens.append(int(c["source"].shape[0]) if c is not None else 0)
-                    if c is not None:
-                        cache_src.append(c["source"])
-                    noise.append(self._noise_for(i, lens[-1] * SAMPLES_PER_FRAME, noise_fns))
-                with self.ctx.lock:
-                    wav, src = self.ctx.hift_inference(torch.cat(tts_mel, 0), lens, torch.cat(noise, 0),
-                                                       torch.cat(cache_src) if cache_src else None, cache_lens if cache_src else None)
-                o = 0
-                for i, m_i, n in zip(voc, tts_mel, lens):
-                    w, s_ = wav[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME], src[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME]
-                    o += n
-                    c = st[i]["cache"]
-                    if c is not None:
-                        w = self._fade_in_out(w, c["speech"])
-                    if i in finishing:
-                        outs[i] = w
-                    else:
-                        st[i]["cache"] = {"mel": m_i[-self.mel_cache_len:].clone(), "source": s_[-self.source_cache_len:].clone(),
-                                          "speech": w[-self.source_cache_len:].clone()}
-                        outs[i] = w[:-self.source_cache_len]
-                flat = torch.cat([outs[i] for i in voc]).cpu() if voc else None       # one D2H for the round
-            if self.stream is not None:
-                self.stream.synchronize()
+        outs = self._stream_vocode(voc, mels, st, finishing, noise_fns) if voc else {}
         for i, this_hop in ready:
             st[i]["offset"] += this_hop
             st[i]["hop"] = min(self.token_max_hop_len, st[i]["hop"] * self.stream_scale_factor)
-        o = 0
         results = []
         for i in order:
-            if i in outs:
-                n = int(outs[i].shape[0])
-                results.append((i, {"tts_speech": flat[o:o + n].unsqueeze(0)}))
-                o += n
-            else:
-                results.append((i, {"tts_speech": torch.zeros(1, 0)}))
+            results.append((i, {"tts_speech": outs[i].unsqueeze(0) if i in outs else torch.zeros(1, 0)}))
         for i in finishing:
             st[i]["done"] = True
             if st[i]["slot"] is not None:

@@ -8,15 +8,20 @@ over them and emits the samples beyond ``speech_offset``.  This class follows th
 Offline requests also batch: the inherited ``tts_batch`` / ``tts_batch_device`` run the LM, the DiT flow and the causal vocoder
 (``hift_batch`` below) once for the whole batch, and ``TtsBatcher`` serves CosyVoice3 offline requests through them.  Each request
 gets what ``tts()`` gives it alone: the causal vocoder reads its stored noise from each utterance's start and its float64 f0
-predictor sums in an order that does not depend on the batch.  Batched streaming (``tts_stream_batch`` / ``tts_bistream_batch``)
-is not built.
+predictor sums in an order that does not depend on the batch.
+
+Streaming requests batch too: ``tts_stream_batch`` / ``tts_bistream_batch`` run the inherited poll loop (multi-slot DiT flow
+sessions, ``flow_batch`` for prefix recomputes and final calls) with the vocoder step replaced by ``_stream_vocode`` below, which
+keeps token2wav's bookkeeping per request (all mel so far, ``speech_offset``) and vocodes every request of a round - streaming
+chunks and final calls together - in one ``hift3_inference_rows`` call with a finalize flag per utterance.  ``TtsBatcher``
+serves CosyVoice3 streaming requests through them.
 
 The class is checked on the CPU against the reference's own CosyVoice3Model.tts with the device primitives faked by the oracle
-(tests/test_host_logic_cpu.py, tests/test_tts3_batch_cpu.py) and on the GPU against the reference's waveform
-(tests/test_zz_model3_gpu.py, tests/test_zz_tts3_batch_gpu.py)."""
+(tests/test_host_logic_cpu.py, tests/test_tts3_batch_cpu.py, tests/test_stream3_batch_cpu.py) and on the GPU against the
+reference's waveform (tests/test_zz_model3_gpu.py, tests/test_zz_tts3_batch_gpu.py, tests/test_zz_stream3_batch_gpu.py)."""
 import torch
 
-from .model import B200CosyVoice2Model, TOKEN_MEL_RATIO, _count
+from .model import B200CosyVoice2Model, SAMPLES_PER_FRAME, TOKEN_MEL_RATIO, _count
 
 
 class B200CosyVoice3Model(B200CosyVoice2Model):
@@ -32,14 +37,36 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
         self.silent_tokens = [1, 2, 28, 29, 55, 248, 494, 2241, 2242, 2322, 2323]
 
     def tts_stream_batch(self, inputs, uniforms=None, noise_fns=None):
-        """Not built for CosyVoice3: the inherited scheduler keeps CosyVoice2's vocoder caches and cross-fade, while CosyVoice3's
-        causal vocoder re-runs over all mel produced so far (cli/model.py:425-450).  The multi-slot DiT sessions exist in libcvk."""
-        raise NotImplementedError("tts_stream_batch is CosyVoice2-only; stream CosyVoice3 requests with tts(stream=True)")
+        """Streaming synthesis of several CosyVoice3 requests at once: a generator of (i, {'tts_speech': float32 CPU [1, n]}).
+
+        `inputs` are tts() kwargs dicts with tensor `text`.  Each request gets the chunks tts(stream=True) gives it alone: the
+        same chunk schedule and the same chunk lengths.  One LM generation decodes every row (uniforms[:, i] for request i); every
+        poll round then makes at most one multi-slot DiT chunk call, one prefix-recompute and one final flow call, and one
+        causal-vocoder call over every request of the round, streaming and finishing ones together (_stream_vocode).  The
+        instance's token_hop_len is not modified.  Closing the generator early returns every slot to the pool.  Refused when
+        called, before any work: `noise_fns` (ValueError: the causal vocoder draws its noise from its stored sine_waves, from
+        each utterance's start) and a model without a libcvk context (NotImplementedError, see _check_stream_batch)."""
+        self._check_stream_batch(noise_fns)
+        return super().tts_stream_batch(inputs, uniforms)
 
     def tts_bistream_batch(self, inputs, uniforms=None, noise_fns=None):
-        """Not built for CosyVoice3, for the reason tts_stream_batch is not; its text-streaming LM is batched
-        (lm_generate_bistream_batch)."""
-        raise NotImplementedError("tts_bistream_batch is CosyVoice2-only; stream CosyVoice3 requests with tts(stream=True)")
+        """tts_stream_batch for text-streaming CosyVoice3 requests: `inputs` are tts() kwargs dicts whose `text` is a generator of
+        int32 [1,k] chunks, decoded by one lm_generate_bistream_batch (uniforms[k, i] for request i's k-th draw).  Each request
+        gets the chunks tts(text=<generator>, stream=True) gives it alone: the same chunk schedule and the same chunk lengths.
+        The instance's token_hop_len is not modified.  Closing the generator early returns every slot to the pool.  Refuses
+        what tts_stream_batch refuses, when called."""
+        self._check_stream_batch(noise_fns)
+        return super().tts_bistream_batch(inputs, uniforms)
+
+    def _check_stream_batch(self, noise_fns):
+        """The batched streaming path vocodes each round with one cvk_hift3_inference_rows call (a finalize flag per utterance);
+        a model whose context does not provide that call - no context loaded, or one without the entry point - cannot serve it,
+        and says so before any LM or flow work is started rather than failing in the middle of a stream."""
+        if noise_fns is not None:
+            raise ValueError("the causal vocoder draws its noise from its stored sine_waves: noise_fns= is not accepted")
+        if not callable(getattr(getattr(self, "ctx", None), "hift3_inference_rows", None)):
+            raise NotImplementedError("batched CosyVoice3 streaming needs a libcvk context with cvk_hift3_inference_rows (one causal-vocoder "
+                                      "call with a finalize flag per utterance); this model has none")
 
     # ---------------------------------------------------------------- weights
     def load_state_dicts(self, llm_sd, flow_sd, hift_sd, rand_ini=None, sine_noise=None):
@@ -80,6 +107,39 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
         with torch.cuda.stream(self.stream), self.ctx.lock:
             wav, _, src = self.ctx.hift3_inference(mel_tm, lens, finalize=True)
         return wav, src
+
+    def _stream_vocode(self, voc, mels, st, finishing, noise_fns):
+        """the vocoder step of a tts_stream_batch round with token2wav's bookkeeping (cli/model.py:425-450) per request: append the
+        new mel to the request's history, re-run the causal vocoder over the whole history - one hift3_inference_rows call for
+        the round, finalize for the requests in `finishing` - and emit the samples past its speech_offset.  Returns
+        {i: float32 CPU [n]}, copied to the host in one D2H for the round.  noise_fns is always None here (refused by
+        _check_stream_batch)."""
+        outs = {}
+        with torch.cuda.stream(self.stream):
+            hist, lens, fin = [], [], []
+            for i in voc:
+                c = st[i]["cache"]
+                if c is None:
+                    c = st[i]["cache"] = {"mel": mels[i], "speech_offset": 0}
+                else:
+                    c["mel"] = torch.cat([c["mel"], mels[i]], 0)
+                hist.append(c["mel"])
+                lens.append(int(c["mel"].shape[0]))
+                fin.append(i in finishing)
+            with self.ctx.lock:
+                wav, _, _ = self.ctx.hift3_inference_rows(torch.cat(hist, 0), lens, fin)
+            o = 0
+            for i, n, f in zip(voc, lens, fin):
+                n_out = SAMPLES_PER_FRAME * (n if f else n - 8)
+                c = st[i]["cache"]
+                w = wav[o:o + n_out][c["speech_offset"]:]
+                c["speech_offset"] += w.shape[0]
+                outs[i] = w
+                o += n_out
+            flat = torch.cat([outs[i] for i in voc]).cpu()       # one D2H for the round
+        if self.stream is not None:
+            self.stream.synchronize()
+        return self._split_host(voc, outs, flat)
 
     def token2wav(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream=False, finalize=False, speed=1.0):
         """cli/model.py:425-450"""

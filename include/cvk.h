@@ -271,10 +271,17 @@ int cvk_flow_stream_chunk_batch(cvk_ctx* ctx, cvk_flow_stream* fs, int B, const 
  * every utterance).  cvk_hift3_inference = CausalHiFTGenerator.inference (:714-726) for B utterances: mel [sum T, 80] ->
  * wav [sum 480 T]; f0_out [sum T] and source_out [sum 480 T] are optional (NULL).  finalize == 0 is the streaming call
  * (:676-683, :709-710, :722-725): 3 + 4 mel frames of look-ahead are consumed and the last frame's samples dropped, i.e.
- * wav [sum 480 (T-8)], f0_out [sum (T-3)], source_out [sum 480 (T-3)]; every utterance needs T >= 9. */
+ * wav [sum 480 (T-8)], f0_out [sum (T-3)], source_out [sum 480 (T-3)]; every utterance needs T >= 9.
+ * cvk_hift3_inference_rows is the same call with a flag per utterance, finalize_host[B]: utterance b's outputs take, back to back,
+ * 480 T / T / 480 T samples when its flag is set and 480 (T-8) / T-3 / 480 (T-3) when it is 0 (then T >= 9).  One call thus
+ * vocodes streaming chunks and final utterances together, with the kernels of one homogeneous call of the same total size;
+ * each utterance's outputs are bit-identical to a cvk_hift3_inference of it alone with its own flag.  cvk_hift3_inference is
+ * the case where every flag equals `finalize`.  All arguments are checked before any device work. */
 int cvk_hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_noise, long long n, int on_device);
 int cvk_hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens_host, int B, int finalize, float* wav, float* f0_out,
                         float* source_out, void* stream);
+int cvk_hift3_inference_rows(cvk_ctx* ctx, const float* mel, const int* lens_host, const int* finalize_host, int B, float* wav,
+                             float* f0_out, float* source_out, void* stream);
 
 /* ---- CosyVoice3 flow (stage "flow3", cvk_finalize cfg = {DiT depth}) -----------------------------------------------------------
  * cosyvoice/flow/DiT/dit.py:145-176 (DiT.forward, the CFM estimator of CosyVoice3; TensorRT swap point flow_matching.py:126-153):
