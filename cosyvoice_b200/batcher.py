@@ -77,7 +77,10 @@ class TtsBatcher:
     ``submit_pcm`` -> Future of the int16 PCM bytes.  ``submit_stream`` / ``submit_stream_pcm`` -> iterator over the request's
     chunks (what ``tts`` yields for stream=True: float [1, n] tensors, or their int16 PCM bytes).  ``tts_kwargs`` are the keyword
     arguments of ``CosyVoice2Model.tts`` that the batched pipeline consumes: text, prompt_text, llm_prompt_speech_token,
-    flow_prompt_speech_token, prompt_speech_feat, flow_embedding.  ``model`` is a ``B200CosyVoice2Model`` or a
+    flow_prompt_speech_token, prompt_speech_feat, flow_embedding, source_speech_token (voice conversion: no LM) and speed (offline
+    only), each of them optional as in ``tts``, so the requests of every ``inference_*`` call - zero-shot, cross-lingual, instruct,
+    voice conversion - batch together.  ``submit*`` raise ValueError in the caller's thread for a speed <= 0 and for a streaming
+    request whose speed is not 1 (the reference refuses it).  ``model`` is a ``B200CosyVoice2Model`` or a
     ``B200CosyVoice3Model``: both serve offline (``tts_batch``) and streaming (``tts_stream_batch``) batches, and a streaming
     request gets the chunk schedule ``tts(stream=True)`` gives it alone."""
 
@@ -107,6 +110,12 @@ class TtsBatcher:
         return self._enqueue(request, True, ChunkStream())
 
     def _enqueue(self, request, pcm, stream=None):
+        # checked in the caller's thread: a request the model would refuse would otherwise fail every request of its batch
+        speed = float(request.get("speed", 1.0))
+        if not speed > 0:
+            raise ValueError(f"speed must be > 0, got {speed}")
+        if stream is not None and speed != 1.0:
+            raise ValueError("speed change only supports offline requests (submit / submit_pcm), as in the reference")
         sink = stream if stream is not None else Future()
         with self._cv:
             if self._closed:

@@ -58,6 +58,7 @@ void llm_sample_step_op(cvk_ctx* ctx, float* logits, int B, int V, const float* 
 void llm_log_softmax_op(cvk_ctx* ctx, float* x, int rows, int V, cudaStream_t st);
 void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int fmax_hz, float* mel, cudaStream_t st);
 void mel_init(cvk_ctx* ctx);
+void mel_resample(cvk_ctx* ctx, const float* mel, const int* lens, const int* out_lens, int B, float* out, cudaStream_t st);
 void prompt_feat_init(cvk_ctx* ctx);
 
 #define CVK_API_BEGIN            \
@@ -901,6 +902,13 @@ int cvk_mel_spectrogram_ex(cvk_ctx* ctx, const float* wav, const int* lens, int 
   CVK_API_BEGIN
   CVK_REQUIRE(wav && lens && mel && B > 0, "cvk_mel_spectrogram_ex: bad arguments");
   mel_spectrogram(ctx, wav, lens, B, fmax_hz, mel, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_mel_resample(cvk_ctx* ctx, const float* mel, const int* lens, const int* out_lens, int B, float* out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(mel && lens && out_lens && out && B > 0 && B <= 65535, "cvk_mel_resample: bad arguments");
+  CVK_REQUIRE(((uintptr_t)mel & 15) == 0 && ((uintptr_t)out & 15) == 0, "cvk_mel_resample: mel and out must be 16-byte aligned");
+  mel_resample(ctx, mel, lens, out_lens, B, out, (cudaStream_t)stream);
   CVK_API_END
 }
 int cvk_whisper_log_mel(cvk_ctx* ctx, const float* wav, const int* lens, int B, float* out, void* stream) {

@@ -161,3 +161,63 @@ void mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens, int B, int
   CVK_LAUNCH_CHECK();
   unpack_rows(ctx, st, out, sf, 0, mel, N_MEL);
 }
+
+// ================================================================================================ mel time-stretch
+// The `speed` of an offline request (cli/model.py:320-322, CV3 :444-446): F.interpolate(mel[None], size=T', mode="linear"),
+// align_corners=False, no scale factor, on a ragged batch.  The arithmetic is that of torch's CUDA upsample_linear1d for fp32, with
+// every rounding pinned (torch's own build contracts the source index and the blend to the same two FMAs):
+//   scale = (float)T / T',  src = max(fma(j + 0.5, scale, -0.5), 0),  i0 = (int)src,  i1 = i0 + (i0 < T-1),
+//   l1 = src - i0,  out = fma(1 - l1, x[i0], l1 * x[i1]);   T' == T copies the rows.
+namespace {
+struct ResampleSeq {
+  int in_off, in_len, out_off, out_len;
+  float scale;
+};
+constexpr int MEL_VEC = N_MEL / 4;   // float4 per mel row
+
+// one thread per (output row, 4 channels); grid.y = sequence
+__global__ void mel_resample_kernel(const float4* __restrict__ in, const ResampleSeq* __restrict__ seqs, float4* __restrict__ out) {
+  const ResampleSeq s = seqs[blockIdx.y];
+  int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= s.out_len * MEL_VEC) return;
+  int j = idx / MEL_VEC, c = idx - j * MEL_VEC;
+  const float4* x = in + (size_t)s.in_off * MEL_VEC + c;
+  float4 v;
+  if (s.in_len == s.out_len) {
+    v = x[(size_t)j * MEL_VEC];
+  } else {
+    float src = __fmaf_rn(__fadd_rn((float)j, 0.5f), s.scale, -0.5f);
+    src = src >= 0.f ? src : 0.f;
+    int i0 = (int)src;
+    int i1 = i0 + (i0 < s.in_len - 1 ? 1 : 0);
+    float l1 = __fsub_rn(src, (float)i0);
+    float l0 = __fsub_rn(1.f, l1);
+    float4 a = x[(size_t)i0 * MEL_VEC], b = x[(size_t)i1 * MEL_VEC];
+    v.x = __fmaf_rn(l0, a.x, __fmul_rn(l1, b.x));
+    v.y = __fmaf_rn(l0, a.y, __fmul_rn(l1, b.y));
+    v.z = __fmaf_rn(l0, a.z, __fmul_rn(l1, b.z));
+    v.w = __fmaf_rn(l0, a.w, __fmul_rn(l1, b.w));
+  }
+  out[((size_t)s.out_off + j) * MEL_VEC + c] = v;
+}
+}  // namespace
+
+void mel_resample(cvk_ctx* ctx, const float* mel, const int* lens, const int* out_lens, int B, float* out, cudaStream_t st) {
+  std::vector<ResampleSeq> seqs(B);
+  int in_off = 0, out_off = 0, max_out = 0;
+  for (int b = 0; b < B; ++b) {
+    CVK_REQUIRE(lens[b] >= 1 && out_lens[b] >= 1, "mel_resample: every input and output length must be at least 1 (torch refuses 0)");
+    seqs[b] = {in_off, lens[b], out_off, out_lens[b], (float)lens[b] / (float)out_lens[b]};
+    in_off += lens[b];
+    out_off += out_lens[b];
+    if (out_lens[b] > max_out) max_out = out_lens[b];
+  }
+  ctx->arena.reset();
+  ResampleSeq* d_seqs = (ResampleSeq*)ctx->arena.alloc(sizeof(ResampleSeq) * B);
+  CVK_CHECK_CUDA(cudaMemcpyAsync(d_seqs, seqs.data(), sizeof(ResampleSeq) * B, cudaMemcpyHostToDevice, st));
+  const int threads = 256;
+  dim3 grid(ceil_div(max_out * MEL_VEC, threads), B);
+  mel_resample_kernel<<<grid, threads, 0, st>>>((const float4*)mel, d_seqs, (float4*)out);
+  ctx->launches++;
+  CVK_LAUNCH_CHECK();
+}

@@ -100,6 +100,7 @@ SIGNATURES = {
     "cvk_op_log_softmax": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp]),
     "cvk_mel_spectrogram": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_mel_spectrogram_ex": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
+    "cvk_mel_resample": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_whisper_log_mel": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
     "cvk_kaldi_fbank": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
 }
@@ -651,3 +652,17 @@ class Context:
         mel = torch.empty(sum(int(l) // 480 for l in lens), 80, device=self.device)
         self._check(self.lib.cvk_mel_spectrogram_ex(self.h, _ptr(wav), _ints(lens), len(lens), int(fmax or 0), _ptr(mel), _stream()))
         return mel
+
+    def mel_resample(self, mel, lens, out_lens):
+        """the `speed` time-stretch (cvk_mel_resample): mel [sum lens, 80] time-major -> [sum out_lens, 80], utterance b linearly
+        interpolated from lens[b] to out_lens[b] frames exactly as F.interpolate(mode="linear") on the device.  A length of 0 is a
+        ValueError (F.interpolate refuses it too)."""
+        lens, out_lens = [int(v) for v in lens], [int(v) for v in out_lens]
+        if len(lens) != len(out_lens) or not lens or min(lens + out_lens) < 1:
+            raise ValueError(f"mel_resample: one input and one output length >= 1 per utterance, got {lens} -> {out_lens}")
+        mel = _f32(mel, self.device)
+        if mel.shape != (sum(lens), 80):
+            raise ValueError(f"mel_resample: mel must be [sum lens, 80] = [{sum(lens)}, 80], got {list(mel.shape)}")
+        out = torch.empty(sum(out_lens), 80, device=self.device)
+        self._check(self.lib.cvk_mel_resample(self.h, _ptr(mel), _ints(lens), _ints(out_lens), len(lens), _ptr(out), _stream()))
+        return out

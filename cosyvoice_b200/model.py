@@ -45,6 +45,32 @@ class SilentTokenFilter:
         return [t for t in ids if self.keep(t)]
 
 
+# tts()'s defaults for the request keys a frontend may leave out: inference_cross_lingual / inference_instruct2 delete prompt keys,
+# inference_vc builds no text (cli/frontend.py:191-225)
+_REQUEST_DEFAULTS = {k: torch.zeros(1, 0, dtype=torch.int32) for k in ("text", "prompt_text", "llm_prompt_speech_token",
+                                                                        "flow_prompt_speech_token", "source_speech_token")}
+_REQUEST_DEFAULTS.update(prompt_speech_feat=torch.zeros(1, 0, 80), flow_embedding=torch.zeros(0, 192))
+
+
+def request_field(r, key):
+    """request r's tts() argument `key`, or tts()'s default when r does not carry it"""
+    v = r.get(key)
+    return _REQUEST_DEFAULTS[key] if v is None else v
+
+
+def is_vc_request(r):
+    """a voice-conversion request (inference_vc): tts() runs token2wav on its source_speech_token and no LM (cli/model.py:336-339)"""
+    return request_field(r, "source_speech_token").shape[1] > 0
+
+
+def request_speed(r):
+    """request r's `speed` (default 1.0) as a float; ValueError unless it is > 0"""
+    s = float(r.get("speed", 1.0))
+    if not s > 0:
+        raise ValueError(f"speed must be > 0, got {s}")
+    return s
+
+
 class _LmStopped(Exception):
     """raised into a batched LM generation whose consumer has gone away"""
 
@@ -601,29 +627,64 @@ class B200CosyVoice2Model:
     def tts_batch_device(self, inputs, uniforms=None, noise=None):
         """The batched pipeline with the result left on the device: returns (wav_flat, lens, stats) - wav_flat is the vocoder's
         output buffer (float32 [sum n_i], the utterances back to back in input order, empty ones skipped), lens[i] the sample
-        count of input i (0 when the LM produced no token).  Used by tts_batch and by the multi-GPU gather (parallel.gather_flat)."""
+        count of input i (0 when the LM produced no token).  Used by tts_batch and by the multi-GPU gather (parallel.gather_flat).
+
+        Every request kind tts() serves: a missing key takes tts()'s default; a voice-conversion request (non-empty
+        source_speech_token) takes those tokens as its speech tokens, without the LM and without the silent-token rule, like vc_job;
+        the LM runs over the other rows only (request i still draws uniforms[:, i]) and not at all when there are none.  `speed`
+        (default 1) stretches a request's mel after the flow as token2wav does (mel_stretch, one call for the batch, made only when
+        some request has speed != 1); the vocoder, its noise draw, the sample counts and stats["mel_frames"] follow the stretched
+        lengths, stats["flow_frames"] holds the flow's.  A speed <= 0 is a ValueError before any device work."""
+        speeds = [request_speed(r) for r in inputs]
+        vc = [b for b, r in enumerate(inputs) if is_vc_request(r)]
+        lm_rows = [b for b in range(len(inputs)) if b not in vc]
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         with torch.cuda.stream(self.stream):
             ev[0].record()
-        ids = self.lm_generate([i["text"] for i in inputs], [i["prompt_text"] for i in inputs],
-                               [i["llm_prompt_speech_token"] for i in inputs], uniforms)
-        ids = [SilentTokenFilter(self.silent_tokens).filter(x) for x in ids]      # what tts() keeps of each request's ids
+        ids = [None] * len(inputs)
+        for b in vc:
+            ids[b] = request_field(inputs[b], "source_speech_token").flatten().tolist()
+        if lm_rows:
+            if vc and uniforms is None:
+                uniforms = self.uniforms_override
+            if vc and uniforms is not None:
+                uniforms = uniforms[:, lm_rows]
+            lm_ids = self.lm_generate([request_field(inputs[b], "text") for b in lm_rows], [request_field(inputs[b], "prompt_text") for b in lm_rows],
+                                      [request_field(inputs[b], "llm_prompt_speech_token") for b in lm_rows], uniforms)
+            for b, x in zip(lm_rows, lm_ids):
+                ids[b] = SilentTokenFilter(self.silent_tokens).filter(x)      # what tts() keeps of each request's ids
         with torch.cuda.stream(self.stream):
             ev[1].record()
         toks = [torch.tensor(x, dtype=torch.int32).unsqueeze(0) for x in ids]
         keep = [b for b, x in enumerate(ids) if len(x) > 0]
-        mel, lens = self.flow_batch([toks[b] for b in keep], [inputs[b]["flow_prompt_speech_token"] for b in keep],
-                                    [inputs[b]["prompt_speech_feat"] for b in keep], [inputs[b]["flow_embedding"] for b in keep])
+        mel, lens = self.flow_batch([toks[b] for b in keep], [request_field(inputs[b], "flow_prompt_speech_token") for b in keep],
+                                    [request_field(inputs[b], "prompt_speech_feat") for b in keep],
+                                    [request_field(inputs[b], "flow_embedding") for b in keep])
+        flow_lens = list(lens)
         with torch.cuda.stream(self.stream):
             ev[2].record()
+        if any(speeds[b] != 1.0 for b in keep):
+            mel, lens = self.mel_stretch(mel, lens, [speeds[b] for b in keep])
         wav, _ = self.hift_batch(mel, lens, noise=noise)
         with torch.cuda.stream(self.stream):
             ev[3].record()
         n = [0] * len(inputs)
         for b, L in zip(keep, lens):
             n[b] = L * SAMPLES_PER_FRAME
-        stats = {"ev": ev, "tokens": [len(x) for x in ids], "mel_frames": lens}
+        stats = {"ev": ev, "tokens": [len(x) for x in ids], "mel_frames": lens, "flow_frames": flow_lens}
         return wav, n, stats
+
+    def mel_stretch(self, mel, lens, speeds):
+        """token2wav's speed change (cli/model.py:320-322) for a ragged batch in one cvk_mel_resample call: utterance b's lens[b]
+        frames of mel [sum lens, 80] are linearly resampled to int(lens[b] / speeds[b]) frames, the length tts() computes, bit for
+        bit what F.interpolate(mode="linear") gives on the device (speed 1 copies).  Returns (mel, stretched lens); a stretched
+        length of 0 is a ValueError before the call (F.interpolate refuses it too)."""
+        out = [int(T / s) for T, s in zip(lens, speeds)]
+        for T, s, n in zip(lens, speeds, out):
+            if n < 1:
+                raise ValueError(f"speed {s} stretches a mel of {T} frames to 0 frames")
+        with torch.cuda.stream(self.stream), self.ctx.lock:
+            return self.ctx.mel_resample(mel, lens, out), out
 
     def _stage_ms(self, stats):
         ev = stats.pop("ev")
@@ -632,8 +693,9 @@ class B200CosyVoice2Model:
 
     def tts_batch(self, inputs, uniforms=None, noise=None, return_stats=False, to_host=True):
         """inputs: list of dicts with the kwargs of tts() (text, prompt_text, llm_prompt_speech_token,
-        flow_prompt_speech_token, prompt_speech_feat, flow_embedding).  Returns a list of waveforms [1,N]
-        (CPU tensors, or views of one device buffer when to_host=False)."""
+        flow_prompt_speech_token, prompt_speech_feat, flow_embedding, source_speech_token, speed), any of them left out as tts()
+        allows.  Each request gets what tts() gives it alone (tts_batch_device).  Returns a list of waveforms [1,N] (CPU tensors, or
+        views of one device buffer when to_host=False)."""
         wav, n, stats = self.tts_batch_device(inputs, uniforms, noise)
         with torch.cuda.stream(self.stream):
             host = wav.cpu() if to_host else wav          # one D2H for the whole batch
@@ -731,8 +793,7 @@ class B200CosyVoice2Model:
             else:
                 if speed != 1.0:
                     assert cache is None, "speed change only support non-stream inference mode"
-                    m = torch.nn.functional.interpolate(tts_mel.t().unsqueeze(0), size=int(tts_mel.shape[0] / speed), mode="linear")
-                    tts_mel = m[0].t()
+                    tts_mel, _ = self.mel_stretch(tts_mel, [tts_mel.shape[0]], [speed])
                 wav, src = self.hift_batch(tts_mel.contiguous(), [tts_mel.shape[0]], cache_source, cache_lens)
                 if cache is not None:
                     wav = self._fade_in_out(wav, cache["speech"])
@@ -877,14 +938,25 @@ class B200CosyVoice2Model:
         flow_inference for the others, one final flow_inference for requests that are finishing, and one vocoder call over all of
         them.  Request i's k-th vocoder call draws noise_fns[i](n) when given, so its audio does not depend on which other
         requests shared its rounds.  The instance's token_hop_len is not modified.  Closing the generator early (or an
-        exception in it) gives the requests' slots back and ends the LM generation within one block of 8 decode steps."""
-        for r in inputs:
-            if not torch.is_tensor(r.get("text")):
+        exception in it) gives the requests' slots back and ends the LM generation within one block of 8 decode steps.
+
+        A voice-conversion request (non-empty source_speech_token, no text needed) has all its tokens at the first round, as with
+        vc_job: the LM runs over the other rows only (still uniforms[:, i] for request i), not at all when every row is one, and the
+        request finishes as soon as its own tokens are used up.  Refused when called, with ValueError: a speed other than 1 (the
+        reference's streaming path asserts it away, cli/model.py:321) and a text generator (tts_bistream_batch serves those)."""
+        vc = self._check_stream_requests(inputs)
+        for i, r in enumerate(inputs):
+            if i not in vc and not torch.is_tensor(r.get("text")):
                 raise ValueError("tts_stream_batch takes token tensors as text; requests with a text generator go to tts_bistream_batch")
-        empty = torch.zeros(1, 0, dtype=torch.int32)
+        lm_rows = [i for i in range(len(inputs)) if i not in vc]
+        if vc:
+            if uniforms is None:
+                uniforms = self.uniforms_override
+            if uniforms is not None:
+                uniforms = uniforms[:, lm_rows]
 
         def lm_run(emit, lm_state):
-            B = len(inputs)
+            B = len(lm_rows)
             consumed = [0] * B
 
             def progress(out_ids, out_count, live):
@@ -895,26 +967,28 @@ class B200CosyVoice2Model:
                 for b in range(B):
                     if cnt[b] > consumed[b]:
                         for tok in ids[b, consumed[b]:cnt[b]].tolist():
-                            emit(b, tok)
+                            emit(lm_rows[b], tok)
                         consumed[b] = cnt[b]
             with self._lm_stream() as lm_stream:
-                self.lm_generate([r["text"] for r in inputs], [r.get("prompt_text", empty) for r in inputs],
-                                 [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms, steps_per_sync=8,
+                self.lm_generate([inputs[i]["text"] for i in lm_rows], [request_field(inputs[i], "prompt_text") for i in lm_rows],
+                                 [request_field(inputs[i], "llm_prompt_speech_token") for i in lm_rows], uniforms=uniforms, steps_per_sync=8,
                                  on_progress=progress, stream=lm_stream)
-        yield from self._stream_batch(inputs, lm_run, noise_fns)
+        return self._stream_batch(inputs, lm_run if lm_rows else None, noise_fns, vc)
 
     def tts_bistream_batch(self, inputs, uniforms=None, noise_fns=None):
         """tts_stream_batch for text-streaming requests: `inputs` are tts() kwargs dicts whose `text` is a generator of int32 [1,k]
         chunks.  Same contract and rounds as tts_stream_batch - (i, {'tts_speech': ...}) with each request's tts(stream=True) chunk
         schedule, the multi-slot flow session, vocoder caches and cross-fade - with the LM job replaced by one
         lm_generate_bistream_batch over all requests (uniforms[k, i] for request i's k-th draw).  Closing the generator early (or an
-        exception in it) gives the requests' slots back and ends the LM generation at its next decoded id."""
-        empty = torch.zeros(1, 0, dtype=torch.int32)
+        exception in it) gives the requests' slots back and ends the LM generation at its next decoded id.  Refused when called,
+        with ValueError: voice-conversion requests (they have no text to stream) and a speed other than 1."""
+        if self._check_stream_requests(inputs):
+            raise ValueError("tts_bistream_batch serves text-streaming requests; voice-conversion requests go to tts_stream_batch")
 
         def lm_run(emit, lm_state):
             with self._lm_stream() as lm_stream:
-                gen = self.lm_generate_bistream_batch([iter(r["text"]) for r in inputs], [r.get("prompt_text", empty) for r in inputs],
-                                                      [r.get("llm_prompt_speech_token", empty) for r in inputs], uniforms=uniforms,
+                gen = self.lm_generate_bistream_batch([iter(r["text"]) for r in inputs], [request_field(r, "prompt_text") for r in inputs],
+                                                      [request_field(r, "llm_prompt_speech_token") for r in inputs], uniforms=uniforms,
                                                       stream=lm_stream)
                 try:
                     for b, tok in gen:
@@ -923,17 +997,28 @@ class B200CosyVoice2Model:
                         emit(b, tok)
                 finally:
                     gen.close()
-        yield from self._stream_batch(inputs, lm_run, noise_fns)
+        return self._stream_batch(inputs, lm_run, noise_fns)
 
-    def _stream_batch(self, inputs, lm_run, noise_fns):
+    @staticmethod
+    def _check_stream_requests(inputs):
+        """the voice-conversion rows of a streaming batch; ValueError for a speed other than 1"""
+        for r in inputs:
+            if request_speed(r) != 1.0:
+                raise ValueError("speed change only supports non-streaming inference (cli/model.py:321); use tts_batch")
+        return [i for i, r in enumerate(inputs) if is_vc_request(r)]
+
+    def _stream_batch(self, inputs, lm_run, noise_fns, vc=()):
         """the poll loop of tts_stream_batch / tts_bistream_batch.  lm_run(emit, lm_state) runs the LM job on a side thread and calls
-        emit(i, id) for every id request i decodes; it ends early once lm_state["stop"] is set."""
+        emit(i, id) for every id request i decodes; it ends early once lm_state["stop"] is set.  Rows in `vc` are voice-conversion
+        requests: their source tokens are all there from the start and they end on their own; lm_run is None when every row is one."""
         B = len(inputs)
-        empty = torch.zeros(1, 0, dtype=torch.int32)
-        req = [dict(ptok=r.get("flow_prompt_speech_token", empty), pfeat=r.get("prompt_speech_feat", torch.zeros(1, 0, 80)),
-                    emb=r.get("flow_embedding", torch.zeros(0, 192))) for r in inputs]
+        req = [dict(ptok=request_field(r, "flow_prompt_speech_token"), pfeat=request_field(r, "prompt_speech_feat"),
+                    emb=request_field(r, "flow_embedding")) for r in inputs]
         toks = [[] for _ in range(B)]
-        lm_state = {"end": False, "err": None, "stop": False}
+        own_end = [False] * B
+        for i in vc:
+            toks[i], own_end[i] = request_field(inputs[i], "source_speech_token").flatten().tolist(), True
+        lm_state = {"end": lm_run is None, "err": None, "stop": False}
         silent = [SilentTokenFilter(self.silent_tokens) for _ in range(B)]
 
         def emit(b, tok):
@@ -956,8 +1041,10 @@ class B200CosyVoice2Model:
             P = int(r["ptok"].shape[1])
             st.append(dict(P=P, pad=int(np.ceil(P / hop0) * hop0 - P), hop=hop0, offset=0, slot=None, eligible=True, cache=None,
                            done=False))
-        p = threading.Thread(target=llm_job, name="cvk-stream-batch-lm", daemon=True)
-        p.start()
+        p = None
+        if lm_run is not None:
+            p = threading.Thread(target=llm_job, name="cvk-stream-batch-lm", daemon=True)
+            p.start()
         try:
             while not all(s["done"] for s in st):
                 end = lm_state["end"]                    # read first: once the LM has ended, the token lists are complete
@@ -970,14 +1057,15 @@ class B200CosyVoice2Model:
                     this_hop = s["hop"] + s["pad"] if s["offset"] == 0 else s["hop"]
                     if len(toks[i]) - s["offset"] >= this_hop + PRE_LOOKAHEAD:
                         ready.append((i, this_hop))
-                    elif end:
+                    elif end or own_end[i]:
                         finishing.append(i)
                 if not ready and not finishing:
                     time.sleep(0.005)
                     continue
                 for i, out in self._stream_round(req, st, toks, ready, finishing, noise_fns):
                     yield i, out
-            p.join()
+            if p is not None:
+                p.join()
         finally:
             lm_state["stop"] = True                      # closed or failed early: the LM stops within one block of 8 steps
             for s in st:

@@ -157,8 +157,7 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
                 cache = self.hift_cache_dict[uuid] = {"mel": tts_mel, "speech_offset": 0}
             if speed != 1.0:
                 assert token_offset == 0 and finalize is True, "speed change only support non-stream inference mode"
-                m = torch.nn.functional.interpolate(tts_mel.t().unsqueeze(0), size=int(tts_mel.shape[0] / speed), mode="linear")
-                tts_mel = m[0].t()
+                tts_mel, _ = self.mel_stretch(tts_mel, [tts_mel.shape[0]], [speed])
             with self.ctx.lock:
                 wav, _, _ = self.ctx.hift3_inference(tts_mel.contiguous(), [tts_mel.shape[0]], finalize=finalize)
             wav = wav[cache["speech_offset"]:]

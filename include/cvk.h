@@ -381,6 +381,14 @@ int cvk_mel_spectrogram(cvk_ctx* ctx, const float* wav, const int* lens_host, in
 /* same with the filterbank's upper edge as a parameter: fmax_hz = 8000 (CosyVoice2) or 0 / 12000 = sr/2 (`fmax: null` of
  * examples/libritts/cosyvoice3/conf/cosyvoice3.yaml:140-147) */
 int cvk_mel_spectrogram_ex(cvk_ctx* ctx, const float* wav, const int* lens_host, int B, int fmax_hz, float* mel, void* stream);
+/* The `speed` time-stretch of an offline request: replaces the F.interpolate(tts_mel, size=int(T / speed), mode="linear") of
+ * cosyvoice/cli/model.py:320-322 (CosyVoice2Model.token2wav) and :444-446 (CosyVoice3Model.token2wav) for B utterances in one launch.
+ * mel [sum lens_host[b], 80] -> out [sum out_lens_host[b], 80], both time-major ragged fp32, 16-byte aligned, not overlapping.
+ * Output row j of utterance b is torch's linear interpolation (align_corners=False, no scale factor) bit for bit: scale =
+ * (float)T / T', src = max((j + 0.5) scale - 0.5, 0), i0 = (int)src, i1 = min(i0 + 1, T - 1), out = (1 - l) x[i0] + l x[i1] with
+ * l = src - i0 (one fused multiply-add each for src and the blend, as torch's kernel rounds them); T' == T copies the rows.  Every
+ * length must be >= 1 (torch refuses a size of 0); a refusal returns CVK_ERR_INVALID before any device work.  Uses the workspace. */
+int cvk_mel_resample(cvk_ctx* ctx, const float* mel, const int* lens_host, const int* out_lens_host, int B, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------- prompt-side features (16 kHz)
  * SURVEY 8(f) rank 2: the two feature extractors the reference frontend runs on the CPU before its ONNX sessions.
