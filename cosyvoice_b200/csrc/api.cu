@@ -28,7 +28,7 @@ void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int*
                      float* source_out, cudaStream_t st);
 void dit_build(cvk_ctx* ctx, const int* cfg, int ncfg);
 void dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
-                   int B, int streaming, float* out, cudaStream_t st);
+                   int B, int streaming, float* out, cudaStream_t st, int n_blocks = 0, float* hidden = nullptr);
 void flow3_inference(cvk_ctx* ctx, const int32_t* tokens, const int* token_lens, const float* prompt_feat, const int* prompt_feat_lens,
                      const float* embedding, int B, int n_timesteps, int streaming, int finalize, float* mel, cudaStream_t st);
 void llm_prefill(cvk_ctx* ctx, cvk_lm_session* s, const int32_t* text, const int* text_lens, const int32_t* speech,
@@ -776,6 +776,13 @@ int cvk_dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float
   CVK_API_BEGIN
   CVK_REQUIRE(x && mu && t && spks && cond && lens_host && out && B > 0, "cvk_dit_estimator: bad arguments");
   dit_estimator(ctx, x, mu, t, spks, cond, lens_host, B, streaming, out, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_dit_hidden(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
+                   const int* lens_host, int B, int streaming, int n_blocks, float* hidden, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(x && mu && t && spks && cond && lens_host && hidden && B > 0, "cvk_dit_hidden: bad arguments");
+  dit_estimator(ctx, x, mu, t, spks, cond, lens_host, B, streaming, nullptr, (cudaStream_t)stream, n_blocks, hidden);
   CVK_API_END
 }
 int cvk_flow3_inference(cvk_ctx* ctx, const int32_t* tokens, const int* token_lens_host, const float* prompt_feat,

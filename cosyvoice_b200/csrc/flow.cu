@@ -849,8 +849,10 @@ void estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& 
 }
 
 // mu, cond, x: fp32 [R1,80] (ld 80) in geometry s1; spks [B,80].  Runs n Euler steps in place on x.
+// hidden != nullptr (the test-only read-out cvk_dit_hidden): stop after the first n_blocks blocks and write the fp32 residual stream
+// [sum T, 1024] there instead of running norm_out / proj_out; `out` is then not written
 void dit_estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& in0, const float* t_dev, int streaming, const Mat& out,
-                           EstInc* inc);
+                           EstInc* inc, int n_blocks = 0, float* hidden = nullptr);
 
 // `dit`: 0 = CosyVoice2 causal U-Net estimator, 1 = CosyVoice3 DiT (32 gap rows: its causal position convolution looks 30 rows back)
 void cfm_solve_packed(cvk_ctx* ctx, cudaStream_t st, const Seqs& s1, const int* lens, const Mat& mu, const Mat& cond, const float* spks,
@@ -1081,7 +1083,7 @@ void gate_add(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat& o, const S
 
 // in0: act [R,320] packed [x | mu | spks | cond]; t_dev [B]; out fp32 [R,80]
 void dit_estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& in0, const float* t_dev, int streaming, const Mat& out,
-                           EstInc* inc) {
+                           EstInc* inc, int n_blocks, float* hidden) {
   DitModel* m = ctx->dit;
   CVK_REQUIRE(m && m->tok_emb, "flow3 stage not finalised");
   const int adt = ctx->act_dtype;
@@ -1146,7 +1148,8 @@ void dit_estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const M
     conv_gemm(ctx, st, c1.slice(g * 64, 64), m->pos2[g], e);
   }
   const int bx = s.max_len < 1024 ? s.max_len : 1024;
-  for (int i = 0; i < m->depth; ++i) {
+  const int n_run = hidden ? n_blocks : m->depth;
+  for (int i = 0; i < n_run; ++i) {
     const DitBlockW& w = m->blocks[i];
     const float* mb = mod.f32() + (size_t)i * 6 * DIT_D;   // [shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp]
     ln_mod(ctx, st, x, s, mb + DIT_D, mb, mod_ld, xn);
@@ -1188,6 +1191,11 @@ void dit_estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const M
       conv_gemm(ctx, st, ff, w.ff2, e);
     }
     gate_add(ctx, st, x, o, s, mb + 5 * DIT_D, mod_ld);
+  }
+  if (hidden) {
+    unpack_rows(ctx, st, x, s, 0, hidden, DIT_D);
+    ctx->arena.off = mark;
+    return;
   }
   const float* mf = mod.f32() + (size_t)m->depth * 6 * DIT_D;   // norm_out: [scale | shift] (modules.py:261)
   ln_mod(ctx, st, x, s, mf, mf + DIT_D, mod_ld, xn);
@@ -1550,10 +1558,12 @@ void dit_build(cvk_ctx* ctx, const int* cfg, int ncfg) {
   ctx->dit = m;
 }
 
-// dit.py:145-176 on dense inputs (same argument layout as cvk_cfm_estimator)
+// dit.py:145-176 on dense inputs (same argument layout as cvk_cfm_estimator).  hidden != nullptr: cvk_dit_hidden, the residual
+// stream after n_blocks blocks to hidden [sum T, 1024] instead of the estimator output
 void dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
-                   int B, int streaming, float* out, cudaStream_t st) {
+                   int B, int streaming, float* out, cudaStream_t st, int n_blocks, float* hidden) {
   CVK_REQUIRE(ctx->dit && ctx->dit->tok_emb, "flow3 stage not finalised");
+  CVK_REQUIRE(!hidden || (n_blocks >= 0 && n_blocks <= ctx->dit->depth), "cvk_dit_hidden: n_blocks outside [0, depth]");
   ctx->arena.reset();
   const int adt = ctx->act_dtype;
   Seqs s = make_seqs(ctx, lens, B, 32, 1, 0, st);
@@ -1566,8 +1576,8 @@ void dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   Mat v = arena_mat(ctx, DT_F32, s.R, N_MEL, N_MEL);
-  dit_estimator_forward(ctx, st, s, in0, t, streaming, v, nullptr);
-  unpack_rows(ctx, st, v, s, 0, out, N_MEL);
+  dit_estimator_forward(ctx, st, s, in0, t, streaming, v, nullptr, n_blocks, hidden);
+  if (!hidden) unpack_rows(ctx, st, v, s, 0, out, N_MEL);
 }
 
 // flow.py:369-414 CausalMaskedDiffWithDiT.inference, batched over ragged utterances

@@ -81,6 +81,7 @@ SIGNATURES = {
     "cvk_hift3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]),
     "cvk_hift3_inference_rows": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp, _vp, _vp, _vp]),
     "cvk_dit_estimator": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
+    "cvk_dit_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_flow3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, _vp, _c_int_p, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_lm_session_create": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp)]),
     "cvk_lm_session_destroy": (None, [_vp, _vp]),
@@ -447,6 +448,15 @@ class Context:
         out = torch.empty_like(x)
         self._check(self.lib.cvk_dit_estimator(self.h, _ptr(x), _ptr(mu), _ptr(t), _ptr(spks), _ptr(cond), _ints(lens), len(lens),
                                                int(streaming), _ptr(out), _stream()))
+        return out
+
+    def dit_hidden(self, x, mu, t, spks, cond, lens, n_blocks, streaming=False):
+        """parity tests: the DiT residual stream [sum T, 1024] after the input embedding and the first n_blocks blocks (0 <= n_blocks
+        <= depth); same inputs as dit_estimator"""
+        x, mu, t, spks, cond = (_f32(a, self.device) for a in (x, mu, t, spks, cond))
+        out = torch.empty(x.shape[0], 1024, device=self.device)
+        self._check(self.lib.cvk_dit_hidden(self.h, _ptr(x), _ptr(mu), _ptr(t), _ptr(spks), _ptr(cond), _ints(lens), len(lens),
+                                            int(streaming), int(n_blocks), _ptr(out), _stream()))
         return out
 
     def flow3_inference(self, tokens, token_lens, prompt_feat, prompt_feat_lens, embedding, n_timesteps=10, streaming=False,

@@ -289,6 +289,11 @@ int cvk_hift3_inference_rows(cvk_ctx* ctx, const float* mel, const int* lens_hos
  * streaming != 0 selects the static 50-frame block-causal mask (dit.py:165-166). */
 int cvk_dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
                       const int* lens_host, int B, int streaming, float* out, void* stream);
+/* parity tests: the arguments of cvk_dit_estimator, but the call stops after the input embedding and the first n_blocks DiT blocks
+ * (0 <= n_blocks <= depth) and writes the fp32 residual stream x [sum T, 1024] (before norm_out) to `hidden` instead of the
+ * estimator output.  An n_blocks outside [0, depth] is refused before any device work. */
+int cvk_dit_hidden(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
+                   const int* lens_host, int B, int streaming, int n_blocks, float* hidden, void* stream);
 /* cosyvoice/flow/flow.py:369-414 CausalMaskedDiffWithDiT.inference for B utterances: tokens = prompt tokens followed by the new
  * tokens of every utterance (token_lens_host), prompt_feat [sum Tp, 80], embedding [B, 192]; finalize == 0: the last 3 tokens of
  * every utterance are look-ahead context (flow.py:389-392).  mel receives 2 * (tokens - context) - Tp frames per utterance.

@@ -243,3 +243,235 @@ def relpos_attention(q, k, v, pos, center, bias_u, bias_v, lens, H, chunk, scale
         outs.append((torch.softmax(s, -1) @ vv).transpose(0, 1).reshape(L, H * HD))
         o += L
     return torch.cat(outs, 0)
+
+
+# ------------------------------------------------------------------------------------------------ CosyVoice3 DiT estimator
+# The DiT of oracle/dit.py (dit.py:145-176 of the reference) restated on the packed time-major rows the kernels use, in fp64, one piece
+# at a time: the time embedding and every AdaLN modulation vector (dit_modulation), the input embedding (dit_input_embedding), one
+# block (dit_block) and norm_out + proj_out (dit_output).  rounding=True emulates the bf16 path: the values it stores as bf16 and
+# reads again are rounded at the same points (DIT_ROUNDING), and the tensor-core weights are taken as bf16.  `mutate` applies one of
+# DIT_MUTATIONS, the defects the sensitivity test of test_kernel_refs_cpu.py injects.
+from oracle import dit as odit  # noqa: E402
+
+DIT_D, DIT_FF, DIT_CK = odit.DIM, odit.FF, odit.CONV_K
+DIT_ROUNDING = ("x_conv", "mish1", "xn", "qkv", "rot", "att", "ff")
+DIT_MUTATIONS = ("rope_half", "rope_all_heads", "kpos_shift", "adaln_swap", "mod_neighbour", "chunk48", "chunk_edge", "silu_pos",
+                 "time_div", "gelu_erf", "ln_eps")
+
+
+def dit_weights(sd, depth, p="decoder.estimator."):
+    """the estimator's weights in fp64, grouped the way the kernels hold them (qkv concatenated, every modulation linear in one matrix)"""
+    g = lambda k: sd[p + k].double()
+    blocks = []
+    for i in range(depth):
+        b = f"transformer_blocks.{i}."
+        blocks.append(dict(qkv_w=torch.cat([g(b + f"attn.to_{n}.weight") for n in "qkv"]),
+                           qkv_b=torch.cat([g(b + f"attn.to_{n}.bias") for n in "qkv"]),
+                           out_w=g(b + "attn.to_out.0.weight"), out_b=g(b + "attn.to_out.0.bias"),
+                           ff1_w=g(b + "ff.ff.0.0.weight"), ff1_b=g(b + "ff.ff.0.0.bias"),
+                           ff2_w=g(b + "ff.ff.2.weight"), ff2_b=g(b + "ff.ff.2.bias")))
+    mods = [f"transformer_blocks.{i}.attn_norm.linear." for i in range(depth)] + ["norm_out.linear."]
+    return dict(depth=depth, blocks=blocks,
+                t1_w=g("time_embed.time_mlp.0.weight"), t1_b=g("time_embed.time_mlp.0.bias"),
+                t2_w=g("time_embed.time_mlp.2.weight"), t2_b=g("time_embed.time_mlp.2.bias"),
+                mod_w=torch.cat([g(m + "weight") for m in mods]), mod_b=torch.cat([g(m + "bias") for m in mods]),
+                in_w=g("input_embed.proj.weight"), in_b=g("input_embed.proj.bias"),
+                c1_w=g("input_embed.conv_pos_embed.conv1.0.weight"), c1_b=g("input_embed.conv_pos_embed.conv1.0.bias"),
+                c2_w=g("input_embed.conv_pos_embed.conv2.0.weight"), c2_b=g("input_embed.conv_pos_embed.conv2.0.bias"),
+                proj_w=g("proj_out.weight"), proj_b=g("proj_out.bias"))
+
+
+def _rd(rounding):
+    return bf16 if rounding else (lambda t: t)
+
+
+def _seq_ids(lens):
+    return torch.repeat_interleave(torch.arange(len(lens)), torch.tensor(lens))
+
+
+def _silu(x):
+    return x / (1.0 + torch.exp(-x))
+
+
+def dit_modulation(W, t, mutate=None):
+    """TimestepEmbedding (modules.py:71-84, 606-616) and every AdaLN linear on SiLU of it, in fp64: t [B] -> dict(a (the sinusoid
+    angles), sc, te1, te, ste, mod [B, depth*6144 + 2048]).  The fp32 CUDA-core GEMMs of the kernels have no bf16 rounding point."""
+    half = 128
+    div = half if mutate == "time_div" else half - 1
+    e = torch.exp(torch.arange(half, dtype=torch.float64) * -(math.log(10000.0) / div))
+    a = 1000.0 * t.double()[:, None] * e[None]
+    sc = torch.cat([a.sin(), a.cos()], -1)
+    te1 = _silu(sc @ W["t1_w"].t() + W["t1_b"])
+    te = te1 @ W["t2_w"].t() + W["t2_b"]
+    ste = _silu(te)
+    return dict(a=a, sc=sc, te1=te1, te=te, ste=ste, mod=ste @ W["mod_w"].t() + W["mod_b"])
+
+
+def _mish(x):
+    return act("mish", x)
+
+
+def _causal_grouped_conv(x, w, b, lens):
+    """CausalConvPositionEmbedding's Conv1d (k31, 16 groups, 30 zero rows in front of every sequence) on packed rows [sum T, 1024]"""
+    outs, o = [], 0
+    for L in lens:
+        y = torch.nn.functional.conv1d(torch.nn.functional.pad(x[o:o + L].t()[None], (DIT_CK - 1, 0)), w, b, groups=odit.CONV_GROUPS)
+        outs.append(y[0].t())
+        o += L
+    return torch.cat(outs, 0)
+
+
+def dit_input_embedding(W, x, mu, cond, spks, lens, rounding=False, mutate=None):
+    """InputEmbedding (modules.py:87-112, 115-145): proj([x | cond | mu | spks]) -> two causal grouped k31 convolutions with Mish ->
+    + proj.  x, mu, cond [sum T, 80], spks [B, 80] (one row per sequence).  Returns dict(h (the projection), xa (conv1's input),
+    c1 (conv1 after Mish), acc2 (conv2 before Mish), x0 = the residual stream entering block 0)."""
+    rd = _rd(rounding)
+    wt = rd if rounding else (lambda t: t)
+    inp = torch.cat([x.double(), cond.double(), mu.double(), spks.double()[_seq_ids(lens)]], -1)
+    h = rd(inp) @ wt(W["in_w"]).t() + W["in_b"]                         # the bf16 path packs its input as bf16
+    act_pos = _silu if mutate == "silu_pos" else _mish
+    xa = rd(h)
+    acc1 = _causal_grouped_conv(xa, wt(W["c1_w"]), W["c1_b"], lens)
+    c1 = rd(act_pos(acc1))
+    acc2 = _causal_grouped_conv(c1, wt(W["c2_w"]), W["c2_b"], lens)
+    return dict(inp=rd(inp), h=h, xa=xa, acc1=acc1, c1=c1, acc2=acc2, x0=act_pos(acc2) + h)
+
+
+def _layer_norm(x, eps=1e-6):
+    mu = x.mean(-1, keepdim=True)
+    v = x - mu
+    return v * torch.rsqrt(v.pow(2).mean(-1, keepdim=True) + eps)
+
+
+def rotary_angles(T, q_off=0):
+    """the reference's fp32 rotary angles (oracle.dit.rotary_freqs: x_transformers' table, position * 10000^(-2i/64) in fp32) of
+    positions q_off .. q_off + T - 1, in fp64: [T, 64], each angle in two adjacent channels"""
+    return odit.rotary_freqs(T + q_off)[0, q_off:].double()
+
+
+def _rotate(t, ang, half_split=False):
+    """x_transformers' rotation of adjacent pairs (2i, 2i+1) -> (a cos - b sin, b cos + a sin) on the last dim (64); half_split: the
+    rotate-half pairing (i, i + 32) instead"""
+    if half_split:
+        a, b = t[..., :32], t[..., 32:]
+        c, s = ang[..., ::2].cos(), ang[..., ::2].sin()
+        return torch.cat([a * c - b * s, b * c + a * s], -1)
+    a2 = t.reshape(*t.shape[:-1], 32, 2)
+    rot = torch.stack((-a2[..., 1], a2[..., 0]), -1).flatten(-2)
+    return t * ang.cos() + rot * ang.sin()
+
+
+def _dit_visible(T, chunk, edge=0):
+    """[T, T] key j visible from query i: all keys, or the static block-causal mask of `chunk` frames (add_optional_chunk_mask),
+    with the chunk's right edge moved by `edge`"""
+    if chunk <= 0:
+        return torch.ones(T, T, dtype=torch.bool)
+    i = torch.arange(T)[:, None]
+    return torch.arange(T)[None, :] < (i // chunk + 1) * chunk + edge
+
+
+def dit_block(W, i, x, mod, lens, chunk, rounding=False, mutate=None):
+    """DiTBlock i (modules.py:500-533) on packed rows x [sum T, 1024] (fp64), mod = dit_modulation(...)["mod"] [B, ...], chunk 0
+    (offline) or 50 (streaming).  Returns every stage: n1 (the normalised rows), xn, qkv, qkv_rot (head 0 of q and k rotated), p
+    (the attention weights per sequence), att, o, x_mid, n2, xn2, hpre, h, f, x_out (all fp64, rounded where DIT_ROUNDING says)."""
+    rd = _rd(rounding)
+    wt = bf16 if rounding else (lambda t: t)
+    w = W["blocks"][i]
+    x = x.double()
+    B = len(lens)
+    seq = _seq_ids(lens)
+    m = mod[:, i * 6 * DIT_D:(i + 1) * 6 * DIT_D]
+    if mutate == "mod_neighbour":
+        m = m[(torch.arange(B) + 1) % B]
+    sh1, sc1, g1, sh2, sc2, g2 = (t[seq] for t in m.split(DIT_D, -1))
+    if mutate == "adaln_swap":
+        sh1, sc1, sh2, sc2 = sc1, sh1, sc2, sh2
+    eps = 1e-5 if mutate == "ln_eps" else 1e-6
+    n1 = _layer_norm(x, eps)
+    xn64 = n1 * (1 + sc1) + sh1
+    xn = rd(xn64)
+    qkv64 = xn @ wt(w["qkv_w"]).t() + w["qkv_b"]
+    qkv = rd(qkv64)
+    heads = 16 if mutate == "rope_all_heads" else 1
+    rot64 = qkv.clone()
+    outs, ps, o0 = [], [], 0
+    for L in lens:
+        ang = rotary_angles(L)
+        for which in (0, 1):
+            kang = rotary_angles(L, 1) if (which == 1 and mutate == "kpos_shift") else ang
+            cols = slice(which * DIT_D, which * DIT_D + 64 * heads)
+            blk = qkv[o0:o0 + L, cols].reshape(L, heads, 64)
+            rot64[o0:o0 + L, cols] = _rotate(blk, kang[:, None], mutate == "rope_half").reshape(L, 64 * heads)
+        o0 += L
+    qkv_rot = rd(rot64)
+    o0 = 0
+    ch = 48 if mutate == "chunk48" else chunk
+    for L in lens:
+        q, k, v = (qkv_rot[o0:o0 + L, n * DIT_D:(n + 1) * DIT_D].reshape(L, 16, 64).transpose(0, 1) for n in range(3))
+        s = (q @ k.transpose(1, 2)) * 0.125
+        s = s.masked_fill(~_dit_visible(L, ch, 1 if mutate == "chunk_edge" else 0)[None], float("-inf"))
+        p = torch.softmax(s, -1)
+        ps.append(p)
+        outs.append((p @ v).transpose(0, 1).reshape(L, DIT_D))
+        o0 += L
+    att64 = torch.cat(outs, 0)
+    att = rd(att64)
+    o = att @ wt(w["out_w"]).t() + w["out_b"]
+    x_mid = x + g1 * o
+    n2 = _layer_norm(x_mid, eps)
+    xn2_64 = n2 * (1 + sc2) + sh2
+    xn2 = rd(xn2_64)
+    hpre = xn2 @ wt(w["ff1_w"]).t() + w["ff1_b"]
+    h64 = act("gelu" if mutate == "gelu_erf" else "gelu_tanh", hpre)
+    h = rd(h64)
+    f = h @ wt(w["ff2_w"]).t() + w["ff2_b"]
+    return dict(x=x, n1=n1, xn64=xn64, xn=xn, qkv64=qkv64, qkv=qkv, rot64=rot64, qkv_rot=qkv_rot, p=ps, att64=att64, att=att, o=o,
+                x_mid=x_mid, n2=n2, xn2_64=xn2_64, xn2=xn2, hpre=hpre, h64=h64, h=h, f=f, x_out=x_mid + g2 * f,
+                sc1=sc1, sh1=sh1, g1=g1, sc2=sc2, sh2=sh2, g2=g2)
+
+
+def dit_output(W, x, mod, lens, rounding=False):
+    """AdaLayerNormZero_Final + proj_out (modules.py:251-264, dit.py:174-175): x [sum T, 1024] -> [sum T, 80]"""
+    depth = W["depth"]
+    sc, sh = (t[_seq_ids(lens)] for t in mod[:, depth * 6 * DIT_D:].split(DIT_D, -1))
+    xn = _rd(rounding)(_layer_norm(x.double()) * (1 + sc) + sh)
+    return xn @ (bf16(W["proj_w"]) if rounding else W["proj_w"]).t() + W["proj_b"]
+
+
+def dit_estimator(W, x, mu, cond, spks, t, lens, streaming, rounding=False, n_blocks=None):
+    """the composed estimator on packed rows: returns (hidden after n_blocks blocks (all by default), output [sum T, 80])"""
+    mod = dit_modulation(W, t)["mod"]
+    h = dit_input_embedding(W, x, mu, cond, spks, lens, rounding)["x0"]
+    for i in range(W["depth"] if n_blocks is None else n_blocks):
+        h = dit_block(W, i, h, mod, lens, 50 if streaming else 0, rounding)["x_out"]
+    return h, dit_output(W, h, mod, lens, rounding)
+
+
+def dit_test_state_dict(depth, seed):
+    """CosyVoice3 flow weights for the DiT checks (named as oracle.dit.flow_param_shapes names them): fan-in-scaled matrices,
+    bf16-representable where the bf16 path streams them as bf16 (so both references see the kernels' weights), and AdaLN
+    modulation vectors of O(1) - gates ~ 1, unlike oracle.dit.SYNTH_GAINS, which keep ten Euler steps tame with gates ~ 0.1 and so
+    shrink each block's contribution under the residual."""
+    from oracle import weights as oweights
+    sd = oweights.synth_state_dict(odit.flow_param_shapes(depth), seed, {"attn_norm.linear.weight": 4.0, "norm_out.linear.weight": 4.0})
+    est = "decoder.estimator."
+    g = torch.Generator().manual_seed(seed)
+    for k in ("input_embed.proj.weight", "time_embed.time_mlp.0.weight", "time_embed.time_mlp.2.weight"):
+        w = sd[est + k]                                     # matrices, not embedding tables: fan-in scaled
+        sd[est + k] = torch.randn(w.shape, generator=g) * w.shape[1] ** -0.5
+    for k, v in sd.items():
+        if v.dim() >= 2 and k.startswith(est) and "time_embed" not in k and ".linear." not in k:
+            sd[k] = bf16(v)
+    return sd
+
+
+# bounds of test_dit_blocks_gpu.py: largest |kernel - reference| of a stage over the rms of that row's contribution (embedding: x0;
+# block: x_out - x).  Largest ratios measured on an H100 80GB HBM3 (700 W) over every layout, both masks, in one run: fp32 embedding
+# 7.6e-6, block 1.1e-4 (the fp32 sinusoid of t, angles up to 950 rad, carries ~6e-5 into the modulation vectors); bf16 (against the
+# bf16-emulating reference) embedding 2.4e-3, block 2.4e-2.  Each bound is about twice that.
+DIT_TOL = {"fp32": dict(embed=2e-5, block=2.5e-4), "bf16": dict(embed=5e-3, block=0.05)}
+# 22-block stack: largest error over the mean row rms of the reference, (hidden, estimator output), per reference.  Measured, same run:
+# fp32 vs exact 1.1e-4 / 8.3e-5, fp32 vs bf16-emulating 1.3e-2 / 1.1e-2, bf16 vs exact 1.2e-2 / 1.2e-2, bf16 vs bf16-emulating
+# 1.3e-2 / 1.2e-2.  Bounds about twice that.
+DIT_STACK_TOL = {"fp32": {"exact": (2.5e-4, 2e-4), "bf16-emulating": (0.03, 0.025)},
+                 "bf16": {"exact": (0.025, 0.025), "bf16-emulating": (0.03, 0.025)}}

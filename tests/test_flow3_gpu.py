@@ -2,7 +2,7 @@
 the committed outputs of the reference modules (tests/golden/dit_*.npz, made by oracle/make_golden.py::gen_dit).
 
 fp32 mode: the reference's export tolerance for an estimator (cosyvoice/bin/export_onnx.py:99-110, rtol 1e-2 / atol 1e-4);
-bf16 mode: measured bounds stated next to each assert."""
+bf16 mode: bounds of twice the largest error measured on an H100, stated and printed next to each assert."""
 import numpy as np
 import pytest
 import torch
@@ -44,7 +44,10 @@ def test_dit_estimator_golden(precision, tag, depth, golden):
         if precision == "fp32":
             np.testing.assert_allclose(out.cpu().numpy(), ref.numpy(), rtol=1e-2, atol=1e-4)
         else:
-            assert maxdiff(out, ref) < 0.05, maxdiff(out, ref)          # |out| ~ 0.7, bf16 operands through 2-22 blocks
+            # |out| ~ 0.7; largest |d| measured on an H100 80GB HBM3 (700 W): 8.0e-3 (depth 2, streaming), 4.4e-3 (depth 22); twice
+            d = maxdiff(out, ref)
+            print(f"[estimator {precision} {tag} streaming={streaming}] max |d| {d:.4g} (bound 0.016)")
+            assert d < 0.016, d
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
@@ -59,7 +62,10 @@ def test_flow3_inference_golden(precision, golden):
         ref = torch.from_numpy(g["mel_" + name])[0].t()
         assert lens == [ref.shape[0]]
         d = maxdiff(mel, ref)
-        assert d < (2e-3 if precision == "fp32" else 0.15), (name, d)    # |mel| ~ 3.7 after ten Euler steps
+        # |mel| ~ 3.7 after ten Euler steps; bf16: largest |d| measured on an H100 80GB HBM3 (700 W) 1.27e-2 (stream_final), twice
+        bound = 2e-3 if precision == "fp32" else 0.025
+        print(f"[flow3_inference {precision} {name}] max |d| {d:.4g} (bound {bound})")
+        assert d < bound, (name, d)
 
 
 def test_dit_ragged_batch_equals_single(golden):
@@ -77,7 +83,7 @@ def test_dit_ragged_batch_equals_single(golden):
     o = 0
     for b, T in enumerate(lens):
         single = c.dit_estimator(xs[b], mus[b], t[b:b + 1], spks[b:b + 1], conds[b], [T], streaming=True)
-        assert maxdiff(out[o:o + T], single) < 1e-5
+        assert torch.equal(out[o:o + T], single), (b, T, maxdiff(out[o:o + T], single))
         o += T
 
 

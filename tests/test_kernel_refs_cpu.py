@@ -253,3 +253,145 @@ def test_relpos_ref_equals_oracle_layer(extra, chunk):
 def test_f16_rounding_saturates():
     x = torch.tensor([1.0, 1.0 + 2 ** -11, 65504.0, 65519.0, 1e6, -1e6, 2.0 ** -25], dtype=torch.float64)
     assert kr.f16(x).tolist() == [1.0, 1.0, 65504.0, 65504.0, 65504.0, -65504.0, 0.0]
+
+
+# ================================================================================================ CosyVoice3 DiT references
+from oracle import cases, dit as odit, weights as oweights  # noqa: E402
+
+
+def _dit_sd(depth=2):
+    return kr.dit_test_state_dict(depth, 31)
+
+
+def _dit_case(lens, seed):
+    g = torch.Generator().manual_seed(seed)
+    R = sum(lens)
+    x, mu, cond = (kr.bf16(torch.rand(R, 80, generator=g) * 2 - 1) for _ in range(3))
+    return x, mu, cond, kr.bf16(torch.randn(len(lens), 80, generator=g)), torch.tensor([0.3, 0.7][:len(lens)], dtype=torch.float64)
+
+
+def test_dit_modulation_ref_equals_oracle():
+    """kr.dit_modulation == oracle.dit's time_embedding and every AdaLN linear on its SiLU, in float32"""
+    sd = _dit_sd()
+    W = kr.dit_weights(sd, 2)
+    t = torch.tensor([0.05, 0.3, 0.95])
+    te = odit.time_embedding(sd, "decoder.estimator.", t)
+    mod = kr.dit_modulation(W, t.double())["mod"]
+    for i, name in enumerate(["transformer_blocks.0.attn_norm", "transformer_blocks.1.attn_norm", "norm_out"]):
+        p = f"decoder.estimator.{name}.linear."
+        want = F.linear(F.silu(te), sd[p + "weight"], sd[p + "bias"]).double()
+        # fp32 angles up to 950 rad: sin / cos good to ~1e-4 (1000 t e_i rounded to 24 bits); through the time MLP ~1e-4 of |mod| ~ 1
+        assert (mod[:, i * 6144:i * 6144 + want.shape[1]] - want).abs().max().item() < 1e-3, name
+
+
+def test_dit_input_embedding_ref_equals_oracle():
+    """kr.dit_input_embedding (exact) == proj([x | cond | mu | spks]) + oracle.dit.conv_pos_embed, per sequence of a ragged pack"""
+    sd = _dit_sd()
+    W = kr.dit_weights(sd, 2)
+    lens = [37, 1, 64]
+    x, mu, cond, spks, _ = _dit_case(lens, 1)
+    spks = torch.cat([spks, spks[:1]])
+    got = kr.dit_input_embedding(W, x, mu, cond, spks, lens)["x0"]
+    p, o = "decoder.estimator.", 0
+    for b, L in enumerate(lens):
+        h = F.linear(torch.cat([x[o:o + L], cond[o:o + L], mu[o:o + L], spks[b].expand(L, 80)], -1)[None], sd[p + "input_embed.proj.weight"],
+                     sd[p + "input_embed.proj.bias"])
+        want = (odit.conv_pos_embed(sd, p, h) + h)[0].double()
+        assert (got[o:o + L] - want).abs().max().item() < 1e-4, (b, L)          # fp32 oracle on O(1) values
+        o += L
+
+
+@pytest.mark.parametrize("streaming", [False, True])
+def test_dit_block_ref_equals_oracle(streaming):
+    """kr.dit_block (exact) == oracle.dit.dit_block on every sequence of a ragged pack (per-sequence modulation, rotary positions
+    from 0, the 50-frame block-causal mask when streaming)"""
+    sd = _dit_sd()
+    W = kr.dit_weights(sd, 2)
+    lens = [120, 51]
+    g = torch.Generator().manual_seed(2)
+    x = torch.randn(sum(lens), 1024, generator=g)
+    t = torch.tensor([0.2, 0.8])
+    mod = kr.dit_modulation(W, t.double())["mod"]
+    got = kr.dit_block(W, 1, x, mod, lens, 50 if streaming else 0)["x_out"]
+    te = odit.time_embedding(sd, "decoder.estimator.", t)
+    o = 0
+    for b, L in enumerate(lens):
+        m = odit._flow.chunk_attention_mask(L, 50)[None] if streaming else torch.ones(1, L, L, dtype=torch.bool)
+        want = odit.dit_block(sd, "decoder.estimator.transformer_blocks.1.", x[o:o + L][None], te[b:b + 1], m.unsqueeze(1),
+                              odit.rotary_freqs(L))[0].double()
+        assert (got[o:o + L] - want).abs().max().item() < 2e-3 * want.abs().max().item(), (b, L)   # fp32 oracle, gates ~ 1
+        o += L
+
+
+def test_dit_ref_composed_equals_golden(golden):
+    """the fp64 pieces composed (kr.dit_estimator) == the reference DiT's outputs in tests/golden/dit_small.npz (depth 2, the synthetic
+    weights of test_flow3_gpu.py) within the export tolerance (rtol 1e-2, atol 1e-4)"""
+    import numpy as np
+    g = golden("dit_small")
+    sd = oweights.synth_state_dict(odit.flow_param_shapes(2), 1986, odit.SYNTH_GAINS)
+    W = kr.dit_weights(sd, 2)
+    x, mask, mu, t, spks, cond = cases.estimator_case(T=130)
+    tm = lambda a: a.transpose(1, 2).reshape(-1, a.shape[1])
+    for streaming, key in ((False, "est_offline"), (True, "est_stream")):
+        _, out = kr.dit_estimator(W, tm(x), tm(mu), tm(cond), spks, t.double(), [130, 130], streaming)
+        np.testing.assert_allclose(out.numpy(), tm(torch.from_numpy(g[key])).double().numpy(), rtol=1e-2, atol=1e-4)
+
+
+def test_dit_rounding_points():
+    """rounding=True stores bf16 exactly at the DIT_ROUNDING points (and nowhere else); rounding=False nowhere"""
+    sd = _dit_sd()
+    W = kr.dit_weights(sd, 2)
+    lens = [60]
+    x, mu, cond, spks, t = _dit_case(lens, 4)
+    is_b = lambda v: torch.equal(v, kr.bf16(v))
+    mod = kr.dit_modulation(W, t[:1])["mod"]
+    for rounding in (True, False):
+        e = kr.dit_input_embedding(W, x, mu, cond, spks, lens, rounding)
+        st = kr.dit_block(W, 0, e["x0"], mod, lens, 50, rounding)
+        stored = [e["xa"], e["c1"], st["xn"], st["qkv"], st["qkv_rot"], st["att"], st["xn2"], st["h"]]
+        assert all(is_b(v) == rounding for v in stored), rounding
+        assert not any(is_b(v) for v in (e["h"], e["x0"], st["o"], st["x_mid"], st["f"], st["x_out"])), rounding
+
+
+# share of the elements of the mutated result beyond the GPU bound (kr.DIT_TOL) that each mode claims; None: not caught in that mode.
+# Measured on this case: fp32 >= 0.73 for every structural defect, 0.05 for the erf GELU, 0 for eps 1e-5; bf16 0.03 - 0.96 for the
+# structural defects, 0 for the erf GELU and eps 1e-5.
+DIT_CAUGHT = {
+    "fp32": dict(rope_half=0.5, rope_all_heads=0.5, kpos_shift=0.5, adaln_swap=0.5, mod_neighbour=0.5, chunk48=0.5, chunk_edge=0.5,
+                 silu_pos=0.5, time_div=0.5, gelu_erf=0.02, ln_eps=None),
+    "bf16": dict(rope_half=0.1, rope_all_heads=0.3, kpos_shift=0.02, adaln_swap=0.5, mod_neighbour=0.5, chunk48=0.02, chunk_edge=0.01,
+                 silu_pos=0.5, time_div=0.5, gelu_erf=None, ln_eps=None),
+}
+
+
+@pytest.mark.parametrize("precision", ["fp32", "bf16"])
+def test_dit_mutations_exceed_bounds(precision):
+    """each defect of kr.DIT_MUTATIONS, injected into the reference of its mode (exact for fp32, bf16-emulating for bf16), moves at
+    least the stated share of the elements beyond the per-element bound test_dit_blocks_gpu.py holds the kernels to, on a ragged
+    pair of 130 + 70 frames with the streaming mask; the defects a mode does not claim stay below a share of 0.1 there, so the claim
+    list is exact.  The embedding defect is judged on x0, the others on block 0's output."""
+    bf = precision == "bf16"
+    sd = _dit_sd()
+    W = kr.dit_weights(sd, 2)
+    lens = [130, 70]
+    x, mu, cond, spks, t = _dit_case(lens, 3)
+    rms = lambda v: v.pow(2).mean(-1, keepdim=True).sqrt()
+    tol = kr.DIT_TOL[precision]
+    e = kr.dit_input_embedding(W, x, mu, cond, spks, lens, bf)
+    mod = kr.dit_modulation(W, t)["mod"]
+    st = kr.dit_block(W, 0, e["x0"], mod, lens, 50, bf)
+    shares = {}
+    for m in kr.DIT_MUTATIONS:
+        if m == "silu_pos":
+            d, scale, bound = kr.dit_input_embedding(W, x, mu, cond, spks, lens, bf, mutate=m)["x0"] - e["x0"], rms(e["x0"]), tol["embed"]
+        else:
+            mm = kr.dit_modulation(W, t, mutate=m)["mod"] if m == "time_div" else mod
+            sm = kr.dit_block(W, 0, e["x0"], mm, lens, 50, bf, mutate=None if m == "time_div" else m)
+            d, scale, bound = sm["x_out"] - st["x_out"], rms(st["x_out"] - st["x"]), tol["block"]
+        shares[m] = ((d.abs() / scale) > bound).double().mean().item()
+    print(precision, {k: round(v, 3) for k, v in shares.items()})
+    for m, need in DIT_CAUGHT[precision].items():
+        if need is None:
+            assert shares[m] < 0.1, (m, shares[m])
+        else:
+            assert shares[m] >= need, (m, shares[m], need)

@@ -31,7 +31,10 @@ def test_hift3_offline_golden(precision, golden):
     np.testing.assert_allclose(f0.cpu().numpy(), g["f0_final"][0], rtol=1e-4, atol=1e-2)         # float64 predictor (weight-norm folded in fp32)
     assert maxdiff(src, torch.from_numpy(g["source_final"]).reshape(-1)) < 2e-3
     d = maxdiff(wav, torch.from_numpy(g["wav_final"]).reshape(-1))
-    assert d < (2e-3 if precision == "fp32" else 8e-2), d
+    # bf16 (IEEE-half vocoder operands): largest |d| measured on an H100 80GB HBM3 (700 W) 1.12e-2 on |wav| <= 1; the bound is about twice
+    bound = 2e-3 if precision == "fp32" else 2.5e-2
+    print(f"[hift3 offline {precision}] max |d| wav {d:.4g} (bound {bound})")
+    assert d < bound, d
 
 
 def test_hift3_ragged_batch_vs_oracle():
