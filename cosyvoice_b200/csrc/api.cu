@@ -176,6 +176,7 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   else if (k == "flow_qkv_panel") ctx->flow_qkv_panel = value;
   else if (k == "tc_epi") ctx->tc_epi = value;
   else if (k == "tc_persist") ctx->tc_persist = value;
+  else if (k == "tc_epi_frag") ctx->tc_epi_frag = value;
   else if (k == "op_out_bf16") ctx->op_out_bf16 = value;
   else if (k == "op_iters") ctx->op_iters = value;
   else if (k == "use_graph") ctx->use_graph = value;

@@ -179,6 +179,7 @@ struct cvk_ctx {
   double op_ms = 0.0;
   int tc_epi = 2;                           // wgmma GEMM epilogue: 2 = smem-staged TMA stores, otherwise direct stores
   int tc_persist = 2;                       // wgmma GEMM, tiles > SMs: persistent CTAs, one per SM (0 = one CTA per tile)
+  int tc_epi_frag = 1;                      // wgmma GEMM and row-panel GEMM: epilogue on the accumulator fragments (0 = transposed to rows first)
   void* tl = nullptr;                       // device int64[4096] LM-chain timeline (debug option chain_timeline): 4 slots per launch
   int tl_seq = 0;
   long long* tl_next() {                    // slot block of the next launch of the decode chain (null when the option is off)

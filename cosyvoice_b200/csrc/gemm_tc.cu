@@ -257,6 +257,202 @@ __device__ __forceinline__ void stage_store16(uint32_t stg, int dtype, int row, 
   }
 }
 
+// ------------------------------------------------------------------------------------------------ fragment-native epilogue
+// The functions above take 16 consecutive columns of one row, so the kernels first move each thread's accumulator values there with
+// wg_frag_rows16 (12 shuffles and ~32 selects per 16 values).  Every epilogue operation is elementwise in (row, column), so the
+// functions below (option "tc_epi_frag", default 1) apply them where the wgmma left the values: thread (warp w, lane l) of a
+// warpgroup holds rows 16 w + l / 4 and + 8 of its 64, columns 8 j + 2 (l & 3) and + 1 - a 32-column block [cb, cb + 32) of the
+// accumulator is a[4 j + 2 h + e] = (row + 8 h, column cb + 8 j + 2 (l & 3) + e), a = acc + cb / 2.  Each of the two rows has its own
+// sequence and validity; bias, rowvec and resid are read as column pairs; the 16-bit results go to the staging tile with stmatrix.
+// The operations, their order and the activation forms are those of epi_math16p / epi_math16 (the 16-wide fast forms for columns in a
+// whole group of 16 columns, the scalar forms in the partial group at the end of N), so both epilogues give the same bits.
+// Only the staged epilogue with 16-bit outputs takes this path: with an fp32 output (8-byte shared stores) and with direct stores
+// (column-pair global stores) it was slower than the transposing epilogue on an H100 (the 40064 x 512 -> 256 projection with an fp32
+// residual 82.5 against 76.3 us per launch, its accumulating direct-store form 112.4 against 72.5 us; H100 80GB HBM3, 700 W).
+struct FragRows {
+  int r[2], seq[2];
+  bool rin[2], valid[2];
+};
+
+__device__ __forceinline__ FragRows frag_rows(const EpiDev& e, int r, int rowsOut) {
+  FragRows f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    f.r[h] = r + 8 * h;
+    f.rin[h] = f.r[h] < rowsOut;
+    f.seq[h] = (f.rin[h] && e.row2seq) ? e.row2seq[f.r[h]] : 0;
+    f.valid[h] = f.rin[h] && (!e.row2seq || f.seq[h] >= 0);
+  }
+  return f;
+}
+
+// columns n and n + 1 of a row; WHOLE: both < N, otherwise those >= N read nothing and give 0
+template <bool WHOLE> __device__ __forceinline__ float2 ld_pair(const float* p, int n, int N) {
+  if (WHOLE) return *reinterpret_cast<const float2*>(p);
+  return make_float2(n < N ? p[0] : 0.f, n + 1 < N ? p[1] : 0.f);
+}
+
+// act16_fast over the block's 16 values; Snake reads its per-column alpha[n + 8 j + e] (1 where alpha is null or beyond N)
+template <bool WHOLE>
+__device__ __forceinline__ void frag_act(int act, float param, const float* alpha, int n, int N, float* v) {
+  if (act != ACT_SNAKE) {
+    act16_fast(act, v, param, nullptr);
+    return;
+  }
+  float al[16];
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = n + 8 * j + e;
+      al[4 * j + e] = al[4 * j + 2 + e] = (alpha && (WHOLE || c < N)) ? alpha[c] : 1.f;
+    }
+  act16_fast(ACT_SNAKE, v, param, al);
+}
+
+// v = act1(a + bias + rowvec) * scale + resid, zero in invalid rows, for the 32-column block [cb, cb + 32) of the tile at matrix column n0
+// (s_bias: the tile's bias), q = lane & 3.  WHOLE: all 32 columns < N.  PLAIN: the epilogue has no activation, rowvec, residual or
+// second output and scale 1 (frag_plain), so v = a + bias and nothing else is compiled in.
+template <bool WHOLE, bool PLAIN = false>
+__device__ __forceinline__ void frag_math(const EpiDev& e, const FragRows& f, const float* s_bias, int n0, int cb, int q, int N, const float* a,
+                                          float* v) {
+  const int cl = cb + 2 * q, n = n0 + cl;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) v[i] = a[i];
+  if (e.bias) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 b = *reinterpret_cast<const float2*>(s_bias + cl + 8 * j);
+      v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.x; v[4 * j + 3] += b.y;
+    }
+  }
+  if (!PLAIN && e.rowvec) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!f.valid[h]) continue;
+      const float* rv = e.rowvec + (size_t)f.seq[h] * e.rowvec_ld + n;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 b = ld_pair<WHOLE>(rv + 8 * j, n + 8 * j, N);
+        v[4 * j + 2 * h] += b.x; v[4 * j + 2 * h + 1] += b.y;
+      }
+    }
+  }
+  if (!PLAIN) {
+    frag_act<WHOLE>(e.act1, e.act1_param, e.alpha1, n, N, v);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] *= e.scale;
+  }
+  if (!PLAIN && e.resid) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!f.rin[h]) continue;
+      const float* rp = e.resid + (size_t)f.r[h] * e.resid_ld + n;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 b = ld_pair<WHOLE>(rp + 8 * j, n + 8 * j, N);
+        v[4 * j + 2 * h] += b.x; v[4 * j + 2 * h + 1] += b.y;
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+    if (!f.valid[h]) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[4 * j + 2 * h] = v[4 * j + 2 * h + 1] = 0.f;
+    }
+}
+
+// v <- act2(v), zero in invalid rows
+template <bool WHOLE>
+__device__ __forceinline__ void frag_act2(const EpiDev& e, const FragRows& f, int n0, int cb, int q, int N, float* v) {
+  frag_act<WHOLE>(e.act2, e.act2_param, e.alpha2, n0 + cb + 2 * q, N, v);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+    if (!f.valid[h]) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[4 * j + 2 * h] = v[4 * j + 2 * h + 1] = 0.f;
+    }
+}
+
+// staged epilogue (epi_mode 2), out values of one 32-column block.  In the block at the end of N the columns of a partial 16-column
+// group take epi_math16's scalar forms; columns >= N hold junk that the clipped TMA store never writes.
+template <bool PLAIN>
+__device__ __forceinline__ void frag_values(const EpiDev& e, const FragRows& f, const float* s_bias, int n0, int cb, int q, int N, const float* a,
+                                            float* v) {
+  if (n0 + cb + 32 <= N) {
+    frag_math<true, PLAIN>(e, f, s_bias, n0, cb, q, N, a, v);
+    return;
+  }
+  frag_math<false, PLAIN>(e, f, s_bias, n0, cb, q, N, a, v);
+  const int n = n0 + cb + 2 * q;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (n0 + cb + 16 * (j >> 1) + 16 <= N) continue;   // a whole group of 16
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int x = 0; x < 2; ++x) {
+        const int c = n + 8 * j + x;
+        if (c >= N) continue;
+        float t = a[4 * j + 2 * h + x] + (e.bias ? e.bias[c] : 0.f);
+        if (e.rowvec && f.valid[h]) t += e.rowvec[(size_t)f.seq[h] * e.rowvec_ld + c];
+        t = apply_act_fast(e.act1, t, e.act1_param, e.alpha1 ? e.alpha1[c] : 1.f) * e.scale;
+        if (e.resid && f.rin[h]) t += e.resid[(size_t)f.r[h] * e.resid_ld + c];
+        v[4 * j + 2 * h + x] = f.valid[h] ? t : 0.f;
+      }
+  }
+}
+
+// ... and its out2 values, in place over the out values
+__device__ __forceinline__ void frag_values2(const EpiDev& e, const FragRows& f, int n0, int cb, int q, int N, float* v) {
+  if (n0 + cb + 32 <= N) {
+    frag_act2<true>(e, f, n0, cb, q, N, v);
+    return;
+  }
+  float w[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) w[i] = v[i];
+  frag_act2<false>(e, f, n0, cb, q, N, w);
+  const int n = n0 + cb + 2 * q;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (n0 + cb + 16 * (j >> 1) + 16 <= N) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int x = 0; x < 2; ++x) {
+        const int c = n + 8 * j + x, i = 4 * j + 2 * h + x;
+        if (c < N) w[i] = f.valid[h] ? apply_act_fast(e.act2, v[i], e.act2_param, e.alpha2 ? e.alpha2[c] : 1.f) : 0.f;
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) v[i] = w[i];
+}
+
+// an epilogue that only adds the bias (no activation, rowvec, residual or second output, scale 1) - the estimator's qkv projection
+// and most of the flow's convolutions: the kernels compile it without the other operations (EPI 2)
+inline bool frag_plain(const EpiDev& e) {
+  return e.act1 == ACT_NONE && !e.rowvec && !e.resid && e.scale == 1.f && !e.out2;
+}
+
+// one 32-column block of the fragment into a 16-bit staging tile (stage_store16's layout), one stmatrix per 16 x 16; row0 = the tile
+// row of the warp's first row
+__device__ __forceinline__ void frag_stage16(uint32_t stg, int dtype, int row0, int lane, int cb, const float* v) {
+  uint32_t pk[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (dtype == DT_BF16) {
+      __nv_bfloat162 h2 = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
+      pk[i] = *reinterpret_cast<uint32_t*>(&h2);
+    } else {
+      pk[i] = (uint32_t)f32_to_16(v[2 * i], DT_F16) | ((uint32_t)f32_to_16(v[2 * i + 1], DT_F16) << 16);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 2; ++k) stmatrix_x4(stg + stg_stmatrix_offset(row0, 0, lane, cb / 16 + k), pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]);
+}
+
 // One CTA computes 128 x BN output tiles: warp 0 (lane 0) is the TMA producer, warpgroups 1 and 2 each issue wgmma for 64 of the
 // 128 rows and run the fused epilogue on their own accumulators.  With more tiles than CTAs (persistent launch, one CTA per SM)
 // a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (column tile fastest, so CTAs running at the same time share A
@@ -266,7 +462,7 @@ __device__ __forceinline__ void stage_store16(uint32_t stg, int dtype, int row, 
 // waits for a store to have read the staging tile only before the next tile is staged.  epi_mode 0: direct per-thread stores.
 constexpr uint32_t TC_STG_BYTES = 65536;
 
-template <int BN, int NSTG>
+template <int BN, int NSTG, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o2, int N, int K, int taps,
@@ -317,6 +513,7 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   const int q = lane & 3;
   const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);   // the tile row this thread's epilogue owns
   const int cq = 16 * (q >> 1);                       // ... and its 16 columns of every 32
+  const int frow0 = wg * 64 + (warp & 3) * 16;        // fragment epilogue: the warp's first tile row
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int r0 = (tile / ntn) * TC_BM, n0 = (tile % ntn) * BN;
@@ -327,8 +524,14 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     asm volatile("bar.sync 1, 256;" ::: "memory");
     for (int i = ct; i < BN; i += 256) s_bias[i] = (ep.bias && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
     int seq = 0;
-    if (rin && ep.row2seq) seq = ep.row2seq[r];
-    const bool valid = rin && (!ep.row2seq || seq >= 0);
+    bool valid = false;
+    FragRows f;
+    if (EPI) {
+      f = frag_rows(ep, r0 + frow0 + (lane >> 2), rowsOut);
+    } else {
+      if (rin && ep.row2seq) seq = ep.row2seq[r];
+      valid = rin && (!ep.row2seq || seq >= 0);
+    }
 
     float acc[BN / 2];
 #pragma unroll
@@ -361,19 +564,33 @@ conv_gemm_wg_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 
     const uint32_t stg1 = stg_base;
     const uint32_t stg2 = stg_base + (uint32_t)TC_BM * BN * (ep.out_dtype == DT_F32 ? 4u : 2u);
+    if (EPI) {
 #pragma unroll
-    for (int cb = 0; cb < BN; cb += 32) {
-      float a16[16], v[16], w2[16];
-      wg_frag_rows16(acc + cb / 2, lane, a16);
-      const int c = cb + cq;
-      if (n0 + c < N) {
-        if (epi_mode == 2) {
-          if (n0 + c + 16 <= N) epi_math16p(ep, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
-          else epi_math16(ep, r, rin, n0 + c, N, a16, v, w2);
-          stage_store16(stg1, ep.out_dtype, row, c, v);
-          if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c, w2);
-        } else if (rin) {
-          epi_store16(ep, r, n0 + c, N, a16);
+      for (int cb = 0; cb < BN; cb += 32) {
+        if (n0 + cb >= N) break;
+        float v[16];
+        frag_values<EPI == 2>(ep, f, s_bias, n0, cb, q, N, acc + cb / 2, v);
+        frag_stage16(stg1, ep.out_dtype, frow0, lane, cb, v);
+        if (EPI == 1 && ep.out2) {
+          frag_values2(ep, f, n0, cb, q, N, v);
+          frag_stage16(stg2, ep.out2_dtype, frow0, lane, cb, v);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int cb = 0; cb < BN; cb += 32) {
+        float a16[16], v[16], w2[16];
+        wg_frag_rows16(acc + cb / 2, lane, a16);
+        const int c = cb + cq;
+        if (n0 + c < N) {
+          if (epi_mode == 2) {
+            if (n0 + c + 16 <= N) epi_math16p(ep, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
+            else epi_math16(ep, r, rin, n0 + c, N, a16, v, w2);
+            stage_store16(stg1, ep.out_dtype, row, c, v);
+            if (ep.out2) stage_store16(stg2, ep.out2_dtype, row, c, w2);
+          } else if (rin) {
+            epi_store16(ep, r, n0 + c, N, a16);
+          }
         }
       }
     }
@@ -399,14 +616,15 @@ constexpr size_t wg_smem() {
   return (size_t)NSTG * (TC_BM * TC_BK * 2 + BN * TC_BK * 2) + TC_STG_BYTES + 1024;
 }
 
-template <int BN, int NSTG>
+template <int BN, int NSTG, int EPI>
 void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& to, const CUtensorMap& to2,
                const ConvW& W, int rowsOut, const EpiDev& e, int epi_mode) {
   constexpr size_t smem = wg_smem<BN, NSTG>();
   const int ntn = ceil_div(W.N, BN), ntiles = ntn * ceil_div(rowsOut, TC_BM);
   // more tiles than SMs: persistent CTAs (one per SM) unless switched off
   const int grid = (ctx->tc_persist && ntiles > ctx->num_sms) ? ctx->num_sms : ntiles;
-  conv_gemm_wg_kernel<BN, NSTG><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode, ntn, ntiles);
+  conv_gemm_wg_kernel<BN, NSTG, EPI><<<grid, TC_THREADS, smem, st>>>(ta, tw, to, to2, W.N, W.K, W.taps, W.dil, W.shift0, rowsOut, e, epi_mode,
+                                                                     ntn, ntiles);
 }
 
 // ------------------------------------------------------------------------------------------------ row-panel GEMM, K = 256
@@ -427,7 +645,8 @@ void launch_wg(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CUten
 // walks units blockIdx.x, blockIdx.x + gridDim.x, ...  The next unit's first W chunk is requested before its A panel; the panel load
 // itself waits for the unit's last MMAs and lands under the last epilogue.
 // Per output the MMAs are those of conv_gemm_wg_kernel (K sub-tiles ascending, four k16 steps each, one fp32 accumulator from zero)
-// and the epilogue is its epi_math16p / stage_store16, so the results agree bit for bit.
+// and the epilogue is its 16-bit staged one (frag_math / frag_stage16; epi_math16p / stage_store16 with tc_epi_frag 0), so the results
+// agree bit for bit.
 constexpr int QP_K = 256, QP_BN = 128, QP_NSTG = 2;
 constexpr uint32_t QP_A_BYTES = TC_BM * QP_K * 2;
 constexpr uint32_t QP_W_BYTES = QP_BN * QP_K * 2;
@@ -437,6 +656,7 @@ constexpr size_t QP_SMEM = QP_A_BYTES + QP_NSTG * QP_W_BYTES + QP_STG_BYTES + 10
 // kernel (H100 80GB HBM3, 700 W); smaller launches, the streaming sessions' 50-frame chunks among them, have not been timed and stay there
 constexpr int QP_MIN_PANELS = 25;
 
+template <int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ CUtensorMap tmap_o, int shift0, int rowsOut, EpiDev ep, int ngroups, int cpu, int nunits) {
@@ -494,6 +714,7 @@ qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int q = lane & 3;
   const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);   // the panel row this thread's epilogue owns
   const int cq = 16 * (q >> 1);                       // ... and its 16 columns of every 32
+  const int frow0 = wg * 64 + (warp & 3) * 16;        // fragment epilogue: the warp's first panel row
   const uint32_t a_wg = smem_base + (uint32_t)wg * (64 * 128u);
   float* s_bias = s_bias_all + wg * QP_BN;
   EpiDev e = ep;
@@ -501,6 +722,7 @@ qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   int r0 = 0, r = 0, seq = 0;
   bool rin = false, valid = false;
+  FragRows f;
   // the 16 MMAs of one chunk: K sub-tiles ascending, four k16 steps each, into a zeroed accumulator
   auto issue = [&](float* acc, uint32_t it) {
     const uint32_t s = it % QP_NSTG;
@@ -535,13 +757,22 @@ qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous store has read the staging tile
     s_bias[wt] = bv;
     asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if (EPI) {
 #pragma unroll
-    for (int cb = 0; cb < QP_BN; cb += 32) {
-      float a16[16], v[16], w2[16];
-      wg_frag_rows16(acc + cb / 2, lane, a16);
-      const int c = cb + cq;
-      epi_math16p(e, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
-      stage_store16(stg_base, e.out_dtype, row, c, v);
+      for (int cb = 0; cb < QP_BN; cb += 32) {
+        float v[16];
+        frag_math<true, EPI == 2>(e, f, s_bias, n0, cb, q, n0 + QP_BN, acc + cb / 2, v);
+        frag_stage16(stg_base, e.out_dtype, frow0, lane, cb, v);
+      }
+    } else {
+#pragma unroll
+      for (int cb = 0; cb < QP_BN; cb += 32) {
+        float a16[16], v[16], w2[16];
+        wg_frag_rows16(acc + cb / 2, lane, a16);
+        const int c = cb + cq;
+        epi_math16p(e, r, rin, seq, valid, s_bias, c, n0 + c, a16, v, w2);
+        stage_store16(stg_base, e.out_dtype, row, c, v);
+      }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
@@ -558,11 +789,15 @@ qkv_panel_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   for (int u = blockIdx.x; u < nunits; u += gridDim.x, ++ui) {
     r0 = (u / ngroups) * TC_BM;
     const int nb = (u % ngroups) * cpu * QP_BN;
-    r = r0 + row;
-    rin = r < rowsOut;
-    seq = 0;
-    if (rin && e.row2seq) seq = e.row2seq[r];
-    valid = rin && (!e.row2seq || seq >= 0);
+    if (EPI) {
+      f = frag_rows(e, r0 + frow0 + (lane >> 2), rowsOut);
+    } else {
+      r = r0 + row;
+      rin = r < rowsOut;
+      seq = 0;
+      if (rin && e.row2seq) seq = e.row2seq[r];
+      valid = rin && (!e.row2seq || seq >= 0);
+    }
     mbar_wait(smem_u32(&bar_a_full), ui & 1u);
     issue(acc0, it);
     for (int c = 0; c < cpu; c += 2) {
@@ -610,7 +845,10 @@ void launch_panel(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CU
     if (best < 0 || cost < best) { best = cost; ngroups = g; }
   }
   const int nunits = panels * ngroups;
-  qkv_panel_kernel<<<std::min(nunits, ctx->num_sms), TC_THREADS, QP_SMEM, st>>>(ta, tw, to, W.shift0, rowsOut, e, ngroups, nch / ngroups, nunits);
+  const int grid = std::min(nunits, ctx->num_sms);
+  const int epi = !ctx->tc_epi_frag ? 0 : frag_plain(e) ? 2 : 1;
+  auto k = epi == 2 ? qkv_panel_kernel<2> : epi == 1 ? qkv_panel_kernel<1> : qkv_panel_kernel<0>;
+  k<<<grid, TC_THREADS, QP_SMEM, st>>>(ta, tw, to, W.shift0, rowsOut, e, ngroups, nch / ngroups, nunits);
 }
 
 // ------------------------------------------------------------------------------------------------ fused feed-forward
@@ -857,8 +1095,20 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
     if (ep.out2.p) mk(&to2, ep.out2);
   }
   if (panel) launch_panel(ctx, st, ta, tw, to, W, rowsOut, e);
-  else if (BN == 128) launch_wg<128, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
-  else launch_wg<64, 4>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+  else {
+    // the fragment epilogue: staged stores of 16-bit outputs only (see frag_values)
+    const bool frag = ctx->tc_epi_frag && epi_mode == 2 && ep.out.esize() == 2 && (!ep.out2.p || ep.out2.esize() == 2);
+    const int epi = !frag ? 0 : frag_plain(e) ? 2 : 1;
+    if (BN == 128) {
+      if (epi == 2) launch_wg<128, 4, 2>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+      else if (epi == 1) launch_wg<128, 4, 1>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+      else launch_wg<128, 4, 0>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+    } else {
+      if (epi == 2) launch_wg<64, 4, 2>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+      else if (epi == 1) launch_wg<64, 4, 1>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+      else launch_wg<64, 4, 0>(ctx, st, ta, tw, to, to2, W, rowsOut, e, epi_mode);
+    }
+  }
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }
@@ -895,8 +1145,14 @@ void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, 
 }
 
 void gemm_tc_setup() {
-  CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<128, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<128, 4>()));
-  CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<64, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<64, 4>()));
-  CVK_CHECK_CUDA(cudaFuncSetAttribute(qkv_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QP_SMEM));
+  auto set = [](auto epi) {
+    constexpr int E = decltype(epi)::value;
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<128, 4, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<128, 4>()));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_wg_kernel<64, 4, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<64, 4>()));
+    CVK_CHECK_CUDA(cudaFuncSetAttribute(qkv_panel_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QP_SMEM));
+  };
+  set(std::integral_constant<int, 0>());
+  set(std::integral_constant<int, 1>());
+  set(std::integral_constant<int, 2>());
   CVK_CHECK_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
 }

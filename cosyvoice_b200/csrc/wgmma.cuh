@@ -93,6 +93,25 @@ __device__ __forceinline__ void wgmma_rs_m64n256(float* d, const uint32_t* a, ui
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
 
+// stmatrix (sm_90): four 8 x 8 matrices of 16-bit values from a warp's registers to shared memory.  Lane l gives the address of row l % 8
+// of matrix l / 8; register i of lane l holds row l / 4, columns 2 (l & 3) (low half) and + 1 of matrix i - the accumulator layout
+// above, so one instruction stores a 16 x 16 block of a warp's fragment.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+
+// 16-bit staging tile of a GEMM epilogue for TMA stores with CU_TENSOR_MAP_SWIZZLE_128B: sub-tiles of 64 columns (128 bytes) by 128
+// rows, 16 KB each, the 16-byte chunk k of a row stored at chunk k ^ (row & 7).  Byte offset of element (row, col).
+__host__ __device__ __forceinline__ uint32_t stg_offset16(int row, int col) {
+  return (uint32_t)(col >> 6) * 16384u + (uint32_t)row * 128u + (((uint32_t)((col & 63) >> 3) ^ (uint32_t)(row & 7)) << 4) + (uint32_t)(col & 7) * 2u;
+}
+// Where lane `lane` of warp w (0..3 of its warpgroup, whose rows start at tile row row0) points stmatrix_x4 for the 16 x 16 block of
+// accumulator columns [16 k, 16 k + 16): matrix m = lane / 8 is rows + 8 (m & 1), columns + 8 (m >> 1) of the block, i.e. the
+// registers packed from d[8 k + 2 m] and d[8 k + 2 m + 1].
+__host__ __device__ __forceinline__ uint32_t stg_stmatrix_offset(int row0, int w, int lane, int k) {
+  return stg_offset16(row0 + 16 * w + (lane & 7) + 8 * ((lane >> 3) & 1), 16 * k + 8 * (lane >> 4));
+}
+
 // four values by a run-time index in 0..3 without local-memory indexing
 __device__ __forceinline__ float wg_sel4(float a0, float a1, float a2, float a3, int i) {
   const float lo = (i & 1) ? a1 : a0, hi = (i & 1) ? a3 : a2;

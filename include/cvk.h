@@ -71,7 +71,7 @@ int cvk_debug_read(cvk_ctx* ctx, long long* out, int n);
  * the calls made so far - what a caller needs to size cvk_create for its largest batch. */
 int cvk_workspace_bytes(cvk_ctx* ctx, size_t* capacity, size_t* high_water);
 /* Test / measurement switches, NOT part of the drop-in surface (every default is the benchmarked configuration): kernel-variant
- * A/B ("use_tc", "tc_persist", "tc_epi", "use_tc_attn", "enc_tc_attn", "use_skinny", "flow_fused_ff", "flow_qkv_panel" (0 / 1 /
+ * A/B ("use_tc", "tc_persist", "tc_epi", "tc_epi_frag", "use_tc_attn", "enc_tc_attn", "use_skinny", "flow_fused_ff", "flow_qkv_panel" (0 / 1 /
  * 2 = the row-panel GEMM never / from 25 panels of 128 rows up / at any row count), "lm_fused", "lm_mega", "mega_coop", "pdl", "use_graph", "hift_f16" - the last one takes effect at the next cvk_finalize("hift")),
  * probes ("op_iters", "op_out_bf16", "chain_timeline").  Unknown keys return CVK_ERR_INVALID. */
 int cvk_set_option(cvk_ctx* ctx, const char* key, int value);
