@@ -11,9 +11,11 @@ void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const f
 void hift_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* noise, const float* cache_source,
                     const int* cache_lens, float* wav, float* source_out, cudaStream_t st);
 void flow_build(cvk_ctx* ctx, const int* cfg, int ncfg);
-void flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B, int streaming, int context_len, float* h, cudaStream_t st);
+void flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B, int streaming, int context_len, float* h, cudaStream_t st,
+                  int n_layers = 0, float* hidden = nullptr);
 void flow_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
-                    int B, int streaming, float* out, cudaStream_t st);
+                    int B, int streaming, float* out, cudaStream_t st, int n_units = 0,
+                    float* hidden = nullptr);
 void flow_cfm_solve(cvk_ctx* ctx, const float* mu, const float* spks, const float* cond, const int* lens, int B, const float* z,
                     int n_timesteps, float cfg_rate, int streaming, float* out, cudaStream_t st);
 void flow_inference(cvk_ctx* ctx, const int32_t* tokens, const int* token_lens, const float* prompt_feat, const int* prompt_feat_lens,
@@ -656,11 +658,25 @@ int cvk_flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B
   flow_encoder(ctx, tokens, lens, B, streaming, context_len, h, (cudaStream_t)stream);
   CVK_API_END
 }
+int cvk_flow_encoder_hidden(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B, int streaming, int context_len, int n_layers,
+                            float* hidden, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(tokens && lens && hidden && B > 0 && (context_len == 0 || context_len == 3), "cvk_flow_encoder_hidden: bad arguments");
+  flow_encoder(ctx, tokens, lens, B, streaming, context_len, nullptr, (cudaStream_t)stream, n_layers, hidden);
+  CVK_API_END
+}
 int cvk_cfm_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
                       int B, int streaming, float* out, void* stream) {
   CVK_API_BEGIN
   CVK_REQUIRE(x && mu && t && spks && cond && lens && out && B > 0, "cvk_cfm_estimator: bad arguments");
   flow_estimator(ctx, x, mu, t, spks, cond, lens, B, streaming, out, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_cfm_estimator_hidden(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
+                             const int* lens, int B, int streaming, int n_units, float* hidden, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(x && mu && t && spks && cond && lens && hidden && B > 0, "cvk_cfm_estimator_hidden: bad arguments");
+  flow_estimator(ctx, x, mu, t, spks, cond, lens, B, streaming, nullptr, (cudaStream_t)stream, n_units, hidden);
   CVK_API_END
 }
 int cvk_cfm_estimator_inplace(cvk_ctx* ctx, float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,

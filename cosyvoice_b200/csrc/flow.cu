@@ -538,8 +538,12 @@ Mat make_pe(cvk_ctx* ctx, cudaStream_t st, int max_len, int* center) {
 }
 
 // tokens (dense, sum of full lens) -> encoder output h [R2, 512] fp32 in the x2 geometry s2 (returned)
+// hidden != nullptr (the test-only read-out cvk_flow_encoder_hidden): stop after the first n_layers units and write the fp32 residual
+// stream there instead: unit 0 is the embedding with the PreLookahead layer, then one per conformer layer, then up_conv + up_embed, then
+// one per up layer ([sum T - context_len, 512] at the token rate up to enc_blocks, [sum 2 (T - context_len), 512] after); *s2_out
+// is then not written
 Mat encoder_forward(cvk_ctx* ctx, cudaStream_t st, const int32_t* tokens, const int* lens, int B, int streaming, int context_len,
-                    Seqs* s2_out) {
+                    Seqs* s2_out, int n_layers = 0, float* hidden = nullptr) {
   FlowModel* m = ctx->flow;
   const int adt = ctx->act_dtype;
   Seqs sf = make_seqs(ctx, lens, B, 8, 1, 0, st);                                       // all tokens incl. look-ahead context
@@ -582,7 +586,13 @@ Mat encoder_forward(cvk_ctx* ctx, cudaStream_t st, const int32_t* tokens, const 
   }
   int center = 0;
   Mat pe = make_pe(ctx, st, s1.max_len, &center);
-  for (auto& l : m->enc) enc_layer(ctx, st, l, s1, x, pe, center, streaming ? CHUNK_TOK : 0);
+  const int n_enc = (int)m->enc.size();
+  const int n_run = hidden ? (n_layers < n_enc ? n_layers : n_enc) : n_enc;
+  for (int i = 0; i < n_run; ++i) enc_layer(ctx, st, m->enc[i], s1, x, pe, center, streaming ? CHUNK_TOK : 0);
+  if (hidden && n_layers <= n_enc) {
+    unpack_rows(ctx, st, x, s1, 0, hidden, D_ENC);
+    return x;
+  }
   // nearest x2 + conv k5 (polyphase): [R, 2*512] == [2R, 512]
   Mat xa = x;
   if (adt != DT_F32) {
@@ -601,7 +611,12 @@ Mat encoder_forward(cvk_ctx* ctx, cudaStream_t st, const int32_t* tokens, const 
   Mat y = arena_mat(ctx, DT_F32, s2.R, D_ENC);
   embed_apply(ctx, st, m->up_embed, up2, s2, y);
   Mat pe2 = make_pe(ctx, st, s2.max_len, &center);
-  for (auto& l : m->enc_up) enc_layer(ctx, st, l, s2, y, pe2, center, streaming ? 2 * CHUNK_TOK : 0);
+  const int n_up = hidden ? n_layers - n_enc - 1 : (int)m->enc_up.size();
+  for (int i = 0; i < n_up; ++i) enc_layer(ctx, st, m->enc_up[i], s2, y, pe2, center, streaming ? 2 * CHUNK_TOK : 0);
+  if (hidden) {
+    unpack_rows(ctx, st, y, s2, 0, hidden, D_ENC);
+    return y;
+  }
   Mat h = arena_mat(ctx, DT_F32, s2.R, D_ENC);
   layernorm(ctx, st, y, m->after_g, m->after_b, 1e-5f, ACT_NONE, 1.f, s2.d_row2seq, h);
   *s2_out = s2;
@@ -733,8 +748,9 @@ void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstB
 
 // resnet (matcha decoder.py:55-61 with CausalBlock1D) + n transformer blocks.  `in` = act operand [R, Cin];
 // the stage's output residual stream ends in b.x (fp32) and, as an activation operand, in *out_act.
+// n_tb >= 0 (the test-only read-out cvk_cfm_estimator_hidden): run only the first n_tb transformer blocks
 void stage_forward(cvk_ctx* ctx, cudaStream_t st, const StageW& w, int stage_idx, const Seqs& s, const Mat& in, EstBuffers& b, int chunk,
-                   const Mat& out_act, EstInc* inc = nullptr) {
+                   const Mat& out_act, EstInc* inc = nullptr, int n_tb = -1) {
   const float* tvec = b.temb_all.f32() + (size_t)stage_idx * C_EST;
   conv_state(ctx, st, inc, in, s);
   {
@@ -759,15 +775,19 @@ void stage_forward(cvk_ctx* ctx, cudaStream_t st, const StageW& w, int stage_idx
     e.out = b.x;
     conv_gemm(ctx, st, in, w.rn.res, e);
   }
-  for (size_t j = 0; j < w.tb.size(); ++j) {
+  const size_t n_run = n_tb < 0 ? w.tb.size() : (size_t)n_tb;
+  for (size_t j = 0; j < n_run; ++j) {
     const bool last = j + 1 == w.tb.size();
     tblock(ctx, st, w.tb[j], s, b, chunk, last ? &out_act : nullptr, inc, j == 0, last ? nullptr : &w.tb[j + 1]);
   }
 }
 
 // in0: act [R,320] packed input; t: [B2] device; out: fp32 [R,80] (ld 80)
+// hidden != nullptr (the test-only read-out cvk_cfm_estimator_hidden): stop after the first n_units units - a unit is one stage's
+// resnet or one of its transformer blocks, in execution order; down_conv belongs to the first mid-stage resnet - and write the fp32
+// residual stream b.x [sum T, 256] there instead of running the tail; `out` is then not written
 void estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& in0, const float* t_dev, int streaming, const Mat& out,
-                       EstInc* inc = nullptr) {
+                       EstInc* inc = nullptr, int n_units = 0, float* hidden = nullptr) {
   FlowModel* m = ctx->flow;
   const int adt = ctx->act_dtype;
   const int chunk = streaming ? 2 * CHUNK_TOK : 0;
@@ -809,8 +829,21 @@ void estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& 
     e.out = b.temb_all;
     conv_gemm_simt(ctx, st, te3, m->tmlp_all, e);
   }
+  // hidden: run `left` more units; stage() is true once they have run and the residual stream is written out
+  int left = hidden ? n_units : -1;
+  auto stage = [&](int k, const Mat& in, const Mat& out_act) {
+    const int per = 1 + (int)m->stages[k].tb.size();
+    const int n = left < 0 || left >= per ? per : left;
+    stage_forward(ctx, st, m->stages[k], k, s, in, b, chunk, out_act, inc, left < 0 ? -1 : n - 1);
+    if (left < 0) return false;
+    left -= n;
+    if (left > 0) return false;
+    unpack_rows(ctx, st, b.x, s, 0, hidden, C_EST);
+    ctx->arena.off = mark;
+    return true;
+  };
   // down stage: output -> skip half of `cat`
-  stage_forward(ctx, st, m->stages[0], 0, s, in0, b, chunk, b.cat.slice(C_EST, C_EST), inc);
+  if (stage(0, in0, b.cat.slice(C_EST, C_EST))) return;
   conv_state(ctx, st, inc, b.cat.slice(C_EST, C_EST), s);
   {
     Epilogue e;      // down_blocks.0.2 causal conv on the skip tensor
@@ -820,10 +853,10 @@ void estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const Mat& 
   }
   for (int i = 0; i < m->num_mid; ++i) {
     bool last = i + 1 == m->num_mid;
-    stage_forward(ctx, st, m->stages[1 + i], 1 + i, s, b.xa, b, chunk, last ? b.cat.slice(0, C_EST) : b.xa, inc);
+    if (stage(1 + i, b.xa, last ? b.cat.slice(0, C_EST) : b.xa)) return;
   }
   if (m->num_mid == 0) convert_mat(ctx, st, b.xa, b.cat.slice(0, C_EST));
-  stage_forward(ctx, st, m->stages[nst - 1], nst - 1, s, b.cat, b, chunk, b.xa, inc);
+  if (stage(nst - 1, b.cat, b.xa)) return;
   conv_state(ctx, st, inc, b.xa, s);
   {
     Epilogue e;      // up_blocks.0.2
@@ -1211,17 +1244,27 @@ void dit_estimator_forward(cvk_ctx* ctx, cudaStream_t st, const Seqs& s, const M
 }  // namespace
 
 // ================================================================================================ entry points
-void flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B, int streaming, int context_len, float* h_out, cudaStream_t st) {
+// hidden != nullptr: cvk_flow_encoder_hidden, the residual stream after n_layers units (encoder_forward) to hidden instead of h_out
+void flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens, int B, int streaming, int context_len, float* h_out, cudaStream_t st,
+                  int n_layers, float* hidden) {
   CVK_REQUIRE(ctx->flow && ctx->flow->tok_emb, "flow stage not finalised");
+  const FlowModel* m = ctx->flow;
+  CVK_REQUIRE(!hidden || (n_layers >= 0 && n_layers <= m->enc_blocks + 1 + m->enc_up_blocks),
+              "cvk_flow_encoder_hidden: n_layers outside [0, enc_blocks + 1 + enc_up_blocks]");
   ctx->arena.reset();
   Seqs s2;
-  Mat h = encoder_forward(ctx, st, tokens, lens, B, streaming, context_len, &s2);
-  unpack_rows(ctx, st, h, s2, 0, h_out, D_ENC);
+  Mat h = encoder_forward(ctx, st, tokens, lens, B, streaming, context_len, &s2, n_layers, hidden);
+  if (!hidden) unpack_rows(ctx, st, h, s2, 0, h_out, D_ENC);
 }
 
+// hidden != nullptr: cvk_cfm_estimator_hidden, the residual stream after n_units units (estimator_forward) to hidden [sum T, 256]
+// instead of the estimator output
 void flow_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
-                    int B, int streaming, float* out, cudaStream_t st) {
+                    int B, int streaming, float* out, cudaStream_t st, int n_units, float* hidden) {
   CVK_REQUIRE(ctx->flow && ctx->flow->tok_emb, "flow stage not finalised");
+  const FlowModel* m = ctx->flow;
+  CVK_REQUIRE(!hidden || (n_units >= 1 && n_units <= (int)m->stages.size() * (1 + m->n_blocks)),
+              "cvk_cfm_estimator_hidden: n_units outside [1, n_stages * (1 + n_blocks)]");
   ctx->arena.reset();
   const int adt = ctx->act_dtype;
   Seqs s = make_seqs(ctx, lens, B, 8, 1, 0, st);
@@ -1234,8 +1277,8 @@ void flow_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* 
   ctx->launches++;
   CVK_LAUNCH_CHECK();
   Mat v = arena_mat(ctx, DT_F32, s.R, N_MEL, N_MEL);
-  estimator_forward(ctx, st, s, in0, t, streaming, v);
-  unpack_rows(ctx, st, v, s, 0, out, N_MEL);
+  estimator_forward(ctx, st, s, in0, t, streaming, v, nullptr, n_units, hidden);
+  if (!hidden) unpack_rows(ctx, st, v, s, 0, out, N_MEL);
 }
 
 void flow_cfm_solve(cvk_ctx* ctx, const float* mu, const float* spks, const float* cond, const int* lens, int B, const float* z,

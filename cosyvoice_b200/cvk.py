@@ -63,6 +63,8 @@ SIGNATURES = {
     "cvk_hift_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp, _c_int_p, _vp, _vp, _vp]),
     "cvk_flow_encoder": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_cfm_estimator": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
+    "cvk_flow_encoder_hidden": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
+    "cvk_cfm_estimator_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_cfm_estimator_inplace": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp]),
     "cvk_workspace_bytes": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)]),
     "cvk_cfm_solve": (ctypes.c_int, [_vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_float, ctypes.c_int, _vp, _vp]),
@@ -384,6 +386,26 @@ class Context:
         h = torch.empty(rows, 512, device=self.device)
         self._check(self.lib.cvk_flow_encoder(self.h, _ptr(tokens), _ints(lens), len(lens), int(streaming), context_len, _ptr(h), _stream()))
         return h
+
+    def flow_encoder_hidden(self, tokens, lens, n_layers, enc_blocks, streaming=False, context_len=0):
+        """parity tests: the encoder's fp32 residual stream after n_layers units (0: embedding + PreLookahead, then one per
+        conformer layer, enc_blocks + 1: up_layer + up_embed, then one per up layer); [sum T - context_len, 512] up to enc_blocks
+        (the loaded model's), [sum 2 (T - context_len), 512] after; same inputs as flow_encoder"""
+        tokens = tokens.to(device=self.device, dtype=torch.int32).contiguous()
+        rate = 1 if n_layers <= enc_blocks else 2
+        h = torch.empty(max(1, sum(rate * (int(l) - context_len) for l in lens)), 512, device=self.device)
+        self._check(self.lib.cvk_flow_encoder_hidden(self.h, _ptr(tokens), _ints(lens), len(lens), int(streaming), context_len,
+                                                     int(n_layers), _ptr(h), _stream()))
+        return h
+
+    def cfm_estimator_hidden(self, x, mu, t, spks, cond, lens, n_units, streaming=False):
+        """parity tests: the estimator's fp32 residual stream [sum T, 256] after n_units units (a stage's resnet or one of its
+        transformer blocks, in execution order; 1 <= n_units <= n_stages * (1 + n_blocks)); same inputs as cfm_estimator"""
+        x, mu, t, spks, cond = (_f32(a, self.device) for a in (x, mu, t, spks, cond))
+        out = torch.empty(x.shape[0], 256, device=self.device)
+        self._check(self.lib.cvk_cfm_estimator_hidden(self.h, _ptr(x), _ptr(mu), _ptr(t), _ptr(spks), _ptr(cond), _ints(lens),
+                                                      len(lens), int(streaming), int(n_units), _ptr(out), _stream()))
+        return out
 
     def cfm_estimator(self, x, mu, t, spks, cond, lens, streaming=False):
         x, mu, t, spks, cond = (_f32(a, self.device) for a in (x, mu, t, spks, cond))

@@ -207,6 +207,19 @@ int cvk_flow_encoder(cvk_ctx* ctx, const int32_t* tokens, const int* lens_host, 
  * x, mu, cond [sum T,80]; t [B]; spks [B,80]; out [sum T,80]; mask = ones within each length. */
 int cvk_cfm_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
                       const int* lens_host, int B, int streaming, float* out, void* stream);
+/* parity tests: the arguments of cvk_flow_encoder, but the call stops after the first n_layers units and writes the fp32 residual
+ * stream to `hidden` instead of h.  Unit 0 is the token embedding, embed and the PreLookahead layer; units 1 .. enc_blocks the
+ * conformer layers (hidden [sum (N - context_len), 512], token rate); unit enc_blocks + 1 up_layer and up_embed, each later one an
+ * up layer (hidden [sum 2 (N - context_len), 512]).  after_norm is not applied.  An n_layers outside
+ * [0, enc_blocks + 1 + enc_up_blocks] is refused before any device work. */
+int cvk_flow_encoder_hidden(cvk_ctx* ctx, const int32_t* tokens, const int* lens_host, int B, int streaming, int context_len,
+                            int n_layers, float* hidden, void* stream);
+/* parity tests: the arguments of cvk_cfm_estimator, but the call stops after the first n_units units and writes the fp32 residual
+ * stream [sum T, 256] to `hidden` instead of the estimator output.  A unit is one stage's resnet or one of its transformer blocks,
+ * in execution order (down, mid 0 .. num_mid - 1, up); down_blocks.0.2 runs with the first mid-stage resnet.  An n_units outside
+ * [1, (num_mid + 2) * (1 + n_blocks)] is refused before any device work. */
+int cvk_cfm_estimator_hidden(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,
+                             const int* lens_host, int B, int streaming, int n_units, float* hidden, void* stream);
 /* the engine contract itself (flow/flow_matching.py:140-148: the last binding of the TensorRT context is x.data_ptr(), the
  * result overwrites x).  `out` of cvk_cfm_estimator may alias `x` as well: x is consumed before the first write. */
 int cvk_cfm_estimator_inplace(cvk_ctx* ctx, float* x, const float* mu, const float* t, const float* spks, const float* cond,

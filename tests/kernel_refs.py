@@ -475,3 +475,360 @@ DIT_TOL = {"fp32": dict(embed=2e-5, block=2.5e-4), "bf16": dict(embed=5e-3, bloc
 # 1.3e-2 / 1.2e-2.  Bounds about twice that.
 DIT_STACK_TOL = {"fp32": {"exact": (2.5e-4, 2e-4), "bf16-emulating": (0.03, 0.025)},
                  "bf16": {"exact": (0.025, 0.025), "bf16-emulating": (0.03, 0.025)}}
+
+
+# ------------------------------------------------------------------------------------------------ CosyVoice2 flow
+# The conformer encoder and the causal U-Net estimator of oracle/flow.py (flow/flow.py:235-281 of the reference) restated on the
+# packed time-major rows the kernels use, in fp64, one unit at a time: the encoder's input embedding with the PreLookahead layer
+# (enc_embed), one conformer layer (enc_layer), the x2 up-sampling with up_embed (enc_upsample) and after_norm; the estimator's time
+# embedding with every per-stage projection (est_time), one stage resnet (est_resnet), one transformer block (est_tblock) and the
+# tail (est_tail).  rounding=True emulates the bf16 path: the values it stores as bf16 (or rounds to bf16 on chip) and reads again
+# are rounded at the same points (FLOW_ROUNDING), and the tensor-core weights are taken as bf16.  `mutate` applies one of
+# FLOW_MUTATIONS, the defects the sensitivity test of test_kernel_refs_cpu.py injects.
+from oracle import flow as oflow  # noqa: E402
+
+FLOW_D, FLOW_C = oflow.D_ENC, oflow.C_EST
+FLOW_ROUNDING = {
+    # encoder: token rows written as the embed Linear's operand, embed output as the PreLookahead operand, its leaky-ReLU output,
+    # LN1 / LN2 outputs, the qkv projection, the position table and its projection, q + pos_bias_u / v, the attention output, the
+    # SiLU hidden, the residual stream as the up-sampler's operand and the up-sampler's output
+    "enc": ("emb", "h0a", "c1", "xn", "qkv", "pe", "pos", "quv", "att", "ff", "xa", "up"),
+    # estimator: the packed [x | mu | spks | cond] input, LN-Mish + temb of each resnet's first block, LN1 / LN3 outputs, qkv, the
+    # attention output, the GELU hidden (on chip in the fused feed-forward), the bf16 copy of every stage output that the next stage
+    # and the skip read, the down_blocks.0.2 output, and the tail's up_blocks.0.2 output and LN-Mish
+    "est": ("in", "h1", "xn", "qkv", "att", "ff", "act", "xa", "tail"),
+}
+FLOW_MUTATIONS = {
+    "est": ("chunk48", "chunk_edge", "temb_neighbour", "temb_before_mish", "skip_swap", "centred_pad", "silu_for_mish", "gelu_tanh",
+            "time_div", "ln_eps"),
+    "enc": ("pos_bias_swap", "rel_shift", "chunk24", "lookahead2", "up_pad3", "no_sqrt", "ln_eps"),
+}
+
+
+def flow_weights(sd, cfg):
+    """the flow's weights in fp64 (oracle.flow.param_shapes names, without the "flow." prefix), with the config"""
+    W = {k: v.double() for k, v in sd.items()}
+    W["cfg"] = cfg
+    return W
+
+
+def _rdw(rounding):
+    return bf16 if rounding else (lambda t: t)
+
+
+def _ln(x, g, b, eps):
+    return _layer_norm(x, eps) * g + b
+
+
+def _seq_conv(x, w, b, lens, shift0):
+    """a conv-GEMM on packed rows, sequence by sequence (rows outside a sequence read as zero): x [sum T, K], w [N, K, taps]"""
+    outs, o = [], 0
+    for L in lens:
+        outs.append(conv_rows(x[o:o + L], w, 1, shift0) + b)
+        o += L
+    return torch.cat(outs, 0)
+
+
+def _enc_in(W, p, x, rounding, mutate):
+    """LinearNoSubsampling + scaled positional input (subsampling.py:92-113, embedding.py:270-272): Linear -> LN(1e-5) -> x sqrt(512)"""
+    y = x @ _rdw(rounding)(W[p + ".out.0.weight"]).t() + W[p + ".out.0.bias"]
+    y = _ln(y, W[p + ".out.1.weight"], W[p + ".out.1.bias"], 1e-5)
+    return y if mutate == "no_sqrt" else y * math.sqrt(FLOW_D)
+
+
+def enc_embed(W, tokens, lens, context_len=0, rounding=False, mutate=None):
+    """token embedding -> embed -> PreLookaheadLayer (upsample_encoder.py:82-103: k4 convolution over the next 3 rows, which are
+    the context rows or zeros, leaky ReLU 0.01, causal k3 convolution, + input).  tokens [sum T] (context included); returns dict
+    h0 (embed output, every row) and x [sum (T - context_len), 512], the stream entering the first conformer layer."""
+    rd = bf16 if rounding else (lambda t: t)
+    p = "encoder.pre_lookahead_layer."
+    emb = rd(W["input_embedding.weight"][tokens.long().clamp(min=0)])
+    h0 = _enc_in(W, "encoder.embed", emb, rounding, mutate)
+    w1, w2 = _rdw(rounding)(W[p + "conv1.weight"]), _rdw(rounding)(W[p + "conv2.weight"])
+    xs, o = [], 0
+    for L in lens:
+        Lo = L - context_len
+        a = rd(h0[o:o + L])
+        c1 = rd(act("lrelu", conv_rows(a, w1, 1, -1 if mutate == "lookahead2" else 0)[:Lo] + W[p + "conv1.bias"], 0.01))
+        xs.append(conv_rows(c1, w2, 1, -2) + W[p + "conv2.bias"] + h0[o:o + Lo])
+        o += L
+    return dict(h0=h0, x=torch.cat(xs, 0))
+
+
+def rel_pos_table(T, extra=0):
+    """the ESPnet relative position table (embedding.py:224-254) in fp64: rows m = 0 .. 2(T + extra) - 2 hold relative position
+    r = T + extra - 1 - m: pe[2i] = sin(r w_i), pe[2i+1] = cos(r w_i), w_i = 10000^(-2i/512)"""
+    n = T + extra
+    r = torch.arange(n - 1, -n, -1, dtype=torch.float64)[:, None]
+    w = torch.exp(torch.arange(0, FLOW_D, 2, dtype=torch.float64) * -(math.log(10000.0) / FLOW_D))
+    pe = torch.zeros(2 * n - 1, FLOW_D, dtype=torch.float64)
+    pe[:, 0::2], pe[:, 1::2] = torch.sin(r * w), torch.cos(r * w)
+    return pe
+
+
+def enc_layer(W, p, x, lens, chunk, rounding=False, mutate=None):
+    """ConformerEncoderLayer (encoder_layer.py:160-236: LN 1e-12, relative-position MHA with pos_bias_u / v, SiLU feed-forward) on
+    packed rows x [sum T, 512]; p the layer's prefix ("encoder.encoders.i" / "encoder.up_encoders.i"); chunk 0 or the block-causal
+    chunk (25 tokens, 50 after the up-sampler).  The position table is sized by the longest sequence, as the kernels size it."""
+    rd = bf16 if rounding else (lambda t: t)
+    wt = _rdw(rounding)
+    a = p + ".self_attn."
+    eps = 1e-5 if mutate == "ln_eps" else 1e-12
+    x = x.double()
+    xn = rd(_ln(x, W[p + ".norm_mha.weight"], W[p + ".norm_mha.bias"], eps))
+    wqkv = torch.cat([W[a + f"linear_{n}.weight"] for n in "qkv"])
+    bqkv = torch.cat([W[a + f"linear_{n}.bias"] for n in "qkv"])
+    qkv = rd(xn @ wt(wqkv).t() + bqkv)
+    T = max(lens)
+    pe = rd(rel_pos_table(T, 1 if mutate == "rel_shift" else 0))      # rel_shift: every relative position read one too far
+    pos = rd(pe @ wt(W[a + "linear_pos.weight"]).t())
+    bu, bv = W[a + "pos_bias_u"].reshape(-1), W[a + "pos_bias_v"].reshape(-1)
+    if mutate == "pos_bias_swap":
+        bu, bv = bv, bu
+    q, k, v = qkv.split(FLOW_D, -1)
+    if rounding:       # the wgmma kernel reads q + u and q + v as bf16
+        qu, qv = bf16(q + bu), bf16(q + bv)
+        att64 = _relpos_att_split(qu, qv, k, v, pos, T - 1, lens, 24 if mutate == "chunk24" else chunk)
+    else:
+        att64 = relpos_attention(q, k, v, pos, T - 1, bu, bv, lens, 8, 24 if mutate == "chunk24" else chunk, 0.125)
+    att = rd(att64)
+    x_mid = x + att @ wt(W[a + "linear_out.weight"]).t() + W[a + "linear_out.bias"]
+    xn2 = rd(_ln(x_mid, W[p + ".norm_ff.weight"], W[p + ".norm_ff.bias"], eps))
+    ff = rd(act("silu", xn2 @ wt(W[p + ".feed_forward.w_1.weight"]).t() + W[p + ".feed_forward.w_1.bias"]))
+    x_out = x_mid + ff @ wt(W[p + ".feed_forward.w_2.weight"]).t() + W[p + ".feed_forward.w_2.bias"]
+    return dict(x=x, xn=xn, qkv=qkv, pos=pos, att=att, x_mid=x_mid, xn2=xn2, ff=ff, x_out=x_out)
+
+
+def _relpos_att_split(qu, qv, k, v, pos, center, lens, chunk):
+    """relpos_attention with q + u and q + v given separately (already rounded as the bf16 path stores them)"""
+    ac_att = []
+    o = 0
+    for L in lens:
+        qq, qqv, kk, vv = (t[o:o + L].view(L, 8, HD).transpose(0, 1) for t in (qu, qv, k, v))
+        pp = pos[center - (L - 1):center + L].view(2 * L - 1, 8, HD).transpose(0, 1)
+        s = (qq @ kk.transpose(1, 2) + rel_shift(qqv @ pp.transpose(1, 2))) * 0.125
+        s = s.masked_fill(~visible(L, L, 0, chunk)[None], float("-inf"))
+        ac_att.append((torch.softmax(s, -1) @ vv).transpose(0, 1).reshape(L, FLOW_D))
+        o += L
+    return torch.cat(ac_att, 0)
+
+
+def enc_upsample(W, x, lens, rounding=False, mutate=None):
+    """Upsample1D (upsample_encoder.py:59-63: nearest x2, left pad 4, k5 convolution) and up_embed on packed token rows
+    x [sum T, 512] -> [sum 2T, 512].  The kernels fold the x2 repeat into a 3-tap polyphase convolution on the token rows whose
+    weights are sums of taps (flow.cu upsample_poly_kernel); the bf16 path holds those sums as bf16, so they are rounded here."""
+    rd = bf16 if rounding else (lambda t: t)
+    w, b = W["encoder.up_layer.conv.weight"], W["encoder.up_layer.conv.bias"]
+    xa = rd(x.double())
+    outs, o = [], 0
+    for L in lens:
+        if mutate == "up_pad3":
+            u = xa[o:o + L].repeat_interleave(2, 0)
+            outs.append(conv_rows(u, w, 1, -3) + b)
+        else:
+            wp0 = torch.stack([w[..., 0] + w[..., 1], w[..., 2] + w[..., 3], w[..., 4]], -1)
+            wp1 = torch.stack([w[..., 0], w[..., 1] + w[..., 2], w[..., 3] + w[..., 4]], -1)
+            y = torch.stack([conv_rows(xa[o:o + L], _rdw(rounding)(wp), 1, -2) for wp in (wp0, wp1)], 1)   # [L, 2, 512]
+            outs.append(y.reshape(2 * L, FLOW_D) + b)
+        o += L
+    up = rd(torch.cat(outs, 0))
+    return dict(up=up, y=_enc_in(W, "encoder.up_embed", up, rounding, mutate))
+
+
+def enc_after_norm(W, y):
+    return _ln(y.double(), W["encoder.after_norm.weight"], W["encoder.after_norm.bias"], 1e-5)
+
+
+def flow_encoder(W, tokens, lens, streaming, context_len=0, rounding=False, n_layers=None, mutate=None):
+    """the composed encoder: returns (the residual stream after n_layers units (all by default; cvk_flow_encoder_hidden's units),
+    the encoder output (None when n_layers stops short))"""
+    cfg = W["cfg"]
+    n = cfg.enc_blocks + 1 + cfg.enc_up_blocks if n_layers is None else n_layers
+    lo = [L - context_len for L in lens]
+    h = enc_embed(W, tokens, lens, context_len, rounding, mutate)["x"]
+    for i in range(min(n, cfg.enc_blocks)):
+        h = enc_layer(W, f"encoder.encoders.{i}", h, lo, 25 if streaming else 0, rounding, mutate)["x_out"]
+    if n > cfg.enc_blocks:
+        h = enc_upsample(W, h, lo, rounding, mutate)["y"]
+        lo2 = [2 * L for L in lo]
+        for i in range(n - cfg.enc_blocks - 1):
+            h = enc_layer(W, f"encoder.up_encoders.{i}", h, lo2, 50 if streaming else 0, rounding, mutate)["x_out"]
+    full = n_layers is None or n_layers == cfg.enc_blocks + 1 + cfg.enc_up_blocks
+    return h, (enc_after_norm(W, h) if full else None)
+
+
+def est_stage_names(cfg):
+    e = "decoder.estimator."
+    return [e + "down_blocks.0"] + [e + f"mid_blocks.{i}" for i in range(cfg.num_mid_blocks)] + [e + "up_blocks.0"]
+
+
+def est_time(W, t, mutate=None):
+    """SinusoidalPosEmb(320) with scale 1000 (frequencies 10000^(-i/159)), TimestepEmbedding (Linear, SiLU, Linear), then every
+    stage resnet's mlp (Mish, Linear) in fp64: t [B] -> dict(a (the angles), sc, te, temb [B, n_stages, 256]).  The kernels keep
+    all of it in fp32 (fp32 weights, no bf16 rounding point)."""
+    e = "decoder.estimator."
+    half = 160
+    div = half if mutate == "time_div" else half - 1
+    fr = torch.exp(torch.arange(half, dtype=torch.float64) * -(math.log(10000.0) / div))
+    a = 1000.0 * t.double()[:, None] * fr[None]
+    sc = torch.cat([a.sin(), a.cos()], -1)
+    te = act("silu", sc @ W[e + "time_mlp.linear_1.weight"].t() + W[e + "time_mlp.linear_1.bias"])
+    te = te @ W[e + "time_mlp.linear_2.weight"].t() + W[e + "time_mlp.linear_2.bias"]
+    m = _mish(te)
+    temb = torch.stack([m @ W[s + ".0.mlp.1.weight"].t() + W[s + ".0.mlp.1.bias"] for s in est_stage_names(W["cfg"])], 1)
+    return dict(a=a, sc=sc, te=te, temb=temb)
+
+
+def est_resnet(W, k, xin, temb, lens, rounding=False, mutate=None):
+    """ResnetBlock1D of stage k (Matcha decoder.py:55-61 with CausalBlock1D, decoder.py:65-78): causal k3 convolution (2 zero rows in
+    front of every sequence), LN 1e-5, Mish, + the stage's time projection, the same again without it, + a 1x1 residual convolution
+    of the input.  xin [sum T, Cin] is the stage input as the kernels read it (the act operand); temb = est_time(...)["temb"]."""
+    rd = bf16 if rounding else (lambda t: t)
+    wt = _rdw(rounding)
+    nst = temb.shape[1]
+    p = est_stage_names(W["cfg"])[k] + ".0."
+    eps = 1e-6 if mutate == "ln_eps" else 1e-5
+    sh = -1 if mutate == "centred_pad" else -2
+    mish = (lambda v: act("silu", v)) if mutate == "silu_for_mish" else _mish
+    tv = temb[:, (k + 1) % nst if mutate == "temb_neighbour" else k][_seq_ids(lens)]
+    xin = xin.double()
+    c = _seq_conv(xin, wt(W[p + "block1.block.0.weight"]), W[p + "block1.block.0.bias"], lens, sh)
+    n1 = _ln(c, W[p + "block1.block.2.weight"], W[p + "block1.block.2.bias"], eps)
+    h1 = rd(mish(n1 + tv) if mutate == "temb_before_mish" else mish(n1) + tv)
+    c2 = _seq_conv(h1, wt(W[p + "block2.block.0.weight"]), W[p + "block2.block.0.bias"], lens, sh)
+    h2 = mish(_ln(c2, W[p + "block2.block.2.weight"], W[p + "block2.block.2.bias"], eps))
+    x_out = xin @ wt(W[p + "res_conv.weight"][..., 0]).t() + W[p + "res_conv.bias"] + h2
+    return dict(c=c, h1=h1, h2=h2, x_out=x_out)
+
+
+def est_tblock(W, k, j, x, lens, chunk, rounding=False, mutate=None):
+    """BasicTransformerBlock j of stage k (Matcha transformer.py:243-316 with diffusers Attention and GELU): LN 1e-5, q / k / v without
+    bias, 8 heads, scale 1/8, full or block-causal (chunk 50) attention, out projection + residual, LN 1e-5, Linear, exact-erf GELU,
+    Linear + residual.  x [sum T, 256] the residual stream."""
+    rd = bf16 if rounding else (lambda t: t)
+    wt = _rdw(rounding)
+    p = est_stage_names(W["cfg"])[k] + f".1.{j}."
+    eps = 1e-6 if mutate == "ln_eps" else 1e-5
+    x = x.double()
+    xn = rd(_ln(x, W[p + "norm1.weight"], W[p + "norm1.bias"], eps))
+    qkv = rd(xn @ wt(torch.cat([W[p + f"attn1.to_{n}.weight"] for n in "qkv"])).t())
+    ch = 48 if (mutate == "chunk48" and chunk) else chunk
+    outs, o = [], 0
+    for L in lens:
+        q, kk, v = (qkv[o:o + L, n * 512:(n + 1) * 512].reshape(L, 8, HD).transpose(0, 1) for n in range(3))
+        s = (q @ kk.transpose(1, 2)) * 0.125
+        s = s.masked_fill(~_dit_visible(L, ch, 1 if (mutate == "chunk_edge" and chunk) else 0)[None], float("-inf"))
+        outs.append((torch.softmax(s, -1) @ v).transpose(0, 1).reshape(L, 512))
+        o += L
+    att = rd(torch.cat(outs, 0))
+    x_mid = x + att @ wt(W[p + "attn1.to_out.0.weight"]).t() + W[p + "attn1.to_out.0.bias"]
+    xn3 = rd(_ln(x_mid, W[p + "norm3.weight"], W[p + "norm3.bias"], eps))
+    ff = rd(act("gelu_tanh" if mutate == "gelu_tanh" else "gelu", xn3 @ wt(W[p + "ff.net.0.proj.weight"]).t() + W[p + "ff.net.0.proj.bias"]))
+    x_out = x_mid + ff @ wt(W[p + "ff.net.2.weight"]).t() + W[p + "ff.net.2.bias"]
+    return dict(x=x, xn=xn, qkv=qkv, att=att, x_mid=x_mid, xn3=xn3, ff=ff, x_out=x_out)
+
+
+def est_down_conv(W, skip_act, lens, rounding=False, mutate=None):
+    """down_blocks.0.2: the causal k3 convolution from the down stage's output (its act copy) to the first mid stage's input"""
+    e = "decoder.estimator.down_blocks.0.2."
+    return (bf16 if rounding else (lambda t: t))(
+        _seq_conv(skip_act.double(), _rdw(rounding)(W[e + "weight"]), W[e + "bias"], lens, -1 if mutate == "centred_pad" else -2))
+
+
+def est_tail(W, up_act, lens, rounding=False, mutate=None):
+    """up_blocks.0.2 (causal k3), final_block (causal k3, LN 1e-5, Mish) and final_proj on the up stage's output (its act copy)"""
+    rd = bf16 if rounding else (lambda t: t)
+    wt = _rdw(rounding)
+    e = "decoder.estimator."
+    sh = -1 if mutate == "centred_pad" else -2
+    h1 = rd(_seq_conv(up_act.double(), wt(W[e + "up_blocks.0.2.weight"]), W[e + "up_blocks.0.2.bias"], lens, sh))
+    c = _seq_conv(h1, wt(W[e + "final_block.block.0.weight"]), W[e + "final_block.block.0.bias"], lens, sh)
+    mish = (lambda v: act("silu", v)) if mutate == "silu_for_mish" else _mish
+    xa = rd(mish(_ln(c, W[e + "final_block.block.2.weight"], W[e + "final_block.block.2.bias"], 1e-6 if mutate == "ln_eps" else 1e-5)))
+    return xa @ wt(W[e + "final_proj.weight"][..., 0]).t() + W[e + "final_proj.bias"]
+
+
+def est_pack(x, mu, cond, spks, lens, rounding=False):
+    """the estimator's packed input [x | mu | spks | cond] (decoder.py:431-434), as the bf16 path stores it"""
+    inp = torch.cat([x.double(), mu.double(), spks.double()[_seq_ids(lens)], cond.double()], -1)
+    return bf16(inp) if rounding else inp
+
+
+def est_stage_input(W, k, acts, lens, rounding=False, mutate=None):
+    """the act operand stage k reads, from the act copies acts[i] of the earlier stages' outputs: the packed input for the down
+    stage (acts[-1] holds it), down_blocks.0.2 of the down stage's output for the first mid stage, the previous stage's output for
+    the other mid stages, and [last mid output | down output] (the U-Net skip) for the up stage"""
+    nst = len(est_stage_names(W["cfg"]))
+    if k == 0:
+        return acts[-1]
+    down = est_down_conv(W, acts[0], lens, rounding, mutate) if (k == 1 or nst == 2) else None
+    if k < nst - 1:
+        return down if k == 1 else acts[k - 1]
+    mid = acts[k - 1] if nst > 2 else down
+    return torch.cat([acts[0], mid] if mutate == "skip_swap" else [mid, acts[0]], -1)
+
+
+def flow_estimator(W, x, mu, cond, spks, t, lens, streaming, rounding=False, n_units=None, mutate=None):
+    """the composed estimator on packed rows: returns (the residual stream after n_units units (all by default; the units of
+    cvk_cfm_estimator_hidden), the output [sum T, 80] (None when n_units stops short))"""
+    cfg = W["cfg"]
+    nst, per = cfg.num_mid_blocks + 2, 1 + cfg.n_blocks
+    n = nst * per if n_units is None else n_units
+    rd = bf16 if rounding else (lambda v: v)
+    temb = est_time(W, t, mutate)["temb"]
+    acts = {-1: est_pack(x, mu, cond, spks, lens, rounding)}
+    chunk = 50 if streaming else 0
+    done = 0
+    h = None
+    for k in range(nst):
+        h = est_resnet(W, k, est_stage_input(W, k, acts, lens, rounding, mutate), temb, lens, rounding, mutate)["x_out"]
+        done += 1
+        for j in range(cfg.n_blocks):
+            if done == n:
+                return h, None
+            h = est_tblock(W, k, j, h, lens, chunk, rounding, mutate)["x_out"]
+            done += 1
+        if done == n and k < nst - 1:
+            return h, None
+        acts[k] = rd(h)
+    return h, est_tail(W, acts[nst - 1], lens, rounding, mutate)
+
+
+def flow_test_state_dict(cfg, seed):
+    """CosyVoice2 flow weights for the block checks (oracle.flow.param_shapes names): fan-in-scaled matrices, so every resnet,
+    transformer block and conformer layer changes the residual stream by O(1); pos_bias_u / v of O(1) (the synthetic default,
+    0.1, leaves them under the noise of the content term); and every matrix the bf16 path streams as bf16 bf16-representable, so
+    both references see the kernels' weights.  The time MLP, the per-stage time projections and the speaker projection stay fp32,
+    as the kernels hold them."""
+    from oracle import weights as oweights
+    sd = oweights.synth_state_dict(oflow.param_shapes(cfg), seed, oflow.SYNTH_GAINS)
+    g = torch.Generator().manual_seed(seed)
+    for k in sd:
+        if "pos_bias_" in k:
+            sd[k] = torch.randn(sd[k].shape, generator=g)
+        elif sd[k].dim() >= 2 and "time_mlp" not in k and ".mlp.1." not in k and "spk_embed" not in k and k != "input_embedding.weight":
+            sd[k] = bf16(sd[k])
+    return sd
+
+
+# bounds of test_flow_blocks_gpu.py: largest |kernel - reference| of a unit over the rms of that row's contribution (encoder embedding,
+# up-sampler, estimator resnet: the unit's output; conformer layer, transformer block: x_out - x; after_norm and the estimator tail:
+# the output row).  Largest ratios measured on an H100 80GB HBM3 (700 W) over every layout, both masks and both contexts, in one run:
+#   fp32: embedding 6.9e-6, conformer layer 1.6e-5, up-sampler 6.1e-6, after_norm 1.1e-6, resnet 2.0e-5, block 5.9e-6, tail 4.9e-6.
+#     The fp32 sinusoids set that floor: the angles 1000 t 10000^(-i/159) (up to 950 rad) rounded to fp32 move the time projections
+#     by 1e-5 and the resnet by 1.6e-5 of its rms on their own (four fifths of the measured 2.0e-5, at 1500 frames); the position
+#     table's fp32 angles r 10000^(-2i/512) (r up to 749) move an up layer by 3.8e-6 on their own (a quarter of the layer's 1.6e-5).
+#   bf16 (against the bf16-emulating reference): embedding 2.4e-3, conformer layer 9.5e-3, up-sampler 3.8e-3, after_norm 9.9e-7 (an
+#     fp32 LayerNorm of the fp32 stream), resnet 4.3e-3, block 1.2e-2, tail 6.1e-3.
+# Each bound is about twice that.
+FLOW_TOL = {"fp32": dict(enc_embed=1.5e-5, enc_layer=3.5e-5, enc_up=1.2e-5, enc_out=2.5e-6, est_resnet=4e-5, est_block=1.2e-5,
+                         est_out=1e-5),
+            "bf16": dict(enc_embed=5e-3, enc_layer=0.02, enc_up=7.5e-3, enc_out=2.5e-6, est_resnet=9e-3, est_block=0.025,
+                         est_out=0.0125)}
+# full config (6, 4, 12, 4): largest error over the mean row rms of the reference, (encoder hidden, encoder output, estimator hidden
+# after 70 units, estimator output), per reference, offline and streaming.  Measured, same run: fp32 vs exact 6.8e-6 / 7.1e-6 /
+# 1.2e-5 / 1.3e-5, fp32 vs bf16-emulating 1.9e-2 / 2.2e-2 / 2.9e-2 / 3.6e-2, bf16 vs exact 2.0e-2 / 2.1e-2 / 3.1e-2 / 4.0e-2, bf16
+# vs bf16-emulating 1.2e-2 / 1.2e-2 / 3.9e-2 / 4.7e-2 (over 70 units the two bf16 trajectories drift apart as far as each drifts
+# from the exact one).  Bounds about twice that.
+FLOW_STACK_TOL = {"fp32": {"exact": (1.5e-5, 1.5e-5, 2.5e-5, 2.5e-5), "bf16-emulating": (0.04, 0.045, 0.06, 0.075)},
+                  "bf16": {"exact": (0.04, 0.04, 0.06, 0.08), "bf16-emulating": (0.025, 0.025, 0.08, 0.095)}}

@@ -395,3 +395,185 @@ def test_dit_mutations_exceed_bounds(precision):
             assert shares[m] < 0.1, (m, shares[m])
         else:
             assert shares[m] >= need, (m, shares[m], need)
+
+
+# ================================================================================================ CosyVoice2 flow references
+FLOW_SMALL = oflow.FlowCfg(2, 2, 2, 2)
+
+
+def _flow_w(cfg=FLOW_SMALL, seed=23):
+    sd = kr.flow_test_state_dict(cfg, seed)
+    return sd, kr.flow_weights(sd, cfg)
+
+
+def _est_case(lens, seed):
+    g = torch.Generator().manual_seed(seed)
+    R = sum(lens)
+    x, mu, cond = (kr.bf16(torch.rand(R, 80, generator=g) * 2 - 1) for _ in range(3))
+    t = (0.05 + 0.9 * torch.rand(len(lens), generator=g)).double()
+    return x, mu, cond, kr.bf16(torch.randn(len(lens), 80, generator=g)), t
+
+
+@pytest.mark.parametrize("context_len", [0, 3])
+@pytest.mark.parametrize("streaming", [False, True])
+def test_flow_encoder_ref_equals_oracle(streaming, context_len):
+    """kr.flow_encoder (exact; the units composed) == oracle.flow.encoder on every utterance of a ragged pack, with the look-ahead
+    context passed to the oracle separately, as flow.py:259-261 passes it"""
+    sd, W = _flow_w()
+    lens = [37 + context_len, 5 + context_len, 60 + context_len]
+    g = torch.Generator().manual_seed(3)
+    tok = torch.randint(0, 6561, (sum(lens),), generator=g)
+    _, got = kr.flow_encoder(W, tok, lens, streaming, context_len)
+    o = oo = 0
+    for L in lens:
+        x = F.embedding(tok[o:o + L].long()[None], sd["input_embedding.weight"])
+        Lo = L - context_len
+        want = oflow.encoder(sd, x[:, :Lo], FLOW_SMALL, streaming, context=x[:, Lo:] if context_len else None)[0].double()
+        assert (got[oo:oo + 2 * Lo] - want).abs().max().item() < 1e-4, L       # fp32 oracle, after_norm output of O(1)
+        o += L
+        oo += 2 * Lo
+
+
+@pytest.mark.parametrize("streaming", [False, True])
+def test_flow_estimator_ref_equals_oracle(streaming):
+    """kr.flow_estimator (exact; the units, down_blocks.0.2, the skip and the tail composed) == oracle.flow.estimator on every sequence
+    of a ragged pack, and a CFG pair (zero mu / spks / cond in its second sequence) sequence by sequence"""
+    sd, W = _flow_w()
+    lens = [70, 1, 51, 51]
+    x, mu, cond, spks, t = _est_case(lens, 4)
+    mu[-51:], cond[-51:], spks[-1] = 0.0, 0.0, 0.0
+    x[-51:] = x[-102:-51]
+    _, got = kr.flow_estimator(W, x, mu, cond, spks, t, lens, streaming)
+    o = 0
+    for b, L in enumerate(lens):
+        cm = lambda a: a[o:o + L].t()[None]
+        want = oflow.estimator(sd, cm(x), torch.ones(1, 1, L), cm(mu), t[b:b + 1].float(), spks[b:b + 1], cm(cond), FLOW_SMALL,
+                               streaming)[0].t().double()
+        assert (got[o:o + L] - want).abs().max().item() < 1e-4, (b, L)          # fp32 oracle on O(1) values
+        o += L
+
+
+@pytest.mark.parametrize("tag,cfg", [("small", oflow.FlowCfg(2, 1, 2, 2)), ("full", oflow.FlowCfg())])
+def test_flow_ref_composed_equals_golden(golden, tag, cfg):
+    """the fp64 pieces composed (kr.flow_encoder, kr.flow_estimator) == the reference flow's encoder and estimator outputs in
+    tests/golden/flow_{small,full}.npz (the synthetic weights, cases.flow_case / cases.estimator_case) within the export tolerance
+    (rtol 1e-2, atol 1e-4)"""
+    import numpy as np
+    gd = golden("flow_" + tag)
+    sd = oweights.synth_state_dict(oflow.param_shapes(cfg), 1986, oflow.SYNTH_GAINS)
+    W = kr.flow_weights(sd, cfg)
+    token, ptok, _, _ = cases.flow_case()
+    tok = torch.cat([ptok, token], 1)[0]
+    _, h = kr.flow_encoder(W, tok, [tok.numel()], False)
+    np.testing.assert_allclose(h.numpy(), gd["enc_offline"][0].astype(np.float64), rtol=1e-2, atol=1e-4)
+    x, mask, mu, t, spks, cond = cases.estimator_case()
+    T = x.shape[2]
+    tm = lambda a: a.transpose(1, 2).reshape(-1, a.shape[1])
+    for streaming, key in ((False, "est_offline"), (True, "est_stream")):
+        _, out = kr.flow_estimator(W, tm(x), tm(mu), tm(cond), spks, t.double(), [T] * x.shape[0], streaming)
+        np.testing.assert_allclose(out.numpy(), tm(torch.from_numpy(gd[key])).double().numpy(), rtol=1e-2, atol=1e-4)
+
+
+def test_flow_rounding_points():
+    """rounding=True stores bf16 exactly at the FLOW_ROUNDING points (and nowhere else); rounding=False nowhere"""
+    sd, W = _flow_w()
+    is_b = lambda v: torch.equal(v, kr.bf16(v))
+    lens = [40, 9]
+    x, mu, cond, spks, t = _est_case(lens, 5)
+    temb = kr.est_time(W, t)["temb"]
+    tok = torch.randint(0, 6561, (sum(lens),), generator=torch.Generator().manual_seed(6))
+    for rounding in (True, False):
+        inp = kr.est_pack(x + 1e-3, mu, cond, spks, lens, rounding)
+        rn = kr.est_resnet(W, 0, inp, temb, lens, rounding)
+        tb = kr.est_tblock(W, 0, 0, rn["x_out"], lens, 50, rounding)
+        acts = {-1: inp, 0: kr.bf16(tb["x_out"]) if rounding else tb["x_out"]}
+        xa = kr.est_stage_input(W, 1, acts, lens, rounding)
+        stored = [inp, rn["h1"], tb["xn"], tb["qkv"], tb["att"], tb["xn3"], tb["ff"], xa]
+        assert all(is_b(v) == rounding for v in stored), rounding
+        assert not any(is_b(v) for v in (rn["c"], rn["h2"], rn["x_out"], tb["x_mid"], tb["x_out"], temb)), rounding
+        e = kr.enc_embed(W, tok, lens, 3, rounding)
+        el = kr.enc_layer(W, "encoder.encoders.0", e["x"], [37, 6], 25, rounding)
+        up = kr.enc_upsample(W, el["x_out"], [37, 6], rounding)
+        assert all(is_b(v) == rounding for v in (el["xn"], el["qkv"], el["pos"], el["att"], el["xn2"], el["ff"], up["up"])), rounding
+        assert not any(is_b(v) for v in (e["h0"], e["x"], el["x_mid"], el["x_out"], up["y"])), rounding
+
+
+def _flow_mutation_shares(precision):
+    """share of the elements that each defect of kr.FLOW_MUTATIONS, injected into the reference of its mode (exact for fp32,
+    bf16-emulating for bf16), moves beyond the per-element bound test_flow_blocks_gpu.py holds the kernels to (kr.FLOW_TOL), on a
+    ragged pair with the streaming masks.  Each defect is judged on the unit it lives in, fed the unmutated reference's input, over
+    the rms of that unit's contribution, as the GPU test judges the kernels."""
+    bf = precision == "bf16"
+    tol = kr.FLOW_TOL[precision]
+    _, W = _flow_w()
+    rms = lambda v: v.pow(2).mean(-1, keepdim=True).sqrt()
+    share = lambda d, scale, bound: ((d.abs() / scale) > bound).double().mean().item()
+    shares = {}
+    # estimator: stage 1 (the first mid stage: down_blocks.0.2, resnet, block 0) and the up stage's resnet on the skip
+    lens = [130, 70]
+    x, mu, cond, spks, t = _est_case(lens, 3)
+    temb = kr.est_time(W, t)["temb"]
+    acts = {-1: kr.est_pack(x, mu, cond, spks, lens, bf)}
+    g = torch.Generator().manual_seed(8)
+    acts[0] = kr.bf16(torch.randn(sum(lens), 256, generator=g))
+    acts[1], acts[2] = (kr.bf16(torch.randn(sum(lens), 256, generator=g)) for _ in range(2))
+    nst = FLOW_SMALL.num_mid_blocks + 2
+    for m in kr.FLOW_MUTATIONS["est"]:
+        if m in ("chunk48", "chunk_edge", "gelu_tanh"):
+            h = kr.est_resnet(W, 1, kr.est_stage_input(W, 1, acts, lens, bf), temb, lens, bf)["x_out"]
+            ref, mut = (kr.est_tblock(W, 1, 0, h, lens, 50, bf, mutate=mm) for mm in (None, m))
+            shares[m] = share(mut["x_out"] - ref["x_out"], rms(ref["x_out"] - ref["x"]), tol["est_block"])
+        elif m == "skip_swap":
+            ref, mut = (kr.est_resnet(W, nst - 1, kr.est_stage_input(W, nst - 1, acts, lens, bf, mutate=mm), temb, lens, bf)["x_out"]
+                        for mm in (None, m))
+            shares[m] = share(mut - ref, rms(ref), tol["est_resnet"])
+        else:
+            tm = kr.est_time(W, t, mutate=m)["temb"] if m == "time_div" else temb
+            mm = None if m == "time_div" else m
+            ref = kr.est_resnet(W, 1, kr.est_stage_input(W, 1, acts, lens, bf), temb, lens, bf)["x_out"]
+            mut = kr.est_resnet(W, 1, kr.est_stage_input(W, 1, acts, lens, bf, mutate=mm), tm, lens, bf, mutate=mm)["x_out"]
+            shares[m] = share(mut - ref, rms(ref), tol["est_resnet"])
+    # encoder: the embedding, conformer layer 0 (token rate, chunk 25), the up-sampler
+    tl = [60 + 3, 23 + 3]
+    tok = torch.randint(0, 6561, (sum(tl),), generator=torch.Generator().manual_seed(9))
+    lo = [60, 23]
+    e = kr.enc_embed(W, tok, tl, 3, bf)["x"]
+    for m in kr.FLOW_MUTATIONS["enc"]:
+        if m in ("lookahead2", "no_sqrt"):
+            mut = kr.enc_embed(W, tok, tl, 3, bf, mutate=m)["x"]
+            shares["enc_" + m] = share(mut - e, rms(e), tol["enc_embed"])
+        elif m == "up_pad3":
+            ref, mut = (kr.enc_upsample(W, e, lo, bf, mutate=mm)["y"] for mm in (None, m))
+            shares["enc_" + m] = share(mut - ref, rms(ref), tol["enc_up"])
+        else:
+            ref, mut = (kr.enc_layer(W, "encoder.encoders.0", e, lo, 25, bf, mutate=mm) for mm in (None, m))
+            shares["enc_" + m] = share(mut["x_out"] - ref["x_out"], rms(ref["x_out"] - ref["x"]), tol["enc_layer"])
+    return shares
+
+
+# share of the elements beyond the GPU bound that each defect must move in each mode; None: not caught in that mode (its share stays
+# under 0.1).  Measured on this case: fp32 0.6 - 1.0 for every structural defect and 0.94 for the tanh GELU, 0.002 and 0 for the
+# LayerNorm eps changes; bf16 0.31 - 0.99 for the structural defects, 0 for the tanh GELU (the bf16 path's own GELU is the tanh form
+# on a half-precision tanh, within 5e-4 of the erf) and for both eps changes.
+FLOW_CAUGHT = {
+    "fp32": dict(chunk48=0.5, chunk_edge=0.5, temb_neighbour=0.5, temb_before_mish=0.5, skip_swap=0.5, centred_pad=0.5, silu_for_mish=0.5,
+                 gelu_tanh=0.5, time_div=0.5, ln_eps=None, enc_pos_bias_swap=0.5, enc_rel_shift=0.5, enc_chunk24=0.3, enc_lookahead2=0.5,
+                 enc_up_pad3=0.5, enc_no_sqrt=0.5, enc_ln_eps=None),
+    "bf16": dict(chunk48=0.2, chunk_edge=0.15, temb_neighbour=0.5, temb_before_mish=0.4, skip_swap=0.5, centred_pad=0.5, silu_for_mish=0.5,
+                 gelu_tanh=None, time_div=0.4, ln_eps=None, enc_pos_bias_swap=0.5, enc_rel_shift=0.4, enc_chunk24=0.2, enc_lookahead2=0.5,
+                 enc_up_pad3=0.5, enc_no_sqrt=0.5, enc_ln_eps=None),
+}
+
+
+@pytest.mark.parametrize("precision", ["fp32", "bf16"])
+def test_flow_mutations_exceed_bounds(precision):
+    """each defect of kr.FLOW_MUTATIONS moves at least the stated share of its unit's elements beyond the bound of its mode; the
+    defects a mode does not claim stay under a share of 0.1, so the claim list is exact"""
+    shares = _flow_mutation_shares(precision)
+    print(precision, {k: round(v, 3) for k, v in shares.items()})
+    assert set(FLOW_CAUGHT[precision]) == set(shares)
+    for m, need in FLOW_CAUGHT[precision].items():
+        if need is None:
+            assert shares[m] < 0.1, (m, shares[m])
+        else:
+            assert shares[m] >= need, (m, shares[m], need)
