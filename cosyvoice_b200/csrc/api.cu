@@ -553,12 +553,12 @@ int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, in
 }
 
 int cvk_op_flow_ff(cvk_ctx* ctx, float* x, int rows, const int* seq_start, const int* seq_len, int B, const float* ln3_g, const float* ln3_b,
-                   const float* w1, const float* b1, const float* w2, const float* b2, const float* ln_g, const float* ln_b, float* out,
-                   void* stream) {
+                   const float* w1, const float* b1, const float* w2, const float* b2, const float* ln_g, const float* ln_b, const float* att,
+                   const float* wo, const float* bo, float* out, void* stream) {
   CVK_API_BEGIN
   cudaStream_t st = (cudaStream_t)stream;
   CVK_REQUIRE(x && rows >= 1 && seq_start && seq_len && B >= 1 && ln3_g && ln3_b && w1 && b1 && w2 && b2 && (!ln_g) == (!ln_b) && out &&
-                  ((uintptr_t)x & 15) == 0,
+                  ((uintptr_t)x & 15) == 0 && (!att) == (!wo) && (!att) == (!bo),
               "cvk_op_flow_ff: bad arguments");
   std::vector<int> row2seq(rows, -1);
   for (int b = 0; b < B; ++b) {
@@ -577,13 +577,20 @@ int cvk_op_flow_ff(cvk_ctx* ctx, float* x, int rows, const int* seq_start, const
   };
   try {
     const ConvW W1 = make_conv(ctx, w1, b1, 1024, 256, 1, 1, 0), W2 = make_conv(ctx, w2, b2, 256, 1024, 1, 1, 0);
+    ConvW Wo;
+    if (att) Wo = make_conv(ctx, wo, bo, 256, 512, 1, 1, 0);
     CVK_CHECK_CUDA(cudaDeviceSynchronize());   // weight repack runs on the default stream
     int* d_row2seq = (int*)ctx->arena.alloc(sizeof(int) * (size_t)rows);
     CVK_CHECK_CUDA(cudaMemcpyAsync(d_row2seq, row2seq.data(), sizeof(int) * (size_t)rows, cudaMemcpyHostToDevice, st));
     const int adt = ctx->act_dtype;
     Mat o = arena_mat(ctx, adt, rows, 256), xn = arena_mat(ctx, adt, rows, 256), hid = arena_mat(ctx, adt, rows, 1024);
+    Mat am;
+    if (att) {
+      am = arena_mat(ctx, adt, rows, 512);
+      convert_mat(ctx, st, Mat(const_cast<float*>(att), DT_F32, rows, 512, 512), am);
+    }
     const Mat xm(x, DT_F32, rows, 256, 256);
-    flow_ff(ctx, st, xm, d_row2seq, ln3_g, ln3_b, W1, W2, ln_g, ln_b, o, xn, hid);
+    flow_ff(ctx, st, xm, att ? &am : nullptr, att ? &Wo : nullptr, d_row2seq, ln3_g, ln3_b, W1, W2, ln_g, ln_b, o, xn, hid);
     convert_mat(ctx, st, o, Mat(out, DT_F32, rows, 256, 256));
     CVK_CHECK_CUDA(cudaStreamSynchronize(st));
   } catch (...) {

@@ -273,15 +273,20 @@ float* dev_copy_f32(cvk_ctx* ctx, const float* src_dev, size_t n);
 void conv_gemm(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_simt(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
 void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep);
-// flow-estimator feed-forward in one launch (gemm_tc.cu): x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0 in place (x fp32 [rows, 256],
-// ff1 256 -> 1024, ff2 1024 -> 256), then out (bf16 [rows, 256]) <- LN1 of the next block (ln_g, ln_b) or, with ln_g null, x itself
-void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& w1,
-               const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out);
-// x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0, then out <- LN(x; ln_g, ln_b) or, with ln_g null, x in out's dtype (flow.cu): the
-// feed-forward half of a flow-estimator transformer block and the first operand of the next one.  ffn_fused in the bf16 mode with
-// option "flow_fused_ff", otherwise LN3, ff1 and ff2 (+ LN) launches with xn [rows, 256] and hid [rows, 1024] (act dtype) as scratch.
-void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& ff1,
-             const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn, const Mat& hid);
+// flow-estimator feed-forward in one launch (gemm_tc.cu): with att (bf16 [rows, 512]) and wo (the attention output projection
+// 512 -> 256) first x <- valid(r) ? x + bo + att wo^T : 0, then x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0 in place (x fp32
+// [rows, 256], ff1 256 -> 1024, ff2 1024 -> 256), then out (bf16 [rows, 256]) <- LN1 of the next block (ln_g, ln_b) or, with ln_g
+// null, x itself.  att and wo null: x is taken as given.
+void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat* att, const ConvW* wo, const int* row2seq, const float* ln3_g,
+               const float* ln3_b, const ConvW& w1, const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out);
+// With att (act dtype [rows, 512]) and wo: x <- valid(r) ? x + bo + att wo^T : 0 (the attention output projection and its residual);
+// then x <- valid(r) ? x + ff2(GELU(ff1(LN3(x)))) : 0, then out <- LN(x; ln_g, ln_b) or, with ln_g null, x in out's dtype (flow.cu):
+// the rest of a flow-estimator transformer block after its attention and the first operand of the next one.  ffn_fused in the bf16
+// mode with option "flow_fused_ff", otherwise the out-projection conv-GEMM, LN3, ff1 and ff2 (+ LN) launches with xn [rows, 256] and
+// hid [rows, 1024] (act dtype) as scratch.
+void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat* att, const ConvW* wo, const int* row2seq, const float* ln3_g,
+             const float* ln3_b, const ConvW& ff1, const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn,
+             const Mat& hid);
 size_t skinny_scratch_floats(int rows, int maxN);
 const bf16* skinny_tiled_weights(cvk_ctx* ctx, const ConvW& W);
 int conv_gemm_skinny_ex(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, const Epilogue& ep, float* scratch, size_t scratch_floats,

@@ -273,11 +273,19 @@ void flow_set_noise(cvk_ctx* ctx, const float* noise_tm, int T, int on_device) {
   m->noise_T = T;
 }
 
-void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& ff1,
-             const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn, const Mat& hid) {
+void flow_ff(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat* att, const ConvW* wo, const int* row2seq, const float* ln3_g,
+             const float* ln3_b, const ConvW& ff1, const ConvW& ff2, const float* ln_g, const float* ln_b, const Mat& out, const Mat& xn,
+             const Mat& hid) {
   if (ctx->flow_fused_ff && ctx->act_dtype == DT_BF16 && ctx->use_tc) {
-    ffn_fused(ctx, st, x, row2seq, ln3_g, ln3_b, ff1, ff2, ln_g, ln_b, out);
+    ffn_fused(ctx, st, x, att, wo, row2seq, ln3_g, ln3_b, ff1, ff2, ln_g, ln_b, out);
     return;
+  }
+  if (att) {
+    Epilogue e;
+    e.resid = x;
+    e.row2seq = row2seq;
+    e.out = x;
+    conv_gemm(ctx, st, *att, *wo, e);
   }
   layernorm(ctx, st, x, ln3_g, ln3_b, 1e-5f, ACT_NONE, 1.f, row2seq, xn);
   {
@@ -719,8 +727,9 @@ Mat kv_cache_append(cvk_ctx* ctx, cudaStream_t st, EstInc* inc, const Mat& qkv, 
   return cache;
 }
 
-// Every block's first operand is LN1(x) in b.xn; a stage's first block computes it, each later one gets it from the feed-forward
-// half of the block before (flow_ff), which in the bf16 mode is a single launch that never stores the 1024-wide hidden activation.
+// Every block's first operand is LN1(x) in b.xn; a stage's first block computes it, each later one gets it from the block before:
+// flow_ff runs everything after the attention (out projection + residual, feed-forward, next LN1), in the bf16 mode as a single
+// launch that never stores the 1024-wide hidden activation.
 void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstBuffers& b, int chunk, const Mat* out2, EstInc* inc,
             bool first, const TBlockW* next) {
   if (first) layernorm(ctx, st, b.x, t.ln1_g, t.ln1_b, 1e-5f, ACT_NONE, 1.f, s.d_row2seq, b.xn);
@@ -735,14 +744,7 @@ void tblock(cvk_ctx* ctx, cudaStream_t st, const TBlockW& t, const Seqs& s, EstB
     attention_fwd(ctx, st, b.qkv.slice(0, 512), cache.slice(0, 512), cache.slice(512, 512), s, H_EST, chunk, 0.125f, b.att, 1, &inc->kg);
   } else
   attention_fwd(ctx, st, b.qkv.slice(0, 512), b.qkv.slice(512, 512), b.qkv.slice(1024, 512), s, H_EST, chunk, 0.125f, b.att);
-  {
-    Epilogue e;
-    e.resid = b.x;
-    e.row2seq = s.d_row2seq;
-    e.out = b.x;
-    conv_gemm(ctx, st, b.att, t.out, e);
-  }
-  flow_ff(ctx, st, b.x, s.d_row2seq, t.ln3_g, t.ln3_b, t.ff1, t.ff2, next ? next->ln1_g : nullptr, next ? next->ln1_b : nullptr,
+  flow_ff(ctx, st, b.x, &b.att, &t.out, s.d_row2seq, t.ln3_g, t.ln3_b, t.ff1, t.ff2, next ? next->ln1_g : nullptr, next ? next->ln1_b : nullptr,
           out2 ? *out2 : b.xn, b.xn, b.ff);
 }
 

@@ -861,7 +861,16 @@ void launch_panel(cvk_ctx* ctx, cudaStream_t st, const CUtensorMap& ta, const CU
 // warp streams the W1 / W2 chunks through a two-stage ring.  Operations and their order are those of the unfused path
 // (layernorm256_kernel, conv_gemm_wg_kernel with the GELU and the residual epilogues: same wgmma K steps in ascending order, same
 // bf16 roundings), so the results agree bit for bit.
+// With the attention output `att` (bf16 [rows, 512]) the launch first folds in the block's attention output projection and its residual
+// (x <- valid(r) ? x + bo + att Wo^T : 0, the out conv-GEMM of the unfused path): the producer streams eight 64-wide K chunks, each the
+// CTA's 128 x 64 att slice and a 256 x 64 Wo slice (48 KB), through the same ring ahead of the W1 / W2 chunks; each consumer warpgroup
+// accumulates m64n256k16 over K = 512 in ascending order from zero (the conv-GEMM's MMAs), stages acc + bo in fp32 over the A tile
+// region (free until LN3) in two 128-column halves, and adds the residual and the row mask per row (the conv-GEMM epilogue's order)
+// as it writes x.  LN3 takes the new x from the registers of the lanes that wrote it, and the ring's first W1 / W2 chunks land meanwhile.
 constexpr int FF_C = 256, FF_HID = 1024, FF_HC = 64, FF_NCH = FF_HID / FF_HC;
+constexpr int FF_OK = 512, FF_OCH = FF_OK / 64;         // out projection: K = 512 (8 heads x 64) in 64-wide ring chunks
+constexpr uint32_t FF_ATT_BYTES = TC_BM * 64 * 2;      // att chunk: [128 rows][64], one SWIZZLE_128B sub-tile
+constexpr uint32_t FF_WO_BYTES = FF_C * 64 * 2;        // Wo chunk: [256 channels][64]
 constexpr uint32_t FF_A_BYTES = TC_BM * FF_C * 2;      // LN3(x): four SWIZZLE_128B sub-tiles [128 rows][64 channels]
 constexpr uint32_t FF_W1_BYTES = FF_HC * FF_C * 2;     // W1 chunk: four sub-tiles [64 hidden][64 channels]
 constexpr uint32_t FF_W2_BYTES = FF_C * FF_HC * 2;     // W2 chunk: [256 channels][64 hidden]
@@ -870,6 +879,8 @@ constexpr int FF_NSTG = 2;
 constexpr int FF_OLD = FF_C + 8;                       // pitch (floats) of the fp32 output tile staged over the operand region
 constexpr size_t FF_SMEM = FF_A_BYTES + FF_NSTG * FF_STAGE_BYTES + 1024;
 static_assert((size_t)TC_BM * FF_OLD * 4 <= FF_A_BYTES + FF_NSTG * FF_STAGE_BYTES, "output staging tile must fit the operand region");
+static_assert(FF_ATT_BYTES + FF_WO_BYTES <= FF_STAGE_BYTES, "an out-projection chunk must fit a ring stage");
+static_assert((size_t)TC_BM * (FF_C / 2) * 4 <= FF_A_BYTES, "a half of the out-projection tile must fit the A tile region");
 
 struct FfnDev {
   float* x;                      // [rows][ldx] fp32 residual stream, in place
@@ -877,12 +888,22 @@ struct FfnDev {
   const int* row2seq;
   const float *ln3_g, *ln3_b, *b1, *b2;
   const float *ln_g, *ln_b;      // LN1 of the next block; null: out is a bf16 copy of x
+  const float* bo;               // out-projection bias; null: no out-projection phase (x is taken as given)
   bf16* out;
   int ldo;
 };
 
+// byte address of (row, column c) of a warpgroup's 128-column half of the fp32 out-projection tile, laid over its own rows of the A tile
+// (row `grow` of the CTA tile; 32 columns per 128-byte sub-tile row, 16-byte chunks XOR-swizzled so that the fragment stores and the
+// row reads are free of bank conflicts).  LN3 later writes these same bytes from the same warpgroup's rows.
+__device__ __forceinline__ uint32_t ff_stg_addr(uint32_t base, int grow, int c) {
+  return base + (uint32_t)(c >> 5) * (TC_BM * 128u) + (uint32_t)grow * 128u + ((((uint32_t)(c & 31) >> 2) ^ ((uint32_t)(grow & 3) << 1)) << 4) +
+         (uint32_t)(c & 3) * 4u;
+}
+
 __global__ void __launch_bounds__(TC_THREADS, 1)
-ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_w2, FfnDev p) {
+ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_w2,
+                 const __grid_constant__ CUtensorMap tmap_att, const __grid_constant__ CUtensorMap tmap_wo, FfnDev p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[FF_NSTG];
   __shared__ __align__(8) uint64_t bar_empty[FF_NSTG];
@@ -900,14 +921,22 @@ ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_const
   }
   __syncthreads();
 
+  const int och = p.bo ? FF_OCH : 0;                  // ring chunks of the out projection, ahead of the FF chunks
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 0 && lane == 0) {
-      for (int c = 0; c < FF_NCH; ++c) {
-        const uint32_t s = c % FF_NSTG, round = c / FF_NSTG;
+      for (int g = 0; g < och + FF_NCH; ++g) {
+        const uint32_t s = g % FF_NSTG, round = g / FF_NSTG;
         mbar_wait(smem_u32(&bar_empty[s]), (round & 1u) ^ 1u);
         const uint32_t sw = w_base + s * FF_STAGE_BYTES;
         const uint32_t fb = smem_u32(&bar_full[s]);
+        if (g < och) {
+          mbar_expect_tx(fb, FF_ATT_BYTES + FF_WO_BYTES);
+          tma_load_2d(sw, &tmap_att, fb, g * 64, r0);
+          tma_load_2d(sw + FF_ATT_BYTES, &tmap_wo, fb, g * 64, 0);
+          continue;
+        }
+        const int c = g - och;
         mbar_expect_tx(fb, FF_STAGE_BYTES);
 #pragma unroll
         for (int kt = 0; kt < FF_C / 64; ++kt) tma_load_2d(sw + kt * (FF_HC * 128u), &tmap_w1, fb, kt * 64, c * FF_HC);
@@ -921,19 +950,87 @@ ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_const
   const int wg = ct >> 7;                             // rows [64 wg, 64 wg + 64) of the tile
   const int cw = ct >> 5;                             // consumer warp 0..7
   const int c0 = lane * 4, c1 = 128 + lane * 4;       // this lane's columns in the row-per-warp phases
+  const int q = lane & 3;
+
+  // this lane's columns c0 and c1 of x in the 16 rows of its warp (valid rows only), loaded together so that their latencies overlap;
+  // with the out projection they become the new x, so LN3 takes them from registers
+  float4 xa[16], xb[16];
+  uint32_t okm = 0;                                   // bit i: row i of the warp is a valid (sequence) row
+  auto load_x = [&](float4* xv, int c) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int r = r0 + cw * 16 + i;
+      xv[i] = (okm >> i) & 1u ? *reinterpret_cast<const float4*>(p.x + (size_t)r * p.ldx + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int r = r0 + cw * 16 + i;
+    if (r < p.rows && p.row2seq[r] >= 0) okm |= 1u << i;
+  }
+
+  if (och) {
+    // out projection: acc = att Wo^T over the ring's first FF_OCH chunks, one MMA group in flight (conv_gemm_wg_kernel's loop)
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int g = 0; g < FF_OCH; ++g) {
+      const uint32_t s = g % FF_NSTG;
+      mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(g / FF_NSTG) & 1u);
+      const uint32_t sa = w_base + s * FF_STAGE_BYTES;
+      const uint64_t da = wg_desc_sw128(sa + (uint32_t)wg * (64 * 128u)), db = wg_desc_sw128(sa + FF_ATT_BYTES);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<256, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+      wg_commit();
+      wg_wait<1>();
+      __syncwarp();
+      if (g > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(g - 1) % FF_NSTG]));
+    }
+    wg_wait<0>();
+    wg_touch<128>(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(FF_OCH - 1) % FF_NSTG]));
+    // per 128-column half: acc + bo staged in fp32 over this warpgroup's rows of the A tile, then per row (one warp per row, the rows
+    // LN3 gives the warp below) + residual and the row mask into x
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of acc[4 j], acc[4 j + 1]; + 8 for acc[4 j + 2], acc[4 j + 3]
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = 8 * j + 2 * q;
+        const float* a = acc + 64 * hf + 4 * j;
+        const float2 b = *reinterpret_cast<const float2*>(p.bo + 128 * hf + col);
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(ff_stg_addr(smem_base, fr, col)), "f"(a[0] + b.x), "f"(a[1] + b.y) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(ff_stg_addr(smem_base, fr + 8, col)), "f"(a[2] + b.x), "f"(a[3] + b.y) : "memory");
+      }
+      if (hf == 0) load_x(xa, c0);                    // the residual of this half, all 16 rows in flight at once
+      else load_x(xb, c1);
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+      float4* xv = hf ? xb : xa;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int row = cw * 16 + i, r = r0 + row;
+        if (r >= p.rows) break;
+        float4 v;
+        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(ff_stg_addr(smem_base, row, c0)) : "memory");
+        const float4 xr = xv[i];
+        xv[i] = (okm >> i) & 1u ? make_float4(v.x + xr.x, v.y + xr.y, v.z + xr.z, v.w + xr.w) : make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(p.x + (size_t)r * p.ldx + 128 * hf + c0) = xv[i];
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");   // the half has been read: the region takes the next one, then LN3
+    }
+  } else {
+    load_x(xa, c0);
+    load_x(xb, c1);
+  }
 
   // LN3 prologue, one warp per row as in layernorm256_kernel: bf16 rows of the A tile (gap rows and rows past the end are zero)
-  for (int i = 0; i < 16; ++i) {
-    const int row = cw * 16 + i, r = r0 + row;
-    float v[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = 0.f;
-    if (r < p.rows && p.row2seq[r] >= 0) {
-      const float* xp = p.x + (size_t)r * p.ldx;
-      const float4 a = *reinterpret_cast<const float4*>(xp + c0), b = *reinterpret_cast<const float4*>(xp + c1);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-      ln256_warp(v, p.ln3_g, p.ln3_b, 1e-5f, c0, c1);
-    }
+  for (int i = 0; i < 16; ++i) {
+    const int row = cw * 16 + i;
+    float v[8] = {xa[i].x, xa[i].y, xa[i].z, xa[i].w, xb[i].x, xb[i].y, xb[i].z, xb[i].w};
+    if ((okm >> i) & 1u) ln256_warp(v, p.ln3_g, p.ln3_b, 1e-5f, c0, c1);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int c = h ? c1 : c0;
@@ -947,15 +1044,15 @@ ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_const
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma operand reads
   asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");     // this warpgroup's 64 rows are complete
 
-  const int q = lane & 3;
   float o[128];
 #pragma unroll
   for (int i = 0; i < 128; ++i) o[i] = 0.f;
   uint32_t hp[16];
   const uint32_t a_wg = smem_base + (uint32_t)wg * (64 * 128u);
   for (int c = 0; c < FF_NCH; ++c) {
-    const uint32_t s = c % FF_NSTG;
-    mbar_wait(smem_u32(&bar_full[s]), (uint32_t)(c / FF_NSTG) & 1u);
+    const uint32_t g = och + c;                       // ring chunk
+    const uint32_t s = g % FF_NSTG;
+    mbar_wait(smem_u32(&bar_full[s]), (g / FF_NSTG) & 1u);
     const uint32_t sw1 = w_base + s * FF_STAGE_BYTES, sw2 = sw1 + FF_W1_BYTES;
     float h[32];
 #pragma unroll
@@ -971,7 +1068,7 @@ ffn_fused_kernel(const __grid_constant__ CUtensorMap tmap_w1, const __grid_const
     wg_wait<0>();                                     // FF1 of this chunk and FF2 of the previous one have completed
     wg_touch<32>(h);
     __syncwarp();
-    if (c > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(c - 1) % FF_NSTG]));
+    if (c > 0 && lane == 0) mbar_arrive(smem_u32(&bar_empty[(g - 1) % FF_NSTG]));
     // bias + GELU as the FF1 epilogue computes them (act16_fast), bf16 pairs in the register A-operand layout
     const float* b1 = p.b1 + c * FF_HC + 2 * q;
 #pragma unroll
@@ -1113,9 +1210,16 @@ void conv_gemm_tc(cvk_ctx* ctx, cudaStream_t st, const Mat& A, const ConvW& W, c
   CVK_LAUNCH_CHECK();
 }
 
-void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, const float* ln3_g, const float* ln3_b, const ConvW& w1,
-               const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out) {
+void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const Mat* att, const ConvW* wo, const int* row2seq, const float* ln3_g,
+               const float* ln3_b, const ConvW& w1, const ConvW& w2, const float* ln_g, const float* ln_b, const Mat& out) {
   CVK_REQUIRE(x.dtype == DT_F32 && x.cols == FF_C && x.ld % 4 == 0 && ((uintptr_t)x.p & 15) == 0, "ffn_fused: x must be fp32 [rows, 256], 16-byte aligned rows");
+  CVK_REQUIRE(!att == !wo, "ffn_fused: the out projection needs both att and its weights");
+  if (att) {
+    CVK_REQUIRE(att->dtype == DT_BF16 && att->cols == FF_OK && att->rows >= x.rows && att->ld % 8 == 0 && ((uintptr_t)att->p & 15) == 0,
+                "ffn_fused: att must be bf16 [rows, 512], 16-byte aligned rows");
+    CVK_REQUIRE(wo->N == FF_C && wo->K == FF_OK && wo->taps == 1 && wo->w16 && wo->bias && ((uintptr_t)wo->bias & 15) == 0,
+                "ffn_fused: unexpected out-projection weights");
+  }
   CVK_REQUIRE(out.dtype == DT_BF16 && out.cols == FF_C && out.rows >= x.rows && out.ld % 8 == 0 && ((uintptr_t)out.p & 15) == 0,
               "ffn_fused: out must be bf16 [rows, 256], 16-byte aligned rows");
   CVK_REQUIRE(w1.N == FF_HID && w1.K == FF_C && w1.taps == 1 && w1.w16 && w1.bias && w2.N == FF_C && w2.K == FF_HID && w2.taps == 1 && w2.w16 &&
@@ -1132,14 +1236,27 @@ void ffn_fused(cvk_ctx* ctx, cudaStream_t st, const Mat& x, const int* row2seq, 
   };
   mk(&t1, w1.w16, FF_HID, FF_C, FF_HC);
   mk(&t2, w2.w16, FF_C, FF_HID, FF_C);
+  CUtensorMap ta = t1, two = t1;                      // not read without the out projection
+  if (att) {
+    const cuuint64_t dims[2] = {(cuuint64_t)FF_OK, (cuuint64_t)att->rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)att->ld * 2};
+    const cuuint32_t box[2] = {64, TC_BM};
+    encode_tma_map(ctx, &ta, att->p, 2, dims, strides, box, DT_BF16, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "att");
+    mk(&two, wo->w16, FF_C, FF_OK, FF_C);
+  }
   FfnDev p;
   p.x = x.f32(); p.ldx = x.ld; p.rows = x.rows; p.row2seq = row2seq;
   p.ln3_g = ln3_g; p.ln3_b = ln3_b; p.b1 = w1.bias; p.b2 = w2.bias; p.ln_g = ln_g; p.ln_b = ln_b;
+  p.bo = att ? wo->bias : nullptr;
   p.out = out.b16(); p.ldo = out.ld;
-  const double flops = 4.0 * x.rows * (double)FF_C * FF_HID;
-  const double bytes = (double)x.rows * FF_C * (4 + 4 + 2) + 2.0 * FF_C * FF_HID * 2;
+  double flops = 4.0 * x.rows * (double)FF_C * FF_HID;
+  double bytes = (double)x.rows * FF_C * (4 + 4 + 2) + 2.0 * FF_C * FF_HID * 2;
+  if (att) {
+    flops += 2.0 * x.rows * (double)FF_C * FF_OK;
+    bytes += (double)x.rows * FF_OK * 2 + (double)FF_C * FF_OK * 2;
+  }
   ProfScope ps(ctx, st, FAM_GEMM_TC, flops, bytes);
-  ffn_fused_kernel<<<ceil_div(x.rows, TC_BM), TC_THREADS, FF_SMEM, st>>>(t1, t2, p);
+  ffn_fused_kernel<<<ceil_div(x.rows, TC_BM), TC_THREADS, FF_SMEM, st>>>(t1, t2, ta, two, p);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
 }

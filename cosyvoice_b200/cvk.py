@@ -54,7 +54,7 @@ SIGNATURES = {
                                         _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                         ctypes.c_float, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]),
     "cvk_op_flow_ff": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _c_int_p, _c_int_p, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                      _vp, _vp]),
+                                      _vp, _vp, _vp, _vp, _vp]),
     "cvk_op_relpos_attention": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int,
                                                ctypes.c_int, ctypes.c_float, _vp, _vp]),
     "cvk_hift_f0": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, _vp, _vp]),
@@ -326,12 +326,13 @@ class Context:
             out2.shape[1] if out2 is not None else 0, _stream()))
         return out, out2
 
-    def flow_ff(self, x, seq_start, seq_len, ln3_g, ln3_b, w1, b1, w2, b2, ln_g=None, ln_b=None):
+    def flow_ff(self, x, seq_start, seq_len, ln3_g, ln3_b, w1, b1, w2, b2, ln_g=None, ln_b=None, att=None, wo=None, bo=None):
         """the feed-forward half of a flow-estimator transformer block (cvk_op_flow_ff): x [rows, 256]; w1 [1024, 256], w2 [256, 1024]
-        torch Linear weights.  Returns (new x, out): out = the next block's LN1 (ln_g, ln_b) of the new x, or the new x itself, both as
-        rounded to the activation dtype."""
+        torch Linear weights; with att [rows, 512], wo [256, 512] and bo [256] the block's attention output projection and its residual
+        come first.  Returns (new x, out): out = the next block's LN1 (ln_g, ln_b) of the new x, or the new x itself, both as rounded to
+        the activation dtype."""
         x = _f32(x, self.device).clone()
-        t = [_f32(v, self.device) if v is not None else None for v in (ln3_g, ln3_b, w1, b1, w2, b2, ln_g, ln_b)]
+        t = [_f32(v, self.device) if v is not None else None for v in (ln3_g, ln3_b, w1, b1, w2, b2, ln_g, ln_b, att, wo, bo)]
         out = torch.empty_like(x)
         self._check(self.lib.cvk_op_flow_ff(self.h, _ptr(x), x.shape[0], _ints(seq_start), _ints(seq_len), len(seq_len), *(_ptr(v) for v in t),
                                             _ptr(out), _stream()))

@@ -166,10 +166,13 @@ int cvk_op_conv_gemm(cvk_ctx* ctx, const float* x, int rows, int K, int x_ld, in
  *   out[r] = valid(r) ? LayerNorm(x[r]; ln_g, ln_b) : 0   (ln_g, ln_b NULL: out = x)
  * rounded to the activation dtype, returned as fp32 [rows, 256].  w1 [1024, 256], b1 [1024], w2 [256, 1024], b2 [256] (torch Linear).
  * Sequence b occupies rows [seq_start_host[b], + seq_len_host[b]) (inside [0, rows), not overlapping); every other row is a gap row.
+ * With att [rows, 512] fp32 (device; rounded to the activation dtype), wo [256, 512] and bo [256] (the attention output projection,
+ * torch Linear) the block's out projection and its residual come first: x[r] = valid(r) ? x[r] + bo + att[r] wo^T : 0.  att, wo and
+ * bo all NULL: x is taken as given.
  * bf16 context: one fused launch, or with option "flow_fused_ff" 0 the LayerNorm / GEMM launches the estimator otherwise runs. */
 int cvk_op_flow_ff(cvk_ctx* ctx, float* x, int rows, const int* seq_start_host, const int* seq_len_host, int B, const float* ln3_g,
                    const float* ln3_b, const float* w1, const float* b1, const float* w2, const float* b2, const float* ln_g,
-                   const float* ln_b, float* out, void* stream);
+                   const float* ln_b, const float* att, const float* wo, const float* bo, float* out, void* stream);
 /* The conformer relative-position attention (tests): score(i, j) = ((q_i + bias_u) . k_j + (q_i + bias_v) . pos[center - (i - j)]) * scale
  * per head, block-causal when chunk > 0 (key j visible iff j < (i / chunk + 1) * chunk), softmax over the visible keys, times v.
  * q, k, v, out [sum lens, H*64] ragged; pos [2*center+1, H*64] (row t holds relative position center - t; the library pads it to a

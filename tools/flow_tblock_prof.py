@@ -2,8 +2,9 @@
 
 Writes <out>/flow_kernels_<opt><value>.md: per kernel name the time and launch count of one flow_batch, then the
 time of the estimator's transformer-block launches by role.  Roles come from the launch order inside a block: the attention kernel
-is preceded by the qkv GEMM (the generic kernel or the row-panel one; and, for the first block of a stage, LN1) and followed by the out GEMM, then either LN3, the ff1 and the
-ff2 GEMMs (and the next block's LN1), or the fused feed-forward kernel.  Not a bench: the profiler slows the host.
+is preceded by the qkv GEMM (the generic kernel or the row-panel one; and, for the first block of a stage, LN1) and followed either by
+the fused feed-forward kernel, which also does the out projection, or by the out GEMM, LN3, the ff1 and the ff2 GEMMs (and the next
+block's LN1).  Not a bench: the profiler slows the host.
 
   python tools/flow_tblock_prof.py --opt flow_fused_ff --values 0,1 --out /tmp/flow_prof
 """
@@ -55,19 +56,20 @@ def roles(kern):
     out = []
     names = [short(k["name"]) for k in kern]
     for i, n in enumerate(names):
-        if "attn_wg_kernel" not in n or i < 1 or i + 2 >= len(names):
+        if "attn_wg_kernel" not in n or i < 1 or i + 1 >= len(names):
             continue
-        if not ("conv_gemm_wg_kernel" in names[i - 1] or "qkv_panel_kernel" in names[i - 1]) or "conv_gemm_wg_kernel" not in names[i + 1]:
+        if not ("conv_gemm_wg_kernel" in names[i - 1] or "qkv_panel_kernel" in names[i - 1]):
             continue
-        if not (is_ln(names[i + 2]) or "ffn_fused_kernel" in names[i + 2]):
+        fused = "ffn_fused_kernel" in names[i + 1]
+        if not fused and not ("conv_gemm_wg_kernel" in names[i + 1] and i + 2 < len(names) and is_ln(names[i + 2])):
             continue      # the conformer encoder's layers continue otherwise
-        seq = [("qkv", i - 1), ("attention", i), ("out", i + 1)]
+        seq = [("qkv", i - 1), ("attention", i)]
         if i >= 2 and is_ln(names[i - 2]):
             seq.insert(0, ("ln1 (stage's first block)", i - 2))
-        if "ffn_fused_kernel" in names[i + 2]:
-            seq.append(("ffn (LN3 + ff1 + ff2 + LN1)", i + 2))
+        if fused:
+            seq.append(("out + ffn (out projection + LN3 + ff1 + ff2 + LN1)", i + 1))
         else:
-            seq += [("ln3", i + 2), ("ff1", i + 3), ("ff2", i + 4)]
+            seq += [("out", i + 1), ("ln3", i + 2), ("ff1", i + 3), ("ff2", i + 4)]
             if i + 5 < len(names) and is_ln(names[i + 5]):
                 seq.append(("ln1 (next block)", i + 5))
         out += [(r, names[j], kern[j]["dur"]) for r, j in seq]
@@ -106,8 +108,10 @@ for v in [int(x) for x in a.values.split(",")]:
     lines += ["", "## estimator transformer blocks by role", "", "| role | kernel | ms | launches | share of all kernel time |", "|---|---|---:|---:|---:|"]
     for (r, n), (us, c) in sorted(rs.items(), key=lambda t: -t[1][0]):
         lines.append(f"| {r} | `{n[:80]}` | {us / 1e3:.2f} | {c} | {100 * us / max(total, 1):.1f}% |")
-    ffn = sum(us for (r, _), (us, _) in rs.items() if r.startswith(("ln3", "ff1", "ff2", "ln1 (next", "ffn")))
-    lines += ["", f"LN3 + ff1 + ff2 + next LN1 (or the fused kernel): {ffn / 1e3:.1f} ms, {100 * ffn / max(total, 1):.1f}% of the flow's kernel time"]
+    ffn = sum(us for (r, _), (us, _) in rs.items() if r.startswith(("out", "ln3", "ff1", "ff2", "ln1 (next")))
+    nff = sum(c for (r, _), (_, c) in rs.items() if r.startswith(("out + ffn", "ff2")))
+    lines += ["", f"out projection + LN3 + ff1 + ff2 + next LN1 (or the fused kernel): {ffn / 1e3:.1f} ms, {100 * ffn / max(total, 1):.1f}% of the "
+              f"flow's kernel time; {ffn / max(nff, 1):.1f} us per block ({nff} blocks)"]
     txt = "\n".join(lines) + "\n"
     open(os.path.join(a.out, f"flow_kernels_{a.opt}{v}.md"), "w").write(txt)
     print(txt)
