@@ -186,10 +186,8 @@ int cvk_set_option(cvk_ctx* ctx, const char* key, int value) {
   else if (k == "use_skinny") ctx->use_skinny = value;
   else if (k == "lm_fused") ctx->lm_fused = value;
   else if (k == "pdl") ctx->pdl = value;
-  else if (k == "lm_mega") ctx->lm_mega = value;
   else if (k == "enc_tc_attn") ctx->enc_tc_attn = value;
   else if (k == "hift_f16") ctx->hift_f16 = value;      // takes effect at the next cvk_finalize("hift" / "hift3")
-  else if (k == "mega_coop") ctx->mega_coop = value;
   else if (k == "chain_timeline") {
     if (value && !ctx->tl) {
       ctx->tl = ctx->dmalloc(4096 * sizeof(long long));

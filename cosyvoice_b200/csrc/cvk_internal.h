@@ -197,9 +197,6 @@ struct cvk_ctx {
   int hift_f16 = 1;                         // tensor-core mode: vocoder operands in IEEE half (TF32-class mantissa) instead of bf16
   int build_f16 = 0;                        // set while a stage whose weights need the half copy is being finalised
   int enc_tc_attn = 1;                      // conformer relative-position attention on the wgmma kernels (attention_tc.cu) instead of CUDA cores
-  int lm_mega = 0;                          // LM decode: all layers of a step in one persistent cooperative kernel (llm_mega.cu); off by
-                                            // default: not faster than the PDL-chained per-op path in earlier measurements
-  int mega_coop = 1;                        // ... launched with the cooperative attribute (co-residency guaranteed by the driver)
   int use_skinny = 1;                       // LM decode GEMMs on the weight-streaming split-K kernel
   int use_tc_attn = 1;                      // bf16 mode: wgmma attention kernel (0 = CUDA-core flash kernel)
   int use_graph = 1;                        // LM decode step replayed as a CUDA graph

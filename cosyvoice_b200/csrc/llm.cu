@@ -10,9 +10,261 @@
 // Batched over B independent rows (the reference decodes one utterance at a time).  One decode step for all rows is
 // captured into a CUDA graph; the sampler advances per-row counters on the device, so the host only polls the
 // number of live rows every few steps - no .item() style host round trip per token (common.py:155-161 has several).
-#include "llm_decode_attn.cuh"
+#include "common.cuh"
 #include <math.h>
 #include <algorithm>
+
+namespace lm {
+constexpr int D = 896, NH = 14, NKV = 2, HD = 64, DFF = 4864, VOUT = 6564, EOS = 6561;
+constexpr int VOUT3 = 6761, VOUT3_PAD = 6764;   // CosyVoice3LM head (llm.py:689), padded to a 16-byte row pitch
+constexpr int QKV_N = NH * HD + 2 * NKV * HD;   // 1152
+constexpr float ROPE_THETA = 1.0e6f, RMS_EPS = 1e-6f;
+constexpr int SAMPLER_THREADS = 256, TOPK = 25, WIN = 10;
+constexpr int SAMPLER_PER = (VOUT3_PAD + SAMPLER_THREADS - 1) / SAMPLER_THREADS;   // 27: largest per-thread segment of the sampler
+
+struct LayerW {
+  float *ln1, *ln2;
+  ConvW qkv, o, gate_up, down;
+  ConvW gate_up_il;   // rows interleaved (2i = gate_i, 2i+1 = up_i) for the SwiGLU epilogue of the decode GEMM
+};
+}  // namespace lm
+
+struct LlmModel {
+  int num_layers = 24;
+  int vout = lm::VOUT;           // width of the head / logits rows: 6564 (Qwen2LM) or 6764 (CosyVoice3LM: 6761 + 3 impossible pad ids)
+  std::vector<lm::LayerW> layers;
+  float* final_norm = nullptr;
+  float* text_emb = nullptr;     // [151936][896]
+  float* llm_emb = nullptr;      // [2][896]  sos, task_id
+  float* speech_emb = nullptr;   // [6564][896]
+  ConvW head;                    // llm_decoder 896 -> 6564
+  float inv_freq[lm::HD / 2];
+  float* d_inv_freq = nullptr;
+};
+
+struct cvk_lm_session {
+  int max_batch = 0, max_ctx = 0, B = 0;
+  int kv_dtype = DT_F32;
+  void* kcache = nullptr;   // [layers][max_batch][NKV][max_ctx][HD]
+  void* vcache = nullptr;
+  int* ctx_len = nullptr;   // [max_batch] cache position of the token currently being fed
+  int* base_len = nullptr;  // [max_batch] prompt length L0
+  bool fresh = false;
+  int fed = 0;              // positions pushed by cvk_lm_feed since cvk_lm_begin
+  int64_t graph_kernels = 0;
+  int* count = nullptr;     // [max_batch] tokens generated so far
+  int* done = nullptr;      // [max_batch]
+  int* live = nullptr;      // [1]
+  float* x = nullptr;       // [max_batch][896] input embedding of the current step (fp32 residual stream)
+  float* hidden = nullptr;  // [max_batch][896] final-normed hidden of the last position
+  float* logits = nullptr;  // [max_batch][VOUT]
+  void* xn = nullptr;       // act [max_batch][896]
+  void* qkv = nullptr;      // act [max_batch][1152]
+  void* att = nullptr;      // act [max_batch][896]
+  void* gu = nullptr;       // act [max_batch][2*4864]
+  void* ffa = nullptr;      // act [max_batch][4864]
+  cudaGraphExec_t graph = nullptr;
+  // arguments baked into the captured graph
+  const float* g_uniforms = nullptr;
+  const int32_t *g_min = nullptr, *g_max = nullptr;
+  int32_t *g_out_ids = nullptr, *g_out_count = nullptr, *g_done = nullptr;
+  int g_out_ld = 0, g_B = 0, g_pdl = -1;
+  float* scratch = nullptr;      // split-K partial sums of the weight-streaming GEMM
+  size_t scratch_floats = 0;
+  // ragged feeding (cvk_lm_feed_rows / cvk_lm_next_logp_rows)
+  bool ragged = false;           // set by cvk_lm_begin; rows_fed mirrors ctx_len only between a begin and the next prefill / decode
+  std::vector<int> rows_fed;     // [max_batch] host mirror of ctx_len: positions fed to each row since cvk_lm_begin
+  int* sel = nullptr;            // [max_batch] device: rows listed by cvk_lm_next_logp_rows
+  int feed_cap = 0;              // positions per forward pass of the feed buffers below (0 until the first cvk_lm_feed_rows)
+  float* fx = nullptr;           // [feed_cap][896] fp32 residual stream of the fed positions
+  void *fxn = nullptr, *fqkv = nullptr, *fatt = nullptr, *fgu = nullptr, *fffa = nullptr;   // act [feed_cap][...]
+  int* fidx = nullptr;           // device copy of a pass's index tables (see llm_feed_rows)
+  float* fscratch = nullptr;     // split-K partial sums of the weight-streaming GEMM for up to 64 fed positions
+  size_t fscratch_floats = 0;
+  std::vector<void*> owned;
+};
+
+// One (row, kv head) unit of the LM decode attention (attn_fused_kernel).
+//
+// qkv split-K reduction + bias + RoPE + KV-cache append + GQA decode attention (transformers Qwen2 attention,
+// SURVEY.md Appendix C; cosyvoice/llm/llm.py:242-254 forward_one_step).  The attention itself is flash-decoding on
+// warp-level tensor-core MMAs (m16n8k16, bf16 in / fp32 accumulate): the 7 query heads of the group are the M rows of the
+// tile (7 of 16 used - wgmma's M >= 64 would waste 9/10 of the tile), each of the NW warps walks its own
+// 16-key blocks with an online softmax held in registers, K and V fragments come straight from the cache with 4-byte loads
+// (V's key pairs are formed with byte permutes, the output dims of a 16-dim block are assigned to the two n-tiles as evens /
+// odds so that each lane ends up with 4 consecutive dims), P never leaves registers (the QK^T accumulator layout is the
+// A-operand layout of the P V MMA), and the warps' partial (max, sum, O) are merged through shared memory.
+namespace lm {
+
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&h2);
+}
+__device__ __forceinline__ void mma_16816(float* c, uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1) {   // A rows 8..15 are zero
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a0), "r"(0u), "r"(a2), "r"(0u), "r"(b0), "r"(b1));
+}
+
+// K / V fragments of one 16-key block (rows j0 .. j0+15, all below `L`), in the MMA operand layout used by decode_attn_unit
+struct KvFrag {
+  uint32_t kf[2][4][2], vw[4][4];
+};
+__device__ __forceinline__ void decode_attn_load_block(const bf16* __restrict__ kb, const bf16* __restrict__ vb, int j0, int L, int lane, KvFrag& f) {
+  const int g = lane >> 2, t4 = lane & 3;
+#pragma unroll
+  for (int nt = 0; nt < 2; ++nt) {
+    const uint32_t* kr = reinterpret_cast<const uint32_t*>(kb + (size_t)min(j0 + nt * 8 + g, L - 1) * HD);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      f.kf[nt][kk][0] = kr[kk * 8 + t4];
+      f.kf[nt][kk][1] = kr[kk * 8 + 4 + t4];
+    }
+  }
+  const uint32_t* v0 = reinterpret_cast<const uint32_t*>(vb + (size_t)min(j0 + t4 * 2, L - 1) * HD);
+  const uint32_t* v1 = reinterpret_cast<const uint32_t*>(vb + (size_t)min(j0 + t4 * 2 + 1, L - 1) * HD);
+  const uint32_t* v2 = reinterpret_cast<const uint32_t*>(vb + (size_t)min(j0 + 8 + t4 * 2, L - 1) * HD);
+  const uint32_t* v3 = reinterpret_cast<const uint32_t*>(vb + (size_t)min(j0 + 9 + t4 * 2, L - 1) * HD);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    f.vw[q][0] = v0[q * 8 + g];
+    f.vw[q][1] = v1[q * 8 + g];
+    f.vw[q][2] = v2[q * 8 + g];
+    f.vw[q][3] = v3[q * 8 + g];
+  }
+}
+
+// tid: thread of the CTA of NW warps that runs the unit (all NW*32 threads must call).
+// partial [splits][rows][1152] fp32 split-K sums of the qkv projection of row b; kb / vb: this (row, kv head)'s cache
+// [max_ctx][64]; out: bf16 [.. ldo], this row's attention output (columns of the kv group's 7 query heads).
+template <int NW>
+__device__ __forceinline__ void decode_attn_unit(float* __restrict__ sm_all, int tid, const float* __restrict__ partial, int splits, int rows,
+                                                 int b, int kvh, const float* __restrict__ bias, bf16* __restrict__ kb, bf16* __restrict__ vb,
+                                                 int pos, int max_ctx, const float* __restrict__ inv_freq, bf16* __restrict__ out_row,
+                                                 KvFrag& fr /*fragment registers; if have_pre: this warp's first block, loaded early*/,
+                                                 bool have_pre) {
+  constexpr int G = NH / NKV;
+  constexpr int NT = NW * 32;
+  const int warp = tid >> 5, lane = tid & 31;
+  float* stage = sm_all;
+  float* ml = stage + (G + 2) * HD;
+  float* po = ml + NW * 8 * 2;
+  for (int e = tid; e < (G + 2) * HD; e += NT) {
+    const int vec = e / HD, d = e % HD;
+    const int col = vec < G ? (kvh * G + vec) * HD + d : (vec == G ? NH * HD + kvh * HD + d : NH * HD + NKV * HD + kvh * HD + d);
+    const float* p = partial + (size_t)b * QKV_N + col;
+    const size_t stride = (size_t)rows * QKV_N;
+    float a0 = bias[col], a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    int s = 0;
+    for (; s + 4 <= splits; s += 4) {      // independent loads in flight
+      a0 += p[(size_t)s * stride];
+      a1 += p[(size_t)(s + 1) * stride];
+      a2 += p[(size_t)(s + 2) * stride];
+      a3 += p[(size_t)(s + 3) * stride];
+    }
+    for (; s < splits; ++s) a0 += p[(size_t)s * stride];
+    stage[e] = (a0 + a1) + (a2 + a3);
+  }
+  __syncthreads();
+  for (int e = tid; e < (G + 1) * (HD / 2); e += NT) {     // rotate the G query heads and k (half-split RoPE, theta 1e6)
+    const int vec = e / (HD / 2), i = e % (HD / 2);
+    const float fr = (float)pos * inv_freq[i];
+    const float c = cosf(fr), sn = sinf(fr);
+    float* p = stage + vec * HD;
+    const float x1 = p[i], x2 = p[i + HD / 2];
+    p[i] = x1 * c - x2 * sn;
+    p[i + HD / 2] = x2 * c + x1 * sn;
+  }
+  __syncthreads();
+  if (pos < max_ctx && tid < 2 * HD) {
+    const int d = tid % HD;
+    if (tid < HD) kb[(size_t)pos * HD + d] = __float2bfloat16_rn(stage[G * HD + d]);
+    else vb[(size_t)pos * HD + d] = __float2bfloat16_rn(stage[(G + 1) * HD + d]);
+  }
+  __syncthreads();
+  const int L = min(pos + 1, max_ctx);
+  const int g = lane >> 2, t4 = lane & 3;        // MMA fragment coordinates: row / column group
+  uint32_t qa[4][2];                             // Q as the A operand: [k step][dims t4*2.. | +8]; row g = query head g (row 7 unused)
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int hv = 0; hv < 2; ++hv) {
+      const int d = kk * 16 + hv * 8 + t4 * 2;
+      qa[kk][hv] = g < G ? pack_bf16x2(__bfloat162float(__float2bfloat16_rn(stage[g * HD + d])) * 0.125f,
+                                       __bfloat162float(__float2bfloat16_rn(stage[g * HD + d + 1])) * 0.125f)
+                         : 0u;
+    }
+  float o[4][2][4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int t = 0; t < 2; ++t)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[q][t][e] = 0.f;
+  float m_run = -INFINITY, l_run = 0.f;
+  for (int j0 = warp * 16; j0 < L; j0 += NW * 16) {
+    // every load of the block is issued before the first use: one memory round trip per 16 keys.  Rows past the end are
+    // clamped to the last valid row (finite data), their probabilities are forced to zero below.
+    if (!(have_pre && j0 == warp * 16)) decode_attn_load_block(kb, vb, j0, L, lane, fr);
+    uint32_t (&kf)[2][4][2] = fr.kf;
+    uint32_t (&vw)[4][4] = fr.vw;
+    float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      mma_16816(s0, qa[kk][0], qa[kk][1], kf[0][kk][0], kf[0][kk][1]);
+      mma_16816(s1, qa[kk][0], qa[kk][1], kf[1][kk][0], kf[1][kk][1]);
+    }
+    // this lane: head g, keys j0 + 2 t4 + {0,1} (s0) and j0 + 8 + 2 t4 + {0,1} (s1)
+    const int ka = j0 + t4 * 2;
+    const bool va0 = ka < L, va1 = ka + 1 < L, vb0 = ka + 8 < L, vb1 = ka + 9 < L;
+    float mx = fmaxf(fmaxf(va0 ? s0[0] : -INFINITY, va1 ? s0[1] : -INFINITY), fmaxf(vb0 ? s1[0] : -INFINITY, vb1 ? s1[1] : -INFINITY));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float m_new = fmaxf(m_run, mx);          // finite: key j0 itself is valid
+    const float corr = __expf(m_run - m_new);      // exp(-inf) = 0 on the first block
+    const float p0 = va0 ? __expf(s0[0] - m_new) : 0.f, p1 = va1 ? __expf(s0[1] - m_new) : 0.f;
+    const float p2 = vb0 ? __expf(s1[0] - m_new) : 0.f, p3 = vb1 ? __expf(s1[1] - m_new) : 0.f;
+    l_run = l_run * corr + ((p0 + p1) + (p2 + p3));
+    m_run = m_new;
+    const uint32_t pa0 = pack_bf16x2(p0, p1), pa2 = pack_bf16x2(p2, p3);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      o[q][0][0] *= corr; o[q][0][1] *= corr;
+      o[q][1][0] *= corr; o[q][1][1] *= corr;
+      // n-tile 0: even dims of the 16-dim block, n-tile 1: odd dims (low / high halves of the loaded words)
+      mma_16816(o[q][0], pa0, pa2, __byte_perm(vw[q][0], vw[q][1], 0x5410), __byte_perm(vw[q][2], vw[q][3], 0x5410));
+      mma_16816(o[q][1], pa0, pa2, __byte_perm(vw[q][0], vw[q][1], 0x7632), __byte_perm(vw[q][2], vw[q][3], 0x7632));
+    }
+  }
+  l_run += __shfl_xor_sync(0xffffffffu, l_run, 1);
+  l_run += __shfl_xor_sync(0xffffffffu, l_run, 2);
+  if (g < G) {
+    if (t4 == 0) {
+      ml[(warp * 8 + g) * 2] = m_run;
+      ml[(warp * 8 + g) * 2 + 1] = l_run;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q)     // dims 16 q + 4 t4 .. + 3
+      *reinterpret_cast<float4*>(po + ((size_t)warp * G + g) * HD + q * 16 + t4 * 4) = make_float4(o[q][0][0], o[q][1][0], o[q][0][1], o[q][1][1]);
+  }
+  __syncthreads();
+  for (int e = tid; e < G * HD; e += NT) {
+    const int hq = e / HD, d = e % HD;
+    float M = -INFINITY;
+#pragma unroll
+    for (int w2 = 0; w2 < NW; ++w2) M = fmaxf(M, ml[(w2 * 8 + hq) * 2]);
+    float num = 0.f, den = 0.f;
+#pragma unroll
+    for (int w2 = 0; w2 < NW; ++w2) {
+      const float wgt = __expf(ml[(w2 * 8 + hq) * 2] - M);    // warps without keys: exp(-inf) = 0
+      den = fmaf(wgt, ml[(w2 * 8 + hq) * 2 + 1], den);
+      num = fmaf(wgt, po[((size_t)w2 * G + hq) * HD + d], num);
+    }
+    out_row[(kvh * G + hq) * HD + d] = __float2bfloat16_rn(num / den);
+  }
+}
+
+}  // namespace lm
 
 using namespace lm;
 
@@ -239,7 +491,7 @@ __global__ void __launch_bounds__(D) finish_rms_kernel(const float* __restrict__
 }
 
 // qkv split-K reduction + bias + RoPE + KV-cache append + GQA decode attention; one CTA per (row, kv head): see
-// llm_decode_attn.cuh (the same unit runs inside the persistent decode kernel, llm_mega.cu).
+// decode_attn_unit.
 // QK^T and P V run on mma.sync instead of CUDA-core FMAs (which would need a bf16->fp32 conversion + FMA per element, per head).
 constexpr int AF_WARPS = 16;
 __global__ void __launch_bounds__(32 * AF_WARPS)
@@ -263,7 +515,7 @@ attn_fused_kernel(const float* __restrict__ partial /*[S][rows][1152]*/, int spl
   if (have_pre) decode_attn_load_block(kb, vb, wj0, p0, threadIdx.x & 31, pre);
   pdl_wait();
   tl_stamp(tl, 1);
-  decode_attn_unit<AF_WARPS, 0>(sm_all, threadIdx.x, partial, splits, rows, b, kvh, bias, kb, vb, ctx_len[b], max_ctx, inv_freq,
+  decode_attn_unit<AF_WARPS>(sm_all, threadIdx.x, partial, splits, rows, b, kvh, bias, kb, vb, ctx_len[b], max_ctx, inv_freq,
                                 out + (size_t)b * ldo, pre, have_pre);
   tl_stamp(tl, 2);
 }
@@ -329,7 +581,7 @@ __device__ __forceinline__ void mma_16816_full(float* c, uint32_t a0, uint32_t a
 // query heads of the first position (rows 0..6) and of the second (rows 8..14), so both positions share every K / V fragment.
 // Each query attends to its row's cache up to and including its own position: the appends of the whole pass ran before this
 // kernel, so causality inside a feed is only the key bound.  The RA_WARPS warps walk interleaved 16-key blocks with an online
-// softmax in registers (the decode unit's scheme, llm_decode_attn.cuh) and merge their partial (max, sum, O) in shared memory.
+// softmax in registers (the decode unit's scheme, decode_attn_unit) and merge their partial (max, sum, O) in shared memory.
 constexpr int RA_WARPS = 4;
 __global__ void __launch_bounds__(32 * RA_WARPS)
 ragged_attn_tc_kernel(const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kc, const bf16* __restrict__ vc, int max_ctx,
@@ -1207,7 +1459,6 @@ void llm_build(cvk_ctx* ctx, const int* cfg, int ncfg) {
   CVK_CHECK_CUDA(cudaMemcpy(m->d_inv_freq, m->inv_freq, sizeof(m->inv_freq), cudaMemcpyHostToDevice));
   CVK_CHECK_CUDA(cudaDeviceSynchronize());
   ctx->llm = m;
-  if (ctx->precision == CVK_PREC_BF16) lm_mega_build(ctx, m);
 }
 
 cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context) {
@@ -1254,7 +1505,6 @@ cvk_lm_session* llm_session_create(cvk_ctx* ctx, int max_batch, int max_context)
   s->scratch = (float*)alloc(s->scratch_floats * sizeof(float));
   s->sel = (int*)alloc(sizeof(int) * max_batch);
   s->rows_fed.assign(max_batch, 0);
-  lm_mega_session_init(ctx, s);
   return s;
 }
 
@@ -1264,7 +1514,6 @@ void llm_session_destroy(cvk_ctx* ctx, cvk_lm_session* s) {
   // stream is drained by cudaFree (it synchronises the device implicitly) before the buffers go away
   if (s->graph) cudaGraphExecDestroy(s->graph);
   for (void* p : s->owned) cudaFree(p);
-  lm_mega_session_free(s);
   delete s;
 }
 
@@ -1327,15 +1576,11 @@ static bool lm_fused_path(cvk_ctx* ctx, cvk_lm_session* s) {
 }
 
 // The layers of a bf16 decode step on the fused path: x (residual stream) and xn = RMSNorm(x) ln1[0] in -> x, xn = the final-normed
-// hidden state out; every layer appends its K / V row at ctx_len.  Persistent kernel when it can run, else the PDL chain of 7
-// launches per layer.  decode_step_fused runs it after the sampler, cvk_op_lm_decode_layers on caller state.
+// hidden state out; every layer appends its K / V row at ctx_len.  A PDL chain of 7 launches per layer.  decode_step_fused runs
+// it after the sampler, cvk_op_lm_decode_layers on caller state.
 static void decode_layers_fused(cvk_ctx* ctx, cudaStream_t st, cvk_lm_session* s) {
   const LlmModel* m = ctx->llm;
   const int B = s->g_B;
-  if (lm_mega_usable(ctx, s, B)) {     // all layers in one persistent cooperative kernel (llm_mega.cu)
-    lm_mega_layers(ctx, st, s, B);
-    return;
-  }
   const bool pdl = ctx->pdl != 0;
   Mat xn(s->xn, DT_BF16, B, D, D), att(s->att, DT_BF16, B, D, D), ffa(s->ffa, DT_BF16, B, DFF, DFF);
   for (int li = 0; li < m->num_layers; ++li) {
@@ -1423,15 +1668,14 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
     s->fresh = false;
   }
   bool same = s->g_out_count == out_count && s->g_done == done && s->g_out_ids == out_ids && s->g_uniforms == uniforms &&
-              s->g_min == min_len && s->g_max == max_len && s->g_out_ld == out_ld && s->g_B == B && s->g_pdl == ctx->pdl &&
-              s->g_mega == ctx->lm_mega;
+              s->g_min == min_len && s->g_max == max_len && s->g_out_ld == out_ld && s->g_B == B && s->g_pdl == ctx->pdl;
   if (!same) {
     if (s->graph) {
       cudaGraphExecDestroy(s->graph);
       s->graph = nullptr;
     }
     s->g_out_count = out_count; s->g_done = done; s->g_out_ids = out_ids; s->g_uniforms = uniforms; s->g_min = min_len; s->g_max = max_len;
-    s->g_out_ld = out_ld; s->g_B = B; s->g_pdl = ctx->pdl; s->g_mega = ctx->lm_mega;
+    s->g_out_ld = out_ld; s->g_B = B; s->g_pdl = ctx->pdl;
   }
   s->g_B = B;
   if (was_fresh && lm_fused_path(ctx, s)) {
@@ -1486,8 +1730,8 @@ void llm_decode(cvk_ctx* ctx, cvk_lm_session* s, int n_steps, const float* unifo
 }
 
 // The layers of one decode step on caller state (cvk_op_lm_decode_layers), on a temporary session of B rows x max_ctx positions:
-// the layer loop cvk_lm_decode runs after the sampler, on the path the step would take (decode_step: the fused chain or the persistent
-// kernel, else the per-op loop).  x [B][896] fp32 in / out; the caches [layers][B][2][max_ctx][64] cross the call as fp32 and run as
+// the layer loop cvk_lm_decode runs after the sampler, on the path the step would take (decode_step: the fused chain, else the per-op
+// loop).  x [B][896] fp32 in / out; the caches [layers][B][2][max_ctx][64] cross the call as fp32 and run as
 // bf16, each layer appending its row at ctx_len_host[b]; xn_out [B][896] the bf16 final-normed row the step hands to the head;
 // att_out [B][896] / ffa_out [B][4864] (nullable) the last layer's o_proj / down_proj operands, which every path leaves in the session's
 // att / ffa buffers.  The entry xn = RMSNorm(x) ln1[0], which the sampler computes in a step, comes from the path's own norm kernel.

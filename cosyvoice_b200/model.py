@@ -355,8 +355,8 @@ class B200CosyVoice2Model:
         does (cli/model.py:101-129, 268).
 
         `self.lm_chains > 1` splits the rows into independent groups, each with its own KV session, CUDA graph and stream (an
-        experiment knob from the per-op decode chain; with the persistent decode kernel one chain is best).  Results are
-        independent of the grouping (rows never interact; every row consumes its own uniforms)."""
+        experiment knob from the per-op decode chain).  Results are independent of the grouping (rows never interact; every row
+        consumes its own uniforms)."""
         B = len(texts)
         d = self.device
         main = stream if stream is not None else self.stream

@@ -72,7 +72,7 @@ int cvk_debug_read(cvk_ctx* ctx, long long* out, int n);
 int cvk_workspace_bytes(cvk_ctx* ctx, size_t* capacity, size_t* high_water);
 /* Test / measurement switches, NOT part of the drop-in surface (every default is the benchmarked configuration): kernel-variant
  * A/B ("use_tc", "tc_persist", "tc_epi", "tc_epi_frag", "use_tc_attn", "enc_tc_attn", "use_skinny", "flow_fused_ff", "flow_qkv_panel" (0 / 1 /
- * 2 = the row-panel GEMM never / from 25 panels of 128 rows up / at any row count), "lm_fused", "lm_mega", "mega_coop", "pdl", "use_graph", "hift_f16" - the last one takes effect at the next cvk_finalize("hift")),
+ * 2 = the row-panel GEMM never / from 25 panels of 128 rows up / at any row count), "lm_fused", "pdl", "use_graph", "hift_f16" - the last one takes effect at the next cvk_finalize("hift")),
  * probes ("op_iters", "op_out_bf16", "chain_timeline").  Unknown keys return CVK_ERR_INVALID. */
 int cvk_set_option(cvk_ctx* ctx, const char* key, int value);
 
@@ -131,10 +131,9 @@ int cvk_op_decode_attention(cvk_ctx* ctx, const float* partial, int splits, int 
  * [layers][B][2][max_ctx][64] fp32, in / out (run as bf16, as in a session; layer l appends row b at position ctx_len_host[b]);
  * xn_out [B][896] the bf16 final-normed row the step hands to the head; att_out [B][896] and ffa_out [B][4864] (nullable) the last
  * layer's attention output and SwiGLU output, the bf16 operands of its o_proj and down_proj.  The options choose the path as in
- * cvk_lm_decode: "lm_fused" 1 the fused chain ("lm_mega" 1: the persistent kernel), "lm_fused" 0 the per-op chain ("use_skinny" 0: the
- * tiled GEMMs); "pdl" is honoured.  The entry xn = RMSNorm(x) ln1[0] comes from the path's own norm kernel.  An fp32 context, an
- * unfinalised stage, B outside [1, 64], ctx_len outside [0, max_ctx) and max_ctx beyond the decode-attention limit are refused with
- * CVK_ERR_INVALID before any device work. */
+ * cvk_lm_decode: "lm_fused" 1 the fused chain, "lm_fused" 0 the per-op chain ("use_skinny" 0: the tiled GEMMs); "pdl" is honoured.
+ * The entry xn = RMSNorm(x) ln1[0] comes from the path's own norm kernel.  An fp32 context, an unfinalised stage, B outside [1, 64],
+ * ctx_len outside [0, max_ctx) and max_ctx beyond the decode-attention limit are refused with CVK_ERR_INVALID before any device work. */
 int cvk_op_lm_decode_layers(cvk_ctx* ctx, int B, const int* ctx_len_host, int max_ctx, float* x, float* k_cache, float* v_cache,
                             float* xn_out, float* att_out, float* ffa_out, void* stream);
 /* element types of the cvk_op_conv_gemm operand and outputs */

@@ -107,9 +107,9 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, ctx_len):
 # ------------------------------------------------------------------------------------------------ LM decode layer
 LM_D, LM_DFF = olm.D, olm.D_FF              # 896, 4864
 LAYER_ROUNDING = {
-    # where a decode path stores a bf16 value that the next stage reads: the fused chain and the persistent kernel keep the qkv and
-    # gate/up projections in fp32 (split-K partial sums reduced by the attention unit, SwiGLU in the GEMM epilogue); the per-op chain
-    # stores both as bf16 first
+    # where a decode path stores a bf16 value that the next stage reads: the fused chain keeps the qkv and gate/up projections in
+    # fp32 (split-K partial sums reduced by the attention unit, SwiGLU in the GEMM epilogue); the per-op chain stores both as bf16
+    # first
     None: (),
     "fused": ("xn", "qkv_rot", "att", "ffa"),
     "per-op": ("xn", "qkv", "qkv_rot", "att", "gu", "ffa"),
