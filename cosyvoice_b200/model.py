@@ -20,7 +20,24 @@ from . import cvk
 
 TOKEN_MEL_RATIO = 2          # cosyvoice2.yaml:14
 PRE_LOOKAHEAD = 3            # cosyvoice2.yaml:46
+STREAM_CHUNK_FRAMES = 25 * TOKEN_MEL_RATIO     # cosyvoice2.yaml:16 static_chunk_size, in mel frames
 SAMPLES_PER_FRAME = 480
+
+
+# the streaming chunk schedule of tts(stream=True) (cli/model.py:346-364), shared by tts() and the batched poll loop
+def _first_hop_pad(P, hop):
+    """tokens added to the first hop so that a P-token prompt and the first hop end on the hop grid"""
+    return int(np.ceil(P / hop) * hop - P)
+
+
+def _this_hop(hop, pad, token_offset):
+    """the tokens of the next chunk: the first one also takes the prompt's padding"""
+    return hop + pad if token_offset == 0 else hop
+
+
+def _hop_ready(n_tokens, token_offset, this_hop):
+    """the next chunk's tokens and their look-ahead have arrived"""
+    return n_tokens - token_offset >= this_hop + PRE_LOOKAHEAD
 
 
 class SilentTokenFilter:
@@ -616,12 +633,17 @@ class B200CosyVoice2Model:
             emb = torch.cat([e.reshape(1, -1).to(d, non_blocking=True) for e in embeddings], 0)
             return self.ctx.flow_inference(toks, tl, pf, pl, emb, n_timesteps=self.n_timesteps, streaming=streaming, finalize=finalize)
 
+    def _vocoder_noise(self, n, noise_fn=None):
+        """vocoder noise for n samples: from noise_fn when given, else from the model's noise_fn hook or its generator"""
+        noise_fn = noise_fn if noise_fn is not None else self.noise_fn
+        if noise_fn is not None:
+            return noise_fn(n).to(self.device)
+        return torch.randn(n, 9, device=self.device, generator=self.generator)
+
     def hift_batch(self, mel_tm, lens, cache_source=None, cache_lens=None, noise=None):
         with torch.cuda.stream(self.stream), self.ctx.lock:
-            if noise is None and self.noise_fn is not None:
-                noise = self.noise_fn(sum(lens) * SAMPLES_PER_FRAME)
             if noise is None:
-                noise = torch.randn(sum(lens) * SAMPLES_PER_FRAME, 9, device=self.device, generator=self.generator)
+                noise = self._vocoder_noise(sum(lens) * SAMPLES_PER_FRAME)
             return self.ctx.hift_inference(mel_tm, lens, noise, cache_source, cache_lens)
 
     def tts_batch_device(self, inputs, uniforms=None, noise=None):
@@ -722,22 +744,25 @@ class B200CosyVoice2Model:
         self.stream.synchronize()
         return h
 
+    def _session_chunk_ok(self, P, prompt_frames, n_tokens, token_offset, has_session):
+        """Whether the streaming chunk of the first n_tokens speech tokens (look-ahead included) past token_offset can come from a
+        cached flow session: it starts and ends on the STREAM_CHUNK_FRAMES grid, the prompt mel has TOKEN_MEL_RATIO frames per
+        prompt token (P of them), its frames fit in stream_cache_frames, and the request has held a session since its first chunk."""
+        total = TOKEN_MEL_RATIO * (P + n_tokens - PRE_LOOKAHEAD)
+        done = TOKEN_MEL_RATIO * (P + token_offset) if token_offset else 0
+        return (total % STREAM_CHUNK_FRAMES == 0 and done % STREAM_CHUNK_FRAMES == 0 and prompt_frames == TOKEN_MEL_RATIO * P
+                and total <= self.stream_cache_frames and (has_session or token_offset == 0))
+
     def _flow_stream_chunk(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid):
         """The frames of this streaming chunk from the request's cached flow session, or None when the request cannot use one
-        (chunk ends off the 50-frame grid, prompt mel not 2 frames per prompt token, longer than the cache): the caller then
-        recomputes the prefix like the reference."""
+        (_session_chunk_ok): the caller then recomputes the prefix like the reference."""
         if not self.incremental_flow or uuid not in self.tts_speech_token_dict:
             return None
         fs = self.flow_stream_dict.get(uuid)
         if fs is False:
             return None
-        P = int(prompt_token.shape[1])
-        total = TOKEN_MEL_RATIO * (P + int(token.shape[1]) - PRE_LOOKAHEAD)
-        done = TOKEN_MEL_RATIO * (P + token_offset) if token_offset else 0
-        chunk = 2 * 25                                   # cosyvoice2.yaml:16 static_chunk_size x token_mel_ratio
-        ok = (total % chunk == 0 and done % chunk == 0 and int(prompt_feat.shape[1]) == TOKEN_MEL_RATIO * P
-              and total <= self.stream_cache_frames and (fs is not None or token_offset == 0))
-        if not ok:
+        if not self._session_chunk_ok(int(prompt_token.shape[1]), int(prompt_feat.shape[1]), int(token.shape[1]), token_offset,
+                                      fs is not None):
             if fs:
                 self._release_flow_stream(uuid)
             self.flow_stream_dict[uuid] = False
@@ -770,34 +795,54 @@ class B200CosyVoice2Model:
                 self.stream.synchronize()
                 self.ctx.flow_stream_destroy(fs)
 
+    def _token2wav_mel(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream, finalize):
+        """The flow half of token2wav: the mel frames past token_offset, from the request's cached flow session when a streaming
+        chunk can use one (_flow_stream_chunk), else from the flow over the whole prefix like the reference (cli/model.py:294-303)."""
+        token = token.to(torch.int32)
+        mel = self._flow_stream_chunk(token, prompt_token, prompt_feat, embedding, token_offset, uuid) if (stream and not finalize) else None
+        if mel is None:
+            mel, _ = self.flow_batch([token], [prompt_token], [prompt_feat], [embedding], streaming=stream, finalize=finalize)
+            mel = mel[token_offset * TOKEN_MEL_RATIO:]
+        return mel
+
+    def _vocode_cached(self, caches, mels, finals, noise_fns):
+        """CosyVoice2's vocoder bookkeeping (cli/model.py:304-326) for several requests in one vocoder call.  Request k has its cache
+        dict caches[k] (None before its first chunk), its new mel frames mels[k], finals[k] for its final call and its noise stream
+        noise_fns[k] (None: _vocoder_noise's default).  Its cached mel frames are prepended, its cached source is passed to the
+        vocoder and its waveform is cross-faded with its cached speech; unless final, its caches are renewed and the last
+        source_cache_len samples are held back.  Returns (the requests' waveforms on the device, their caches)."""
+        with torch.cuda.stream(self.stream):
+            tts_mel = [torch.cat([c["mel"], m], 0) if c is not None else m for c, m in zip(caches, mels)]
+            lens = [int(m.shape[0]) for m in tts_mel]
+            noise = torch.cat([self._vocoder_noise(n * SAMPLES_PER_FRAME, fn) for n, fn in zip(lens, noise_fns)], 0)
+            cached = [c for c in caches if c is not None]
+            cache_lens = [int(c["source"].shape[0]) if c is not None else 0 for c in caches] if cached else None
+            wav, src = self.hift_batch(torch.cat(tts_mel, 0), lens, torch.cat([c["source"] for c in cached]) if cached else None, cache_lens,
+                                       noise)
+            wavs, new_caches, o = [], [], 0
+            for c, m, n, final in zip(caches, tts_mel, lens, finals):
+                w, s = wav[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME], src[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME]
+                o += n
+                if c is not None:
+                    w = self._fade_in_out(w, c["speech"])
+                if not final:
+                    c = {"mel": m[-self.mel_cache_len:].clone(), "source": s[-self.source_cache_len:].clone(),
+                         "speech": w[-self.source_cache_len:].clone()}
+                    w = w[:-self.source_cache_len]
+                wavs.append(w)
+                new_caches.append(c)
+        return wavs, new_caches
+
     def token2wav(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream=False, finalize=False, speed=1.0):
         """cli/model.py:292-326"""
-        new_mel = self._flow_stream_chunk(token.to(torch.int32), prompt_token, prompt_feat, embedding, token_offset, uuid) \
-            if (stream and not finalize) else None
-        if new_mel is None:
-            mel, lens = self.flow_batch([token.to(torch.int32)], [prompt_token], [prompt_feat], [embedding], streaming=stream, finalize=finalize)
-        with torch.cuda.stream(self.stream):
-            tts_mel = new_mel if new_mel is not None else mel[token_offset * TOKEN_MEL_RATIO:]
-            cache = self.hift_cache_dict[uuid]
-            cache_source, cache_lens = None, None
-            if cache is not None:
-                tts_mel = torch.cat([cache["mel"], tts_mel], 0)
-                cache_source, cache_lens = cache["source"], [cache["source"].shape[0]]
-            if finalize is False:
-                wav, src = self.hift_batch(tts_mel.contiguous(), [tts_mel.shape[0]], cache_source, cache_lens)
-                if cache is not None:
-                    wav = self._fade_in_out(wav, cache["speech"])
-                self.hift_cache_dict[uuid] = {"mel": tts_mel[-self.mel_cache_len:].clone(), "source": src[-self.source_cache_len:].clone(),
-                                              "speech": wav[-self.source_cache_len:].clone()}
-                wav = wav[:-self.source_cache_len]
-            else:
-                if speed != 1.0:
-                    assert cache is None, "speed change only support non-stream inference mode"
-                    tts_mel, _ = self.mel_stretch(tts_mel, [tts_mel.shape[0]], [speed])
-                wav, src = self.hift_batch(tts_mel.contiguous(), [tts_mel.shape[0]], cache_source, cache_lens)
-                if cache is not None:
-                    wav = self._fade_in_out(wav, cache["speech"])
-        return wav.unsqueeze(0)
+        mel = self._token2wav_mel(token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream, finalize)
+        cache = self.hift_cache_dict[uuid]
+        if finalize and speed != 1.0:
+            assert cache is None, "speed change only support non-stream inference mode"
+            mel, _ = self.mel_stretch(mel, [mel.shape[0]], [speed])
+        wavs, caches = self._vocode_cached([cache], [mel], [finalize], [None])
+        self.hift_cache_dict[uuid] = caches[0]
+        return wavs[0].unsqueeze(0)
 
     def llm_job(self, text, prompt_text, llm_prompt_speech_token, llm_embedding, uuid):
         """cli/model.py:101-129 (non-generator text).  Tokens are appended to the session list as they arrive."""
@@ -831,6 +876,10 @@ class B200CosyVoice2Model:
         self.tts_speech_token_dict[uuid] = source_speech_token.flatten().tolist()
         self.llm_end_dict[uuid] = True
 
+    def _grow_hop(self, hop):
+        """the hop after a streaming chunk (cli/model.py:362)"""
+        return min(self.token_max_hop_len, hop * self.stream_scale_factor)
+
     def tts(self, text=torch.zeros(1, 0, dtype=torch.int32), flow_embedding=torch.zeros(0, 192), llm_embedding=torch.zeros(0, 192),
             prompt_text=torch.zeros(1, 0, dtype=torch.int32), llm_prompt_speech_token=torch.zeros(1, 0, dtype=torch.int32),
             flow_prompt_speech_token=torch.zeros(1, 0, dtype=torch.int32), prompt_speech_feat=torch.zeros(1, 0, 80),
@@ -846,21 +895,21 @@ class B200CosyVoice2Model:
             p = threading.Thread(target=self.vc_job, args=(source_speech_token, this_uuid))
         p.start()
         if stream is True:
+            # the hop lives on the instance, shared by concurrent requests, like the reference's self.token_hop_len
             token_offset = 0
-            P = flow_prompt_speech_token.shape[1]
-            prompt_token_pad = int(np.ceil(P / self.token_hop_len) * self.token_hop_len - P)
+            prompt_token_pad = _first_hop_pad(flow_prompt_speech_token.shape[1], self.token_hop_len)
             while True:
                 time.sleep(0.005)
-                this_hop = self.token_hop_len + prompt_token_pad if token_offset == 0 else self.token_hop_len
+                this_hop = _this_hop(self.token_hop_len, prompt_token_pad, token_offset)
                 toks = self.tts_speech_token_dict[this_uuid]
-                if len(toks) - token_offset >= this_hop + PRE_LOOKAHEAD:
+                if _hop_ready(len(toks), token_offset, this_hop):
                     this_tok = torch.tensor(toks[:token_offset + this_hop + PRE_LOOKAHEAD]).unsqueeze(0)
                     speech = self.token2wav(this_tok, flow_prompt_speech_token, prompt_speech_feat, flow_embedding, token_offset,
                                             this_uuid, stream=True, finalize=False)
                     token_offset += this_hop
-                    self.token_hop_len = min(self.token_max_hop_len, self.token_hop_len * self.stream_scale_factor)
+                    self.token_hop_len = self._grow_hop(self.token_hop_len)
                     yield {"tts_speech": self._to_host(speech)}
-                if self.llm_end_dict[this_uuid] is True and len(self.tts_speech_token_dict[this_uuid]) - token_offset < this_hop + PRE_LOOKAHEAD:
+                if self.llm_end_dict[this_uuid] is True and not _hop_ready(len(self.tts_speech_token_dict[this_uuid]), token_offset, this_hop):
                     break
             p.join()
             this_tok = torch.tensor(self.tts_speech_token_dict[this_uuid]).unsqueeze(0)
@@ -917,14 +966,6 @@ class B200CosyVoice2Model:
         with self._pool_lock:
             self._free_slots.append(slot)
             self._free_slots.sort()
-
-    def _noise_for(self, i, n, noise_fns):
-        """vocoder noise of request i for n samples: its own stream when given, else the model's hook or generator"""
-        if noise_fns is not None:
-            return noise_fns[i](n).to(self.device)
-        if self.noise_fn is not None:
-            return self.noise_fn(n).to(self.device)
-        return torch.randn(n, 9, device=self.device, generator=self.generator)
 
     def tts_stream_batch(self, inputs, uniforms=None, noise_fns=None):
         """Streaming synthesis of several requests at once: a generator of (i, {'tts_speech': float32 CPU [1, n]}).
@@ -1039,8 +1080,7 @@ class B200CosyVoice2Model:
         st = []
         for r in req:
             P = int(r["ptok"].shape[1])
-            st.append(dict(P=P, pad=int(np.ceil(P / hop0) * hop0 - P), hop=hop0, offset=0, slot=None, eligible=True, cache=None,
-                           done=False))
+            st.append(dict(P=P, pad=_first_hop_pad(P, hop0), hop=hop0, offset=0, slot=None, eligible=True, cache=None, done=False))
         p = None
         if lm_run is not None:
             p = threading.Thread(target=llm_job, name="cvk-stream-batch-lm", daemon=True)
@@ -1054,8 +1094,8 @@ class B200CosyVoice2Model:
                 for i, s in enumerate(st):
                     if s["done"]:
                         continue
-                    this_hop = s["hop"] + s["pad"] if s["offset"] == 0 else s["hop"]
-                    if len(toks[i]) - s["offset"] >= this_hop + PRE_LOOKAHEAD:
+                    this_hop = _this_hop(s["hop"], s["pad"], s["offset"])
+                    if _hop_ready(len(toks[i]), s["offset"], this_hop):
                         ready.append((i, this_hop))
                     elif end or own_end[i]:
                         finishing.append(i)
@@ -1076,51 +1116,22 @@ class B200CosyVoice2Model:
                 self.stream.synchronize()
 
     def _stream_vocode(self, voc, mels, st, finishing, noise_fns):
-        """the vocoder step of a poll round: requests `voc` (in order) with their new mel frames mels[i], in one vocoder call, each
-        with its own cached mel / source and token2wav's cross-fade (cli/model.py:292-326); requests in `finishing` make their
-        final call.  Returns {i: float32 CPU [n]}, copied to the host in one D2H for the round."""
-        outs = {}
+        """the vocoder step of a poll round: requests `voc` (in order) with their new mel frames mels[i], in one vocoder call with
+        token2wav's bookkeeping per request (_vocode_cached); requests in `finishing` make their final call.  Returns
+        {i: float32 CPU [n]}, copied to the host in one D2H for the round."""
+        wavs, caches = self._vocode_cached([st[i]["cache"] for i in voc], [mels[i] for i in voc], [i in finishing for i in voc],
+                                           [noise_fns[i] if noise_fns is not None else None for i in voc])
+        for i, c in zip(voc, caches):
+            st[i]["cache"] = c
+        return self._round_to_host(voc, wavs)
+
+    def _round_to_host(self, voc, wavs):
+        """{i: host copy of wavs[k]} for the requests i = voc[k], in one D2H"""
         with torch.cuda.stream(self.stream):
-            tts_mel, lens, cache_src, cache_lens, noise = [], [], [], [], []
-            for i in voc:
-                c = st[i]["cache"]
-                m_i = torch.cat([c["mel"], mels[i]], 0) if c is not None else mels[i]
-                tts_mel.append(m_i)
-                lens.append(int(m_i.shape[0]))
-                cache_lens.append(int(c["source"].shape[0]) if c is not None else 0)
-                if c is not None:
-                    cache_src.append(c["source"])
-                noise.append(self._noise_for(i, lens[-1] * SAMPLES_PER_FRAME, noise_fns))
-            with self.ctx.lock:
-                wav, src = self.ctx.hift_inference(torch.cat(tts_mel, 0), lens, torch.cat(noise, 0),
-                                                   torch.cat(cache_src) if cache_src else None, cache_lens if cache_src else None)
-            o = 0
-            for i, m_i, n in zip(voc, tts_mel, lens):
-                w, s_ = wav[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME], src[o * SAMPLES_PER_FRAME:(o + n) * SAMPLES_PER_FRAME]
-                o += n
-                c = st[i]["cache"]
-                if c is not None:
-                    w = self._fade_in_out(w, c["speech"])
-                if i in finishing:
-                    outs[i] = w
-                else:
-                    st[i]["cache"] = {"mel": m_i[-self.mel_cache_len:].clone(), "source": s_[-self.source_cache_len:].clone(),
-                                      "speech": w[-self.source_cache_len:].clone()}
-                    outs[i] = w[:-self.source_cache_len]
-            flat = torch.cat([outs[i] for i in voc]).cpu()       # one D2H for the round
+            flat = torch.cat(wavs).cpu()
         if self.stream is not None:
             self.stream.synchronize()
-        return self._split_host(voc, outs, flat)
-
-    @staticmethod
-    def _split_host(voc, outs, flat):
-        """the host copy `flat` of the device tensors outs[i] (concatenated in voc order), split back per request"""
-        host, o = {}, 0
-        for i in voc:
-            n = int(outs[i].shape[0])
-            host[i] = flat[o:o + n]
-            o += n
-        return host
+        return dict(zip(voc, flat.split([int(w.shape[0]) for w in wavs])))
 
     def _stream_round(self, req, st, toks, ready, finishing, noise_fns):
         """one poll round of tts_stream_batch: flow for every ready / finishing request (at most three calls), then one vocoder call
@@ -1129,16 +1140,10 @@ class B200CosyVoice2Model:
         slot_grp, prefix_grp = [], []
         for i, this_hop in ready:
             s = st[i]
-            ptok, pfeat = req[i]["ptok"], req[i]["pfeat"]
             n_tok = s["offset"] + this_hop + PRE_LOOKAHEAD
             this_tok = torch.tensor(toks[i][:n_tok], dtype=torch.int32).unsqueeze(0)
             if s["eligible"]:
-                # the rule of _flow_stream_chunk: chunk ends on the 50-frame grid, 2 prompt frames per prompt token, capacity, and a
-                # slot from the request's first chunk on
-                total = TOKEN_MEL_RATIO * (s["P"] + n_tok - PRE_LOOKAHEAD)
-                done = TOKEN_MEL_RATIO * (s["P"] + s["offset"]) if s["offset"] else 0
-                ok = (total % 50 == 0 and done % 50 == 0 and int(pfeat.shape[1]) == TOKEN_MEL_RATIO * s["P"]
-                      and total <= self.stream_cache_frames and (s["slot"] is not None or s["offset"] == 0))
+                ok = self._session_chunk_ok(s["P"], int(req[i]["pfeat"].shape[1]), n_tok, s["offset"], s["slot"] is not None)
                 if ok and s["slot"] is None:
                     s["slot"] = self._take_slot()
                     s["begin"] = s["slot"] is not None
@@ -1178,7 +1183,7 @@ class B200CosyVoice2Model:
         outs = self._stream_vocode(voc, mels, st, finishing, noise_fns) if voc else {}
         for i, this_hop in ready:
             st[i]["offset"] += this_hop
-            st[i]["hop"] = min(self.token_max_hop_len, st[i]["hop"] * self.stream_scale_factor)
+            st[i]["hop"] = self._grow_hop(st[i]["hop"])
         results = []
         for i in order:
             results.append((i, {"tts_speech": outs[i].unsqueeze(0) if i in outs else torch.zeros(1, 0)}))

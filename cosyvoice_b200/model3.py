@@ -1,9 +1,10 @@
 """Host-side mirror of the reference's CosyVoice3Model (cosyvoice/cli/model.py:397-450) over libcvk.
 
 CosyVoice3Model inherits CosyVoice2Model.tts (thread-per-request LM job, chunk schedule hop 25 -> 50 -> 100 with 3 look-ahead
-tokens) and replaces token2wav: the flow is the DiT one (stage "flow3"), the vocoder is the causal one (stage "hift3"), and instead
-of the CosyVoice2 mel / source / speech caches with a cross-fade it keeps ALL mel frames produced so far, re-runs the causal vocoder
-over them and emits the samples beyond ``speech_offset``.  This class follows that bookkeeping literally.
+tokens) and replaces token2wav: the flow is the DiT one (stage "flow3", through the inherited flow half of token2wav with
+``flow_batch`` below and DiT flow sessions), the vocoder is the causal one (stage "hift3"), and instead of the CosyVoice2 mel /
+source / speech caches with a cross-fade it keeps ALL mel frames produced so far, re-runs the causal vocoder over them and emits
+the samples beyond ``speech_offset``.  ``_append_mel`` and ``_new_speech`` keep that bookkeeping on a request's cache dict.
 
 Offline requests also batch: the inherited ``tts_batch`` / ``tts_batch_device`` run the LM, the DiT flow and the causal vocoder
 (``hift_batch`` below) once for the whole batch, and ``TtsBatcher`` serves CosyVoice3 offline requests through them.  Each request
@@ -12,16 +13,16 @@ predictor sums in an order that does not depend on the batch.
 
 Streaming requests batch too: ``tts_stream_batch`` / ``tts_bistream_batch`` run the inherited poll loop (multi-slot DiT flow
 sessions, ``flow_batch`` for prefix recomputes and final calls) with the vocoder step replaced by ``_stream_vocode`` below, which
-keeps token2wav's bookkeeping per request (all mel so far, ``speech_offset``) and vocodes every request of a round - streaming
-chunks and final calls together - in one ``hift3_inference_rows`` call with a finalize flag per utterance.  ``TtsBatcher``
-serves CosyVoice3 streaming requests through them.
+keeps token2wav's bookkeeping per request and vocodes every request of a round - streaming chunks and final calls together - in
+one ``hift3_inference_rows`` call with a finalize flag per utterance.  ``TtsBatcher`` serves CosyVoice3 streaming requests
+through them.
 
 The class is checked on the CPU against the reference's own CosyVoice3Model.tts with the device primitives faked by the oracle
 (tests/test_host_logic_cpu.py, tests/test_tts3_batch_cpu.py, tests/test_stream3_batch_cpu.py) and on the GPU against the
 reference's waveform (tests/test_zz_model3_gpu.py, tests/test_zz_tts3_batch_gpu.py, tests/test_zz_stream3_batch_gpu.py)."""
 import torch
 
-from .model import B200CosyVoice2Model, SAMPLES_PER_FRAME, TOKEN_MEL_RATIO, _count
+from .model import B200CosyVoice2Model, SAMPLES_PER_FRAME, _count
 
 
 class B200CosyVoice3Model(B200CosyVoice2Model):
@@ -114,52 +115,43 @@ class B200CosyVoice3Model(B200CosyVoice2Model):
         the round, finalize for the requests in `finishing` - and emit the samples past its speech_offset.  Returns
         {i: float32 CPU [n]}, copied to the host in one D2H for the round.  noise_fns is always None here (refused by
         _check_stream_batch)."""
-        outs = {}
         with torch.cuda.stream(self.stream):
-            hist, lens, fin = [], [], []
             for i in voc:
-                c = st[i]["cache"]
-                if c is None:
-                    c = st[i]["cache"] = {"mel": mels[i], "speech_offset": 0}
-                else:
-                    c["mel"] = torch.cat([c["mel"], mels[i]], 0)
-                hist.append(c["mel"])
-                lens.append(int(c["mel"].shape[0]))
-                fin.append(i in finishing)
+                st[i]["cache"] = self._append_mel(st[i]["cache"], mels[i])
+            lens, fin = [int(st[i]["cache"]["mel"].shape[0]) for i in voc], [i in finishing for i in voc]
             with self.ctx.lock:
-                wav, _, _ = self.ctx.hift3_inference_rows(torch.cat(hist, 0), lens, fin)
-            o = 0
+                wav, _, _ = self.ctx.hift3_inference_rows(torch.cat([st[i]["cache"]["mel"] for i in voc], 0), lens, fin)
+            outs, o = [], 0
             for i, n, f in zip(voc, lens, fin):
                 n_out = SAMPLES_PER_FRAME * (n if f else n - 8)
-                c = st[i]["cache"]
-                w = wav[o:o + n_out][c["speech_offset"]:]
-                c["speech_offset"] += w.shape[0]
-                outs[i] = w
+                outs.append(self._new_speech(st[i]["cache"], wav[o:o + n_out]))
                 o += n_out
-            flat = torch.cat([outs[i] for i in voc]).cpu()       # one D2H for the round
-        if self.stream is not None:
-            self.stream.synchronize()
-        return self._split_host(voc, outs, flat)
+        return self._round_to_host(voc, outs)
+
+    @staticmethod
+    def _append_mel(cache, mel):
+        """a request's cache dict (None before its first chunk) with `mel` appended to its mel history"""
+        if cache is None:
+            return {"mel": mel, "speech_offset": 0}
+        cache["mel"] = torch.cat([cache["mel"], mel], 0)
+        return cache
+
+    @staticmethod
+    def _new_speech(cache, wav):
+        """the samples of `wav` (the vocoder over the request's whole mel history) past its speech_offset, which moves past them"""
+        wav = wav[cache["speech_offset"]:]
+        cache["speech_offset"] += wav.shape[0]
+        return wav
 
     def token2wav(self, token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream=False, finalize=False, speed=1.0):
         """cli/model.py:425-450"""
-        new_mel = self._flow_stream_chunk(token.to(torch.int32), prompt_token, prompt_feat, embedding, token_offset, uuid) \
-            if (stream and not finalize) else None
-        if new_mel is None:
-            mel, _ = self.flow_batch([token.to(torch.int32)], [prompt_token], [prompt_feat], [embedding], streaming=stream, finalize=finalize)
+        mel = self._token2wav_mel(token, prompt_token, prompt_feat, embedding, token_offset, uuid, stream, finalize)
         with torch.cuda.stream(self.stream):
-            tts_mel = new_mel if new_mel is not None else mel[token_offset * TOKEN_MEL_RATIO:]
-            cache = self.hift_cache_dict[uuid]
-            if cache is not None:
-                tts_mel = torch.cat([cache["mel"], tts_mel], 0)
-                cache["mel"] = tts_mel
-            else:
-                cache = self.hift_cache_dict[uuid] = {"mel": tts_mel, "speech_offset": 0}
+            cache = self.hift_cache_dict[uuid] = self._append_mel(self.hift_cache_dict[uuid], mel)
+            tts_mel = cache["mel"]
             if speed != 1.0:
                 assert token_offset == 0 and finalize is True, "speed change only support non-stream inference mode"
                 tts_mel, _ = self.mel_stretch(tts_mel, [tts_mel.shape[0]], [speed])
             with self.ctx.lock:
                 wav, _, _ = self.ctx.hift3_inference(tts_mel.contiguous(), [tts_mel.shape[0]], finalize=finalize)
-            wav = wav[cache["speech_offset"]:]
-            cache["speech_offset"] += wav.shape[0]
-        return wav.unsqueeze(0)
+        return self._new_speech(cache, wav).unsqueeze(0)
