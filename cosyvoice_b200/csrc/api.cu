@@ -7,7 +7,8 @@
 void hift_build(cvk_ctx* ctx);
 void hift_f0(cvk_ctx* ctx, const float* mel, const int* lens, int B, float* f0_out, cudaStream_t st);
 void hift_source(cvk_ctx* ctx, const float* f0, const int* lens, int B, const float* noise, float* source_out, cudaStream_t st);
-void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* source, float* wav, cudaStream_t st);
+void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* source, float* wav, cudaStream_t st, int unit = -1,
+                 float* hidden = nullptr);
 void hift_inference(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* noise, const float* cache_source,
                     const int* cache_lens, float* wav, float* source_out, cudaStream_t st);
 void flow_build(cvk_ctx* ctx, const int* cfg, int ncfg);
@@ -27,7 +28,7 @@ void llm_session_destroy(cvk_ctx* ctx, cvk_lm_session* s);
 void hift3_build(cvk_ctx* ctx);
 void hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_noise, long long n, int on_device);
 void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int* finalize, int B, float* wav, float* f0_out,
-                     float* source_out, cudaStream_t st);
+                     float* source_out, cudaStream_t st, int unit = -1, float* hidden = nullptr);
 void dit_build(cvk_ctx* ctx, const int* cfg, int ncfg);
 void dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond, const int* lens,
                    int B, int streaming, float* out, cudaStream_t st, int n_blocks = 0, float* hidden = nullptr);
@@ -791,6 +792,21 @@ int cvk_hift3_inference_rows(cvk_ctx* ctx, const float* mel, const int* lens_hos
   CVK_API_BEGIN
   CVK_REQUIRE(mel && lens_host && finalize_host && wav && B > 0, "cvk_hift3_inference_rows: bad arguments");
   hift3_inference(ctx, mel, lens_host, finalize_host, B, wav, f0_out, source_out, (cudaStream_t)stream);
+  CVK_API_END
+}
+int cvk_hift_hidden(cvk_ctx* ctx, int causal, const float* mel, const int* lens_host, const int* finalize_host, int B, const float* source,
+                    int unit, float* out, void* stream) {
+  CVK_API_BEGIN
+  CVK_REQUIRE(mel && lens_host && out && B > 0 && (causal == 0 || causal == 1), "cvk_hift_hidden: bad arguments");
+  CVK_REQUIRE(unit >= 0 && unit <= 20, "cvk_hift_hidden: unit outside [0, 20]");
+  if (causal) {
+    std::vector<int> flags(B, 1);
+    if (finalize_host) flags.assign(finalize_host, finalize_host + B);
+    hift3_inference(ctx, mel, lens_host, flags.data(), B, nullptr, nullptr, nullptr, (cudaStream_t)stream, unit, out);
+  } else {
+    CVK_REQUIRE(source != nullptr, "cvk_hift_hidden: stage \"hift\" reads the given source");
+    hift_decode(ctx, mel, lens_host, B, source, nullptr, (cudaStream_t)stream, unit, out);
+  }
   CVK_API_END
 }
 int cvk_dit_estimator(cvk_ctx* ctx, const float* x, const float* mu, const float* t, const float* spks, const float* cond,

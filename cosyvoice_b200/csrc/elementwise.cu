@@ -490,6 +490,7 @@ void unpack_rows(cvk_ctx* ctx, cudaStream_t st, const Mat& in, const Seqs& s, in
   int bx = grid_for((size_t)s.max_len * C);
   if (bx > 256) bx = 256;
   if (in.dtype == DT_F32) unpack_rows_kernel<float><<<dim3(bx, s.B), 256, 0, st>>>(in.f32(), in.ld, s.d_start, s.d_len, skip, nullptr, dense, C, off);
+  else if (in.dtype == DT_F16) unpack_rows_kernel<__half><<<dim3(bx, s.B), 256, 0, st>>>((const __half*)in.p, in.ld, s.d_start, s.d_len, skip, nullptr, dense, C, off);
   else unpack_rows_kernel<bf16><<<dim3(bx, s.B), 256, 0, st>>>(in.b16(), in.ld, s.d_start, s.d_len, skip, nullptr, dense, C, off);
   ctx->launches++;
   CVK_LAUNCH_CHECK();

@@ -451,10 +451,19 @@ static void run_resblock(cvk_ctx* ctx, cudaStream_t st, const ResBlockW& rb, con
   }
 }
 
-// mel packed + source packed -> conv_post output [R3, 18] fp32 (ld 24)
+// mel packed + source packed -> conv_post output [R3, 18] fp32 (ld 24).
+// hidden != nullptr (the test-only read-out cvk_hift_hidden): stop at read-out `unit` and write its sequence rows densely, widened to
+// fp32, to `hidden`; the returned Mat is then empty.  Read-outs: 0 the source STFT (18 columns), 1 conv_pre + LReLU (xin); per level
+// i: 2 + 6i the up-sampled xu (after the reflect pad at i = 2), 3 + 6i xu + the source branch, 4 + 6i .. 6 + 6i the running resblock
+// sum xs, 7 + 6i the level output; 20 conv_post.
 static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat& mel32, const float* src_packed,
-                     const HiftModel* m = nullptr, const int* d_len_sig = nullptr) {
+                     const HiftModel* m = nullptr, const int* d_len_sig = nullptr, int unit = -1, float* hidden = nullptr) {
   if (!m) m = ctx->hift;
+  auto read_out = [&](int u, const Mat& x, const Seqs& s, int C) {
+    if (!hidden || u != unit) return false;
+    unpack_rows(ctx, st, x, s, 0, hidden, C);
+    return true;
+  };
   // tensor-core mode: IEEE-half operands (10-bit mantissa, the class of the TF32 convolutions the reference's "fp32" vocoder runs
   // on under cuDNN's defaults) unless the option hift_f16 is off (then bf16, 7 bits: narrower than the reference)
   const int adt = (ctx->act_dtype == DT_BF16 && m->half_weights) ? DT_F16 : ctx->act_dtype;
@@ -473,6 +482,7 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
     ctx->launches++;
     CVK_LAUNCH_CHECK();
   }
+  if (read_out(0, stft, s3, 18)) return Mat();
   // conv_pre (+ leaky_relu 0.1 for ups[0])
   Mat mel_a = mel32;
   if (adt != DT_F32) {
@@ -488,6 +498,7 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
     e.out = xin;
     conv_gemm(ctx, st, mel_a, m->conv_pre, e);
   }
+  if (read_out(1, xin, s0, 512)) return Mat();
   const Seqs* sin_ = &s0;
   // ping-pong buffers for the activated level outputs, sized for the largest level (x120, 64 ch)
   const size_t lvl_elems = (size_t)g.lv[2].R * 64 > (size_t)g.lv[1].R * 128 ? (size_t)g.lv[2].R * 64 : (size_t)g.lv[1].R * 128;
@@ -512,6 +523,7 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
       ctx->launches++;
       CVK_LAUNCH_CHECK();
     }
+    if (read_out(2 + 6 * i, xu, sl, C)) return Mat();
     // source branch
     Mat si = arena_mat(ctx, DT_F32, sl.R, C);
     Mat a = arena_mat(ctx, adt, sl.R, C);
@@ -529,16 +541,19 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
       conv_gemm(ctx, st, view, m->src_down[i], e);
     }
     run_resblock(ctx, st, m->src_rb[i], sl, si, a, ya, xr, xu, 1);   // xu += source_resblock(si)
+    if (read_out(3 + 6 * i, xu, sl, C)) return Mat();
     // main resblocks, summed into xs
     Mat xs = arena_mat(ctx, DT_F32, sl.R, C);
     for (int j = 0; j < 3; ++j) {
       const ResBlockW& rb = m->rb[i * 3 + j];
       act_copy(ctx, st, xu, ACT_SNAKE, 0.f, rb.a1[0], sl.d_row2seq, a);
       run_resblock(ctx, st, rb, sl, xu, a, ya, xr, xs, j > 0);
+      if (read_out(4 + 6 * i + j, xs, sl, C)) return Mat();
     }
     // x = xs / 3 ; leaky_relu (0.1 before the next ups, default 0.01 before conv_post, generator.py:513,532)
     Mat nxt(nxt_buf[i & 1], adt, sl.R, C, C);
     act_copy_scaled(ctx, st, xs, 1.f / 3.f, ACT_LRELU, i < 2 ? 0.1f : 0.01f, nullptr, sl.d_row2seq, nxt);
+    if (read_out(7 + 6 * i, nxt, sl, C)) return Mat();
     xin = nxt;
     sin_ = &sl;
     ctx->arena.off = mark;
@@ -550,6 +565,7 @@ static Mat hift_body(cvk_ctx* ctx, cudaStream_t st, const HiftGeom& g, const Mat
     e.out = xp;
     conv_gemm(ctx, st, xin, m->conv_post, e);
   }
+  if (read_out(20, xp, s3, 18)) return Mat();
   return xp;
 }
 
@@ -623,7 +639,9 @@ void hift_source(cvk_ctx* ctx, const float* f0_dense, const int* lens, int B, co
   CVK_LAUNCH_CHECK();
 }
 
-void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* source, float* wav, cudaStream_t st) {
+// unit / hidden: cvk_hift_hidden's read-out instead of the waveform (hift_body)
+void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const float* source, float* wav, cudaStream_t st, int unit,
+                 float* hidden) {
   CVK_REQUIRE(ctx->hift, "hift stage not finalised");
   ctx->arena.reset();
   HiftGeom g = hift_geom(ctx, lens, B, st);
@@ -634,7 +652,8 @@ void hift_decode(cvk_ctx* ctx, const float* mel, const int* lens, int B, const f
   copy_samples_kernel<<<dim3(256, B), 256, 0, st>>>(source, src, g.s0.d_start, g.s0.d_len, off, 1);
   ctx->launches++;
   CVK_LAUNCH_CHECK();
-  Mat xp = hift_body(ctx, st, g, mel32, src);
+  Mat xp = hift_body(ctx, st, g, mel32, src, nullptr, nullptr, unit, hidden);
+  if (hidden) return;
   hift_istft(ctx, st, g, lens, xp, wav);
 }
 
@@ -718,12 +737,24 @@ __global__ void upsample_causal_poly_kernel(const float* __restrict__ w /*[Cout]
   }
 }
 
-// ConvW.w32 [N][taps][K] fp32 -> [taps][K][N] fp64
-__global__ void f64_weight_kernel(const float* __restrict__ w, double* __restrict__ o, int N, int taps, int K) {
-  const size_t total = (size_t)N * taps * K;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int k = (int)(i % K), j = (int)((i / K) % taps), n = (int)(i / ((size_t)K * taps));
-    o[((size_t)j * K + k) * N + n] = (double)w[i];
+// weight norm folded in float64, as the reference's float64 predictor module computes it (generator.py:716-717 converts the module,
+// so its parametrization runs in double): g [N], v [N][K][taps] fp32 -> w = g v / ||v|| as [taps][K][N] fp64.  One block per n.
+__global__ void f64_weight_norm_kernel(const float* __restrict__ g, const float* __restrict__ v, double* __restrict__ o, int N, int K,
+                                       int taps) {
+  __shared__ double red[32];
+  const int n = blockIdx.x, inner = K * taps;
+  const float* vp = v + (size_t)n * inner;
+  double s = 0.0;
+  for (int i = threadIdx.x; i < inner; i += blockDim.x) s += (double)vp[i] * (double)vp[i];
+  for (int o2 = 16; o2 > 0; o2 >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o2);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double tot = 0.0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+  const double scale = (double)g[n] / sqrt(tot);
+  for (int i = threadIdx.x; i < inner; i += blockDim.x) {
+    const int k = i / taps, j = i % taps;
+    o[((size_t)j * K + k) * N + n] = (double)vp[i] * scale;
   }
 }
 __global__ void f64_copy_kernel(const float* __restrict__ a, double* __restrict__ o, size_t n) {
@@ -913,14 +944,18 @@ void hift3_build(cvk_ctx* ctx) {
   const std::string P = "hift3.";
   // float64 f0 predictor: conv0 k4 looking RIGHT (f0_predictor.py:71), then four causal k3 convolutions
   for (int i = 0; i < 5; ++i) {
-    ConvW c = wn_conv(ctx, P + "f0_predictor.condnet." + std::to_string(2 * i), 1, i == 0 ? 0 : -2);
+    const std::string pre = P + "f0_predictor.condnet." + std::to_string(2 * i);
+    ConvW c = wn_conv(ctx, pre, 1, i == 0 ? 0 : -2);
     CVK_CHECK_CUDA(cudaDeviceSynchronize());
     F64Conv& f = x->conv[i];
     f.N = c.N; f.K = c.K; f.taps = c.taps; f.shift0 = c.shift0;
     CVK_REQUIRE(f.K % F0_BK == 0 && f.N % F0_BN == 0 && f.taps == (i == 0 ? 4 : 3), "unexpected f0 predictor convolution shape");
     f.w = (double*)ctx->dmalloc((size_t)c.N * c.taps * c.K * sizeof(double));
     f.bias = (double*)ctx->dmalloc((size_t)c.N * sizeof(double));
-    f64_weight_kernel<<<256, 256>>>(c.w32, f.w, c.N, c.taps, c.K);
+    const bool pz = ctx->has_raw(pre + ".parametrizations.weight.original0");
+    const RawTensor& wg = ctx->get_raw(pre + (pz ? ".parametrizations.weight.original0" : ".weight_g"));
+    const RawTensor& wv = ctx->get_raw(pre + (pz ? ".parametrizations.weight.original1" : ".weight_v"));
+    f64_weight_norm_kernel<<<c.N, 256>>>(wg.p, wv.p, f.w, c.N, c.K, c.taps);
     f64_copy_kernel<<<4, 256>>>(c.bias, f.bias, (size_t)c.N);
     CVK_LAUNCH_CHECK();
   }
@@ -1008,9 +1043,10 @@ void hift3_set_noise(cvk_ctx* ctx, const float* rand_ini, const float* sine_nois
 
 // generator.py:714-726 with a finalize flag per utterance.  mel dense [sum T, 80]; utterance b's outputs, back to back:
 // finalize[b] != 0: wav 480 T, f0_out T, source_out 480 T (f0_out / source_out optional);
-// finalize[b] == 0 (streaming): wav 480 (T-8), f0_out T-3, source_out 480 (T-3)
+// finalize[b] == 0 (streaming): wav 480 (T-8), f0_out T-3, source_out 480 (T-3).
+// unit / hidden: cvk_hift_hidden's read-out instead of the waveform (hift_body)
 void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int* finalize, int B, float* wav, float* f0_out,
-                     float* source_out, cudaStream_t st) {
+                     float* source_out, cudaStream_t st, int unit, float* hidden) {
   const HiftModel* m = ctx->hift3;
   Hift3Extra* x = (Hift3Extra*)ctx->hift3_extra;
   CVK_REQUIRE(m && x && x->conv[0].w, "hift3 stage not finalised");
@@ -1092,6 +1128,7 @@ void hift3_inference(cvk_ctx* ctx, const float* mel, const int* lens, const int*
   }
   // ---- vocoder body (shared with CosyVoice2) + ISTFT
   // per utterance: the source length the STFT reads and the samples the ISTFT drops (nullptr when every utterance is final)
-  Mat xp = hift_body(ctx, st, g, mel32, src, m, any_stream ? s0.d_len : nullptr);
+  Mat xp = hift_body(ctx, st, g, mel32, src, m, any_stream ? s0.d_len : nullptr, unit, hidden);
+  if (hidden) return;
   hift_istft(ctx, st, g, lens_out.data(), xp, wav, any_stream ? upload_ints(ctx, drop, st) : nullptr);
 }

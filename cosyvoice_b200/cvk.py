@@ -83,6 +83,7 @@ SIGNATURES = {
     "cvk_hift3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]),
     "cvk_hift3_inference_rows": (ctypes.c_int, [_vp, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp, _vp, _vp, _vp]),
     "cvk_dit_estimator": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, _vp, _vp]),
+    "cvk_hift_hidden": (ctypes.c_int, [_vp, ctypes.c_int, _vp, _c_int_p, _c_int_p, ctypes.c_int, _vp, ctypes.c_int, _vp, _vp]),
     "cvk_dit_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _c_int_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_flow3_inference": (ctypes.c_int, [_vp, _vp, _c_int_p, _vp, _c_int_p, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]),
     "cvk_lm_session_create": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp)]),
@@ -375,6 +376,30 @@ class Context:
         self._check(self.lib.cvk_hift_inference(self.h, _ptr(mel), _ints(lens), len(lens), _ptr(noise), _ptr(cs), cl, _ptr(wav),
                                                 _ptr(src), _stream()))
         return wav, src
+
+    def hift_hidden(self, mel, lens, unit, source=None, causal=False, finalize=None):
+        """parity tests: read-out `unit` (0 .. 20) of the vocoder body, sequence rows only, as fp32.  causal=False: stage "hift" on the
+        given source [sum 480 T] (as hift_decode); causal=True: stage "hift3" on its own f0 and source (as hift3_inference_rows, every
+        utterance final when finalize is None).  With Tb the body frames (T, or T - 7 for a streaming utterance): unit 0 the source
+        STFT [sum 120 Tb + 1, 18], 1 conv_pre [sum Tb, 512], 2 + 6i .. 7 + 6i level i (up-sampled, + source branch, after each of the
+        three resblocks, level output) with [8 Tb, 40 Tb, 120 Tb + 1][i] rows and [256, 128, 64][i] channels, 20 conv_post
+        [sum 120 Tb + 1, 18]"""
+        mel = _f32(mel, self.device)
+        fin = [True] * len(lens) if finalize is None else [bool(f) for f in finalize]
+        tb = [int(l) - (0 if f or not causal else 7) for l, f in zip(lens, fin)]
+        if unit == 1:
+            rows, cols = sum(tb), 512
+        elif 2 <= unit <= 19:
+            i = (unit - 2) // 6
+            rows, cols = sum([8 * t, 40 * t, 120 * t + 1][i] for t in tb), [256, 128, 64][i]
+        else:
+            rows, cols = sum(120 * t + 1 for t in tb), 18
+        out = torch.empty(max(rows, 1), cols, device=self.device)
+        src = _f32(source, self.device) if source is not None else None
+        fl = _ints([int(f) for f in fin]) if finalize is not None else None
+        self._check(self.lib.cvk_hift_hidden(self.h, int(causal), _ptr(mel), _ints(lens), fl, len(lens), _ptr(src), int(unit), _ptr(out),
+                                             _stream()))
+        return out[:rows]
 
     # ------------------------------------------------------------------ flow
     def set_cfm_noise(self, noise_tm):

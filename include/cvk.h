@@ -196,6 +196,16 @@ int cvk_hift_decode(cvk_ctx* ctx, const float* mel, const int* lens_host, int B,
  * (generator.py:566-567, streaming glue).  Outputs wav [sum 480T], source [sum 480T]. */
 int cvk_hift_inference(cvk_ctx* ctx, const float* mel, const int* lens_host, int B, const float* noise,
                        const float* cache_source, const int* cache_lens_host, float* wav, float* source, void* stream);
+/* parity tests: one read-out point of the vocoder body, its sequence rows written densely (gap rows dropped) and widened to fp32.
+ * causal 0: stage "hift" with the arguments of cvk_hift_decode (source required); causal 1: stage "hift3" with those of
+ * cvk_hift3_inference_rows (its own f0 and source; finalize_host may be NULL = every utterance final).  With Tb the body's frames
+ * (T, or T - 7 for a streaming utterance): unit 0 the source STFT [sum 120 Tb + 1, 18] (re 0..8, im 9..17); 1 conv_pre + leaky
+ * ReLU 0.1 [sum Tb, 512]; level i in 0..2 with rows 8 Tb, 40 Tb, 120 Tb + 1 and 256 / 128 / 64 channels: 2 + 6i the up-sampled
+ * rows (after the reflect pad at i = 2), 3 + 6i those plus the source branch, 4 + 6i .. 6 + 6i the running sum of the three
+ * resblocks, 7 + 6i the level output (leaky ReLU of the sum / 3); 20 conv_post [sum 120 Tb + 1, 18].  A unit outside [0, 20] is
+ * refused before any device work. */
+int cvk_hift_hidden(cvk_ctx* ctx, int causal, const float* mel, const int* lens_host, const int* finalize_host, int B,
+                    const float* source, int unit, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------- flow (token -> mel)
  * replaces cosyvoice/flow/flow.py:235-281 (CausalMaskedDiffWithXvec.inference) and the engine plug-in points

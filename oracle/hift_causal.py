@@ -90,10 +90,16 @@ def resblock_causal(sd, prefix, x, k):
     return x
 
 
+def _w64(sd, prefix):
+    """weight norm folded in float64: the reference converts the predictor module to float64 before its parametrization runs"""
+    return H.weight_norm_effective(sd[prefix + ".parametrizations.weight.original0"].double(),
+                                   sd[prefix + ".parametrizations.weight.original1"].double())
+
+
 def f0_predict(sd, mel, finalize=True):
     """f0_predictor.py:95-103 in float64 (generator.py:716-717).  mel [B,80,T] -> f0 [B,T] (finalize) or [B,T-3]."""
     x = mel.double()
-    w0, b0 = _w(sd, "f0_predictor.condnet.0").double(), sd["f0_predictor.condnet.0.bias"].double()
+    w0, b0 = _w64(sd, "f0_predictor.condnet.0"), sd["f0_predictor.condnet.0.bias"].double()
     if finalize:
         x = causal_conv(x, w0, b0, right=True)
     else:
@@ -101,7 +107,7 @@ def f0_predict(sd, mel, finalize=True):
     x = F.elu(x)
     for i in range(1, 5):
         p = f"f0_predictor.condnet.{2 * i}"
-        x = F.elu(causal_conv(x, _w(sd, p).double(), sd[p + ".bias"].double()))
+        x = F.elu(causal_conv(x, _w64(sd, p), sd[p + ".bias"].double()))
     x = x.transpose(1, 2)
     f0 = torch.abs(F.linear(x, sd["f0_predictor.classifier.weight"].double(), sd["f0_predictor.classifier.bias"].double()).squeeze(-1))
     return f0.float()

@@ -832,3 +832,430 @@ FLOW_TOL = {"fp32": dict(enc_embed=1.5e-5, enc_layer=3.5e-5, enc_up=1.2e-5, enc_
 # from the exact one).  Bounds about twice that.
 FLOW_STACK_TOL = {"fp32": {"exact": (1.5e-5, 1.5e-5, 2.5e-5, 2.5e-5), "bf16-emulating": (0.04, 0.045, 0.06, 0.075)},
                   "bf16": {"exact": (0.04, 0.04, 0.06, 0.08), "bf16-emulating": (0.025, 0.025, 0.08, 0.095)}}
+
+
+# ------------------------------------------------------------------------------------------------ HiFT vocoders
+# The CosyVoice2 vocoder (oracle/hift.py, generator.py:507-569 of the reference) and the CosyVoice3 causal one (oracle/hift_causal.py,
+# generator.py:572-726) restated per sequence on time-major rows [rows, channels], in fp64, one read-out of cvk_hift_hidden at a
+# time: the f0 predictor (hift_f0), the harmonic source (hift_phase, hift_source), the source STFT (hift_stft, read-out 0), conv_pre
+# (1), per level i the up-sampling (hift_ups, 2 + 6i), the source branch (hift_source_branch, 3 + 6i), the three resblocks
+# (hift_resblock, 4 + 6i .. 6 + 6i), the level output (hift_level_out, 7 + 6i), conv_post (hift_conv_post, 20) and the ISTFT
+# (hift_istft).  Every convolution pads with zeros at the ends of the rows it is given, so a unit fed a window of a sequence's rows
+# is exact on the window's inner rows.  `causal` selects the CosyVoice3 form: left-padded convolutions, conv_pre looking 4 frames to
+# the right, nearest up-sampling + causal convolution, left-only source_downs padding, nearest phase up-sampling, stored noise
+# indexed from the utterance's start.  `rounding` ("fp16" for IEEE half, "bf16" for hift_f16 = 0, None for exact) rounds where the
+# 16-bit path stores a 16-bit value that the next kernel reads: the source STFT, the packed mel, xin, the Snake-activated operands a
+# and ya of every resblock convolution and the level outputs; xu, xs, the resblock stream and si stay fp32 in the kernels and
+# exact here.  `mutate` applies one of HIFT_MUTATIONS, the defects the sensitivity test of test_kernel_refs_cpu.py injects.
+from oracle import hift as ohift  # noqa: E402
+import numpy as np  # noqa: E402
+
+HIFT_CH = (512, 256, 128, 64)
+HIFT_RATE = (8, 40, 120)                 # level rows per mel frame (level 2 has one more row, the reflect pad, in front)
+HIFT_MUTATIONS = ("lrelu_post", "no_reflect", "reflect_back", "down_pad", "poly_phase", "snake_swap", "dil1", "no_div3", "hann_sym",
+                  "no_env", "phase_x", "clip_first", "uv_ge", "pre_left", "f0_look2")
+
+
+def hift_weights(sd, causal):
+    """the vocoder's weights in fp64 with every weight norm folded in float64 (the reference's CosyVoice3 f0 predictor runs as a
+    float64 module, generator.py:716-717, so its parametrization computes g v / ||v|| in double; the fp32 folds of the other
+    convolutions are within an fp32 ulp of it).  Keys: the state-dict names, "<conv>.weight" for the weight-normed ones."""
+    W = {"causal": causal}
+    for k, v in sd.items():
+        if k.endswith(".parametrizations.weight.original0"):
+            p = k[:-len(".parametrizations.weight.original0")]
+            g, vv = v.double(), sd[p + ".parametrizations.weight.original1"].double()
+            W[p + ".weight"] = g * vv / vv.flatten(1).norm(dim=1).view(g.shape)
+        elif not k.endswith(".parametrizations.weight.original1"):
+            W[k] = v.double()
+    return W
+
+
+def hift_test_state_dict(seed, causal, clip=False):
+    """synthetic vocoder weights (oracle SYNTH_GAINS); clip=True shifts the bias of conv_post's magnitude channels so that some
+    frames exceed ln 100 (the ISTFT's magnitude clip) and some samples exceed +-0.99 (the output clamp)"""
+    from oracle import hift_causal as ohc, weights as oweights
+    sd = oweights.synth_state_dict((ohc if causal else ohift).param_shapes(), seed, ohift.SYNTH_GAINS)
+    if clip:
+        b = sd["conv_post.bias"].clone()
+        b[:9] += 2.5
+        sd["conv_post.bias"] = b
+    return sd
+
+
+def _hrd(rounding):
+    return (lambda t: t) if rounding is None else (lambda t: round_to(t, rounding))
+
+
+def _conv(x, w, b, shift0, dil=1):
+    return conv_rows(x, w, dil, shift0) + b.double()
+
+
+def _elu(x):
+    return torch.where(x > 0, x, torch.expm1(x))
+
+
+def hift_f0(W, mel, mutate=None):
+    """f0 predictor (f0_predictor.py:56-59; causal: :60-103, conv 0 reading 3 frames ahead, the others causal) on one sequence's
+    mel rows [T, 80] -> f0 [T].  A streaming CosyVoice3 call's f0 (T - 3 frames) is the first T - 3 rows: its look-ahead frames are
+    the next rows of the same mel."""
+    x = mel.double()
+    for i in range(5):
+        p = f"f0_predictor.condnet.{2 * i}"
+        if W["causal"]:
+            sh = (-1 if mutate == "f0_look2" else 0) if i == 0 else -2
+        else:
+            sh = -1
+        x = _elu(_conv(x, W[p + ".weight"], W[p + ".bias"], sh))
+    return (x @ W["f0_predictor.classifier.weight"].t() + W["f0_predictor.classifier.bias"]).abs()[:, 0]
+
+
+def hift_phase(f0, emulate=False):
+    """SineGen2's per-frame phase (generator.py:255-257; the 1/480 linear down-sampling reads samples 480 d + 239 and 480 d + 240,
+    both of frame d, so it is the frame's own value): (cumsum over frames of (f0 h / 24000 mod 1)) 2 pi 480 for harmonics h = 1..9,
+    f0 [T] -> [T, 9].  emulate=True: the fp32 arithmetic of phase_kernel - fmodf(f0 h / 24000, 1) in fp32, a running sum in double
+    rounded to float, ((c 2) pi_f) 480 in fp32 - returned as float32 values in fp64."""
+    h = torch.arange(1, 10, dtype=torch.float64)
+    if not emulate:
+        rad = torch.remainder(f0.double()[:, None] * h / ohift.SR, 1.0)
+        return torch.cumsum(rad, 0) * 2 * math.pi * ohift.UPSCALE
+    f = f0.float().numpy().astype(np.float32)
+    fn = f[:, None] * np.arange(1, 10, dtype=np.float32)[None]
+    rad = np.fmod(fn / np.float32(24000.0), np.float32(1.0))
+    c = np.cumsum(rad.astype(np.float64), 0).astype(np.float32)
+    ph = ((c * np.float32(2.0)) * np.float32(math.pi)) * np.float32(480.0)
+    return torch.from_numpy(ph.astype(np.float64))
+
+
+def _interp_index(L, T):
+    """F.interpolate(scale_factor=480, mode='linear', align_corners=False) as source_kernel computes it in fp32: srcf =
+    fma(1/480, l + 0.5, -0.5) clamped at 0, i0 = trunc, i1 = min(i0 + 1, T - 1), l1 = srcf - i0, l0 = 1 - l1"""
+    l = np.arange(L, dtype=np.float32)
+    srcf = ((l + np.float32(0.5)).astype(np.float64) * np.float64(np.float32(1.0 / 480.0)) - 0.5).astype(np.float32)
+    srcf = np.maximum(srcf, np.float32(0.0))
+    i0 = srcf.astype(np.int64)
+    i1 = np.minimum(i0 + 1, T - 1)
+    l1 = (srcf - i0.astype(np.float32)).astype(np.float32)
+    return i0, i1, (np.float32(1.0) - l1).astype(np.float32), l1
+
+
+def hift_sample_phase(phase, causal, emulate=False):
+    """the phase at every sample [480 T, 9] from the per-frame phase [T, 9]: linear x480 up-sampling (align_corners False) or,
+    causal, nearest.  emulate=True: source_kernel's fp32 interpolation, fma(l0, p0, l1 * p1) with one rounding of the fused sum"""
+    T = phase.shape[0]
+    L = T * ohift.UPSCALE
+    if causal:
+        return phase.repeat_interleave(ohift.UPSCALE, 0)
+    i0, i1, l0, l1 = _interp_index(L, T)
+    if not emulate:
+        p = phase.double()
+        return torch.from_numpy(l0.astype(np.float64))[:, None] * p[i0] + torch.from_numpy(l1.astype(np.float64))[:, None] * p[i1]
+    p = phase.numpy().astype(np.float32)
+    t = (l1[:, None] * p[i1]).astype(np.float32)
+    ph = (l0.astype(np.longdouble)[:, None] * p[i0].astype(np.longdouble) + t.astype(np.longdouble)).astype(np.float32)
+    return torch.from_numpy(ph.astype(np.float64))
+
+
+def hift_source(W, f0, noise, emulate=False, mutate=None):
+    """the harmonic source of one sequence (SourceModuleHnNSF + SineGen2, generator.py:289-317, 358-375): f0 [T], noise [480 T, 9]
+    (the CosyVoice2 Gaussian draws, or the CosyVoice3 stored noise from the utterance's start) -> s [480 T].  emulate=False: exact
+    fp64 phase; emulate=True: the kernel's fp32 phase (hift_phase, hift_sample_phase), the rest in fp64."""
+    causal = W["causal"]
+    ph = hift_sample_phase(hift_phase(f0, emulate), causal, emulate)
+    f0u = f0.double().repeat_interleave(ohift.UPSCALE)[:, None]
+    uv = ((f0u >= ohift.VOICED_THR) if mutate == "uv_ge" else (f0u > ohift.VOICED_THR)).double()
+    sines = (ph if mutate == "phase_x" else torch.sin(ph)) * ohift.SINE_AMP
+    amp = uv * ohift.NOISE_STD + (1 - uv) * ohift.SINE_AMP / 3
+    sw = sines * uv + amp * noise.double()[:f0u.shape[0]]
+    return torch.tanh(sw @ W["m_source.l_linear.weight"].t() + W["m_source.l_linear.bias"])[:, 0]
+
+
+def _hann(mutate):
+    n = torch.arange(ohift.N_FFT, dtype=torch.float64)
+    return 0.5 - 0.5 * torch.cos(2 * math.pi * n / (ohift.N_FFT - 1 if mutate == "hann_sym" else ohift.N_FFT))
+
+
+def hift_stft(s, rounding=None, mutate=None):
+    """torch.stft(n_fft 16, hop 4, periodic Hann, center, reflect) of one source s [L] -> [L / 4 + 1, 18] (re 0..8, im 9..17)"""
+    x = torch.nn.functional.pad(s.double()[None, None], (8, 8), mode="reflect")[0, 0]
+    fr = x.unfold(0, ohift.N_FFT, ohift.HOP) * _hann(mutate)
+    n = torch.arange(ohift.N_FFT, dtype=torch.float64)
+    ang = 2 * math.pi * torch.arange(9, dtype=torch.float64)[:, None] * n[None] / ohift.N_FFT
+    return _hrd(rounding)(torch.cat([fr @ torch.cos(ang).t(), -(fr @ torch.sin(ang).t())], -1))
+
+
+def hift_conv_pre(W, mel, rows=None, rounding=None, mutate=None):
+    """conv_pre + leaky ReLU 0.1 (the first up-sampler's activation, stored as xin) on mel rows [T, 80] -> [rows (T), 512].  Causal:
+    k5 reading 4 frames to the right; a streaming call's body covers rows = T - 7 frames of the mel it is given"""
+    rd = _hrd(rounding)
+    sh = (-4 if mutate == "pre_left" else 0) if W["causal"] else -3
+    y = _conv(rd(mel.double()), W["conv_pre.weight"], W["conv_pre.bias"], sh)
+    return rd(act("lrelu", y, 0.1))[:rows]
+
+
+def hift_ups(W, i, x, head=True, mutate=None):
+    """ups[i] on the level input x [R, C_i] (xin or the previous level output) -> xu [u R (+1 at i = 2 when head), C_(i+1)].
+    CosyVoice2: ConvTranspose1d(stride u, padding (k - u) / 2); CosyVoice3: nearest x u then a causal k convolution.  At the last
+    level the reflect pad (1, 0) puts a copy of row 1 in front when the rows start the sequence (head)."""
+    u, k = ohift.UPS_RATES[i], ohift.UPS_KERNELS[i]
+    w, b = W[f"ups.{i}.weight"], W[f"ups.{i}.bias"]
+    R = x.shape[0]
+    shift = 1 if mutate == "poly_phase" else 0
+    if W["causal"]:
+        y = _conv(x.double().repeat_interleave(u, 0), w, b, -(k - 1) + shift)
+    else:
+        full = torch.nn.functional.conv_transpose1d(x.double().t()[None], w, None, stride=u)[0].t()     # [(R - 1) u + k, C]
+        full = torch.cat([full, full.new_zeros(1, full.shape[1])], 0)
+        p = (k - u) // 2 + shift
+        y = full[p:p + u * R] + b
+    if i == 2 and head:
+        if mutate == "no_reflect":
+            y = torch.cat([torch.zeros_like(y[:1]), y], 0)
+        elif mutate == "reflect_back":
+            y = torch.cat([y, y[-2:-1]], 0)
+        else:
+            y = torch.cat([y[1:2], y], 0)
+    return y
+
+
+def _snake(x, alpha):
+    return act("snake", x, alpha=alpha.double())
+
+
+def hift_resblock(W, p, x, k, rounding=None, mutate=None):
+    """ResBlock (generator.py:110-117; causal: left-padded convolutions) on x [R, C] (fp32 in the kernels): three dilation steps
+    x += conv2(snake2(conv1(snake1(x), dilation d))), d = 1, 3, 5; the Snake outputs a and ya are the 16-bit operands.  Returns x."""
+    rd = _hrd(rounding)
+    x = x.double()
+    for n, d in enumerate(ohift.RB_DILS):
+        d = 1 if mutate == "dil1" else d
+        a1, a2 = W[f"{p}.activations1.{n}.alpha"], W[f"{p}.activations2.{n}.alpha"]
+        if mutate == "snake_swap":
+            a1, a2 = a2, a1
+        s1, s2 = (-(k - 1) * d, -(k - 1)) if W["causal"] else (-((k - 1) * d) // 2, -(k - 1) // 2)
+        ya = rd(_snake(_conv(rd(_snake(x, a1)), W[f"{p}.convs1.{n}.weight"], W[f"{p}.convs1.{n}.bias"], s1, d), a2))
+        x = x + _conv(ya, W[f"{p}.convs2.{n}.weight"], W[f"{p}.convs2.{n}.bias"], s2)
+    return x
+
+
+def hift_source_downs(W, i, stft, rounding=None, mutate=None):
+    """source_downs[i] on the source STFT rows [F, 18] (the 16-bit operand) -> si [F / s rows at the level's rate, C].  CosyVoice2:
+    Conv1d(k 2s, stride s, padding s / 2) (k 1 at the last level); CosyVoice3: left padding s - 1 only.  The STFT rows given start
+    at frame 120 f of the level's first mel frame f (or at the front pad row at the last level's head)."""
+    s = (15, 3, 1)[i]
+    w, b = W[f"source_downs.{i}.weight"], W[f"source_downs.{i}.bias"]
+    x = stft.double()
+    if s == 1:
+        return x @ w[:, :, 0].t() + b
+    F = x.shape[0]
+    left = (s - 1) if W["causal"] else (7, 1)[i]
+    left += 1 if mutate == "down_pad" else 0
+    xp = torch.nn.functional.pad(x.t()[None], (left, 2 * s))
+    y = torch.nn.functional.conv1d(xp, w, b, stride=s)[0].t()
+    return y[:F // s]
+
+
+def hift_source_branch(W, i, stft, xu, rounding=None, mutate=None):
+    """read-out 3 + 6i: xu + source_resblocks[i](source_downs[i](stft)); stft rows as hift_source_downs takes them, xu the level's
+    rows (the same rows of the sequence)"""
+    si = hift_source_downs(W, i, stft, rounding, mutate)[:xu.shape[0]]
+    return xu.double() + hift_resblock(W, f"source_resblocks.{i}", si, ohift.SRC_RB_KERNELS[i], rounding, mutate)
+
+
+def hift_level_out(i, xs, rounding=None, mutate=None):
+    """read-out 7 + 6i: leaky ReLU(xs / 3), slope 0.1 before the next up-sampler and the default 0.01 before conv_post
+    (generator.py:513, 532), stored as the next convolution's operand"""
+    slope = 0.1 if (i < 2 or mutate == "lrelu_post") else 0.01
+    return _hrd(rounding)(act("lrelu", xs.double() if mutate == "no_div3" else xs.double() / 3, slope))
+
+
+def hift_conv_post(W, x):
+    """read-out 20: conv_post (k7, centred or causal) on the last level output [R, 64] -> [R, 18]"""
+    return _conv(x.double(), W["conv_post.weight"], W["conv_post.bias"], -6 if W["causal"] else -3)
+
+
+def hift_istft(xp, drop=0, mutate=None):
+    """magnitude min(exp(x[:9]), 100), phase sin(x[9:]), inverse real DFT, periodic-Hann overlap-add over the window envelope, trim
+    8, clamp +-0.99 (generator.py:533-538): conv_post rows [F, 18] -> wav [4 (F - 1) - drop]"""
+    x = xp.double()
+    mag = torch.exp(x[:, :9].clamp(max=100.0)) if mutate == "clip_first" else torch.exp(x[:, :9]).clamp(max=100.0)
+    ph = torch.sin(x[:, 9:])
+    re, im = mag * torch.cos(ph), mag * torch.sin(ph)
+    Fr = x.shape[0]
+    w = _hann(mutate)
+    n = torch.arange(16, dtype=torch.float64)
+    ang = 2 * math.pi * torch.arange(9, dtype=torch.float64)[:, None] * n[None] / 16
+    coef = torch.full((9, 1), 2.0, dtype=torch.float64)
+    coef[0] = coef[-1] = 1.0
+    ci = -coef * torch.sin(ang) / 16
+    ci[0] = ci[-1] = 0
+    frames = (re @ (coef * torch.cos(ang) / 16) + im @ ci) * w
+    total = 4 * (Fr - 1) + 16
+    y = torch.zeros(total, dtype=torch.float64)
+    env = torch.zeros(total, dtype=torch.float64)
+    idx = (torch.arange(Fr)[:, None] * 4 + torch.arange(16)[None]).reshape(-1)
+    y.index_add_(0, idx, frames.reshape(-1))
+    env.index_add_(0, idx, (w * w).repeat(Fr))
+    y = y[8:total - 8]
+    if mutate != "no_env":
+        y = y / env[8:total - 8]
+    return y[:y.shape[0] - drop].clamp(-ohift.AUDIO_LIMIT, ohift.AUDIO_LIMIT)
+
+
+def hift_body(W, mel, s, body_frames=None, rounding=None, mutate=None):
+    """the composed body of one sequence, every read-out of cvk_hift_hidden: mel [T, 80], source s [480 T_src] -> list of 21
+    read-outs (fp64).  body_frames: Tb (T by default; a streaming CosyVoice3 call's T - 7, with its STFT cut to 120 Tb + 1 frames)"""
+    Tb = mel.shape[0] if body_frames is None else body_frames
+    stft = hift_stft(s, rounding, mutate)[:120 * Tb + 1]
+    outs = [stft, hift_conv_pre(W, mel, Tb, rounding, mutate)]
+    x = outs[1]
+    for i in range(3):
+        xu = hift_ups(W, i, x, True, mutate)
+        outs.append(xu)
+        xu = hift_source_branch(W, i, stft, xu, rounding, mutate)
+        outs.append(xu)
+        xs = 0
+        for j, k in enumerate(ohift.RB_KERNELS):
+            xs = xs + hift_resblock(W, f"resblocks.{3 * i + j}", xu, k, rounding, mutate)
+            outs.append(xs)
+        x = hift_level_out(i, xs, rounding, mutate)
+        outs.append(x)
+    outs.append(hift_conv_post(W, x))
+    return outs
+
+
+def hift_decode(W, mel, s, finalize=True, rounding=None, mutate=None):
+    """decode of one sequence: (read-outs, wav).  CosyVoice3 streaming (finalize False): mel [T, 80] with T - 3 source frames; the
+    body covers T - 7 frames, the last 480 samples are dropped"""
+    T = mel.shape[0]
+    Tb = T if finalize else T - 7
+    outs = hift_body(W, mel, s, Tb, rounding, mutate)
+    return outs, hift_istft(outs[20], 0 if finalize else ohift.UPSCALE, mutate)
+
+
+# frames of halo a window of a level's rows needs on each side, so that the rows a unit computes from zero padding at the window's
+# cut edges stay outside the frames that are compared: the receptive field of the unit at that rate (an 11-tap resblock with
+# dilations 1, 3, 5 reaches 60 rows each way, twice that to the left when causal; conv_pre 4 frames) rounded up to whole frames
+_HALO = {False: (8, 2, 1), True: (16, 4, 2)}
+
+
+def hift_level_rows(i, f0, f1):
+    """rows of mel frames [f0, f1) at level i (0, 1, 2; -1 the mel rate): the last level's row 0 is the reflect pad, in front of
+    frame 0"""
+    if i < 0:
+        return f0, f1
+    if i < 2:
+        return HIFT_RATE[i] * f0, HIFT_RATE[i] * f1
+    return (0 if f0 == 0 else 120 * f0 + 1), 120 * f1 + 1
+
+
+def _unit_level(u):
+    return -1 if u == 1 else (2 if u in (0, 20) else (u - 2) // 6)
+
+
+def hift_unit_refs(W, K, mel, Tb, windows, rounding=None):
+    """fp64 references of read-outs 1 .. 20 of one sequence, each unit fed the kernel's own read-outs K[u] (fp64, the sequence's
+    rows) of the units before it: per window [fa, fb) of body frames, {u: (reference rows, kernel rows)} of the frames [fa, fb) at
+    the unit's rate, each computed from the window widened by the unit's halo.  mel [T, 80] (T >= Tb: a streaming call's conv_pre
+    reads look-ahead rows past Tb)."""
+    halo = _HALO[W["causal"]]
+    T = mel.shape[0]
+    res = []
+    for fa, fb in windows:
+        out = {}
+
+        def grab(u, g0, g1):
+            lo, hi = hift_level_rows(_unit_level(u), g0, g1)
+            return K[u][lo:hi]
+
+        def keep(u, ref, g0):
+            i = _unit_level(u)
+            base = hift_level_rows(i, g0, g0 + 1)[0]
+            lo, hi = hift_level_rows(i, fa, fb)
+            out[u] = (ref[lo - base:hi - base], K[u][lo:hi])
+
+        g0, g1 = max(0, fa - 5), min(Tb, fb + 5)
+        keep(1, hift_conv_pre(W, mel[g0:min(T, g1 + 5)], g1 - g0, rounding), g0)
+        for i in range(3):
+            h = halo[i]
+            g0, g1 = max(0, fa - h), min(Tb, fb + h)
+            prev = 1 if i == 0 else 7 + 6 * (i - 1)
+            keep(2 + 6 * i, hift_ups(W, i, grab(prev, g0, g1), g0 == 0), g0)
+            if i < 2:
+                stft = K[0][120 * g0:120 * g1 + 1]
+            else:
+                lo, hi = hift_level_rows(2, g0, g1)
+                stft = K[0][lo:hi]
+            keep(3 + 6 * i, hift_source_branch(W, i, stft, grab(2 + 6 * i, g0, g1), rounding), g0)
+            xu = grab(3 + 6 * i, g0, g1)
+            for j, k in enumerate(ohift.RB_KERNELS):
+                xs = grab(3 + 6 * i + j, g0, g1) if j > 0 else 0
+                keep(4 + 6 * i + j, xs + hift_resblock(W, f"resblocks.{3 * i + j}", xu, k, rounding), g0)
+            keep(7 + 6 * i, hift_level_out(i, grab(6 + 6 * i, g0, g1), rounding), g0)
+        g0, g1 = max(0, fa - 1), min(Tb, fb + 1)
+        keep(20, hift_conv_post(W, grab(19, g0, g1)), g0)
+        res.append(out)
+    return res
+
+
+def hift_windows(Tb, seams=(), width=6):
+    """the body frames checked on a long sequence: the head, the tail and `width` frames around every seam frame; the whole
+    sequence when it is short"""
+    if Tb <= 3 * width + 4:
+        return [(0, Tb)]
+    w = [(0, width), (Tb - width, Tb)]
+    for s in seams:
+        if width < s < Tb - width:
+            w.append((s - width // 2, s + width - width // 2))
+    return w
+
+
+def hift_ratio(ref, got):
+    """largest |got - ref| over the rms of its reference row, the row rms floored at a tenth of the mean row rms (a row of a
+    leaky-ReLU output can be nearly zero)"""
+    rms = ref.pow(2).mean(-1, keepdim=True).sqrt()
+    rms = rms.clamp_min(0.1 * rms.mean().item() + 1e-30)
+    r = ((got.double() - ref) / rms).abs().max().item()
+    assert r == r, "NaN"
+    return r
+
+
+HIFT_UNIT_GROUP = {1: "conv_pre", 20: "conv_post", **{2 + 6 * i: "ups" for i in range(3)}, **{3 + 6 * i: "source_branch" for i in range(3)},
+                   **{4 + 6 * i + j: "resblock" for i in range(3) for j in range(3)}, **{7 + 6 * i: "level_out" for i in range(3)}}
+
+
+def hift_source_ulp_bound(W, f0):
+    """what one fp32 ulp of the phase can move the source by: the phase is held in fp32 (the reference's own arithmetic), and one
+    ulp of phase harmonic h (up to 2 rad at 2.7e7 rad) moves sin by up to min(2, ulp), the sine by 0.1 times that and the tanh of the
+    merged source by at most sum_h 0.1 |l_linear_h| min(2, 2 ulp_h) - the rounding of c, of (c 2) pi 480 and of the interpolation
+    each contribute half an ulp.  Plus 1e-5 for the rest of the fp32 arithmetic."""
+    ph = hift_phase(f0).abs().max(0).values.float()
+    ulp = (torch.nextafter(ph, torch.full_like(ph, float("inf"))) - ph).double()
+    return (0.1 * W["m_source.l_linear.weight"][0].abs() * (2 * ulp).clamp(max=2.0)).sum().item() + 1e-5
+
+
+# bounds of test_hift_blocks_gpu.py and test_zz_hift3_blocks_gpu.py: largest |kernel - reference| of a unit over the rms of its
+# reference row (kernel_refs.hift_ratio), fp32 against the exact reference, f16 (hift_f16 = 1, IEEE-half operands) and bf16
+# (hift_f16 = 0) against the reference rounding where the 16-bit path stores; istft: largest |wav - fp64 ISTFT of the kernel's
+# conv_post|; f0: largest error over the utterance's f0 rms (the CosyVoice2 predictor runs fp32 in every mode).  Largest values
+# measured on an H100 80GB HBM3 (700 W) in one run over every length, layout, final and streaming call of both vocoders:
+#   fp32: stft 1.1e-6, conv_pre 4.2e-6, ups 9.5e-6, source_branch 1.0e-5, resblock 8.0e-6, level_out 4.4e-7, conv_post 2.5e-6,
+#     istft 4.5e-6, f0 2.6e-6;
+#   f16: stft 3.4e-3, conv_pre 4.4e-3, ups 1.2e-3, source_branch 4.5e-3, resblock 4.6e-3, level_out 2.5e-3, conv_post 7.1e-4,
+#     istft 4.5e-6;
+#   bf16: stft 2.9e-2, conv_pre 3.5e-2, ups 9.7e-3, source_branch 3.6e-2, resblock 4.0e-2, level_out 1.2e-2, conv_post 6.8e-3,
+#     istft 4.4e-6.
+# (A 16-bit STFT element that the kernel's fp32 sum and the fp64 sum round to neighbouring 16-bit values is one 16-bit ulp apart;
+# over the rms of an 18-column row that is up to the stft ratios above.)  Each bound is about twice the measurement.  source: the
+# largest |source - fp32-emulating source|, measured 4.5e-8; held at 1e-5, far under the 1e-2 .. 1e-1 that one ulp of a long
+# utterance's phase moves the source by.  The CosyVoice3 f0 is held to one fp32 ulp of the fp64-fold predictor (measured 0.5 ulp:
+# correctly rounded).
+HIFT_TOL = {
+    "fp32": dict(stft=2.5e-6, conv_pre=1e-5, ups=2e-5, source_branch=2e-5, resblock=1.6e-5, level_out=1e-6, conv_post=5e-6, istft=1e-5,
+                 f0=5e-6),
+    "f16": dict(stft=7e-3, conv_pre=9e-3, ups=2.5e-3, source_branch=9e-3, resblock=1e-2, level_out=5e-3, conv_post=1.5e-3, istft=1e-5,
+                f0=5e-6),
+    "bf16": dict(stft=6e-2, conv_pre=7e-2, ups=2e-2, source_branch=7e-2, resblock=8e-2, level_out=2.5e-2, conv_post=1.4e-2, istft=1e-5,
+                 f0=5e-6),
+    "source": 1e-5,
+}

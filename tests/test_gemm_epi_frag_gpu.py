@@ -12,6 +12,7 @@ dilation and a shift.  Which kernel ran is read from a torch.profiler trace.  Th
 the flow stages (tools/epi_ab.py compares the flow stage's mels and bench.py's waveforms under both values)."""
 import pytest
 import torch
+from torch.autograd import DeviceType
 from torch.profiler import ProfilerActivity, profile
 
 import kernel_refs as kr
@@ -67,11 +68,16 @@ class Case:
         c.set_option("tc_persist", tc_persist)
         c.set_option("flow_qkv_panel", panel)
         try:
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                out, out2 = c.conv_gemm(self.x, [s for s, _ in self.seqs], [n for _, n in self.seqs], self.w, self.bias, self.dil, self.shift0,
-                                        self.operand, self.act1, 0.1, self.alpha1, self.resid, False, self.accumulate, self.out_init, self.out,
-                                        self.act2 or "none", 0.2, self.alpha2, self.out2_init, self.out2)
-                torch.cuda.synchronize()
+            # the launch is deterministic, so a trace that came back without any device-side record (the profiler lost the window's
+            # GPU activity, as it occasionally does on a shared device) is taken again; the caller still requires the kernel's name
+            for _ in range(3):
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    out, out2 = c.conv_gemm(self.x, [s for s, _ in self.seqs], [n for _, n in self.seqs], self.w, self.bias, self.dil,
+                                            self.shift0, self.operand, self.act1, 0.1, self.alpha1, self.resid, False, self.accumulate,
+                                            self.out_init, self.out, self.act2 or "none", 0.2, self.alpha2, self.out2_init, self.out2)
+                    torch.cuda.synchronize()
+                if any(e.device_type == DeviceType.CUDA for e in prof.key_averages()):
+                    break
         finally:
             c.set_option("tc_epi_frag", 1)
             c.set_option("tc_epi", 2)

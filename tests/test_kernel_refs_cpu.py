@@ -1,6 +1,7 @@
 """CPU: the fp64 references of test_kernel_edges_gpu.py and test_kernel_epilogues_gpu.py (tests/kernel_refs.py) against independent
 formulations - torch's scaled_dot_product_attention with an explicit mask and expanded K/V heads, one KV-cached step of the oracle
 Qwen2 LM, F.conv1d with torch's activations, and the oracle conformer layer's relative-position attention."""
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -577,3 +578,171 @@ def test_flow_mutations_exceed_bounds(precision):
             assert shares[m] < 0.1, (m, shares[m])
         else:
             assert shares[m] >= need, (m, shares[m], need)
+
+
+# ------------------------------------------------------------------------------------------------ HiFT vocoders
+def _hift_oracle_sd(causal):
+    from oracle import hift_causal as ohc, weights as oweights
+    return oweights.synth_state_dict((ohc if causal else ohift).param_shapes(), 1986, ohift.SYNTH_GAINS)
+
+
+def test_hift_ref_composed_equals_oracle_and_goldens(golden):
+    """the fp64 units composed (f0, source, body, ISTFT) against oracle.hift.decode and the reference's outputs hift_b2_t24 and
+    hift_cache_source at fp32 tolerance; the fp32-emulating source against the goldens to 1e-7"""
+    from oracle import cases
+    sd = _hift_oracle_sd(False)
+    W = kr.hift_weights(sd, False)
+    g, gc = golden("hift_b2_t24"), golden("hift_cache_source")
+    mel, noise, _ = cases.hift_case()
+    for b in range(2):
+        s = torch.from_numpy(g["source"][b, 0])
+        outs, wav = kr.hift_decode(W, mel[b].t(), s)
+        pre = ohift.decode(sd, mel[b:b + 1], s[None, None], return_pre_istft=True)[0].t().double()
+        assert (outs[20] - pre).abs().max() < 5e-5
+        assert (wav - ohift.decode(sd, mel[b:b + 1], s[None, None])[0].double()).abs().max() < 1e-5
+        assert (wav - torch.from_numpy(g["decode"][b]).double()).abs().max() < 1e-5
+        assert (kr.hift_f0(W, mel[b].t()) - torch.from_numpy(g["f0"][b]).double()).abs().max() < 2e-4
+        f0 = torch.from_numpy(g["f0"][b])
+        assert (kr.hift_source(W, f0, noise[b], emulate=True) - s.double()).abs().max() < 1e-7
+        assert (kr.hift_source(W, f0, noise[b]) - s.double()).abs().max() < 1e-4
+    _, wav = kr.hift_decode(W, mel[0].t(), torch.from_numpy(gc["source"][0, 0]))
+    assert (wav - torch.from_numpy(gc["wav"][0]).double()).abs().max() < 1e-5
+
+
+def test_hift3_ref_composed_equals_oracle_and_golden(golden):
+    """the causal units against oracle.hift_causal.inference and the reference's hift_causal outputs, final and streaming; the
+    fp64-fold f0 predictor equals the reference's float64 predictor to within fp32 rounding of its output"""
+    from oracle import cases, hift_causal as ohc
+    sd = _hift_oracle_sd(True)
+    W = kr.hift_weights(sd, True)
+    g = golden("hift_causal")
+    mel, rand_ini, sine_noise = cases.hift_causal_case()
+    m = mel[0].t()
+    f0 = kr.hift_f0(W, m)
+    assert (f0.float() - torch.from_numpy(g["f0_final"][0])).abs().max() == 0
+    assert (f0[:21].float() - torch.from_numpy(g["f0_chunk"][0])).abs().max() == 0
+    for fin, n, key in ((True, 24, "final"), (False, 21, "chunk")):
+        s = kr.hift_source(W, torch.from_numpy(g[f"f0_{key}"][0]), sine_noise[0], emulate=True)
+        assert s.shape[0] == 480 * n and (s - torch.from_numpy(g[f"source_{key}"][0, 0]).double()).abs().max() < 1e-7
+        _, wav = kr.hift_decode(W, m, torch.from_numpy(g[f"source_{key}"][0, 0]), finalize=fin)
+        assert (wav - torch.from_numpy(g[f"wav_{key}"][0]).double()).abs().max() < 2e-5, key
+        ow, _ = ohc.inference(sd, mel, rand_ini, sine_noise, fin)
+        assert (wav - ow[0].double()).abs().max() < 2e-5, key
+
+
+def test_hift_windows_equal_whole_sequence():
+    """a unit computed on a window of a sequence's rows widened by kernel_refs' halo equals the whole-sequence composition on the
+    window's frames (head, tail, interior), final, causal and causal streaming; and a one-row defect in a read-out is seen"""
+    for causal in (False, True):
+        W = kr.hift_weights(kr.hift_test_state_dict(7, causal), causal)
+        g = torch.Generator().manual_seed(3)
+        T = 44
+        mel = torch.randn(T, 80, generator=g) * 2 - 5
+        s = torch.tanh(torch.randn(480 * T, generator=g))
+        for fin in ((True, False) if causal else (True,)):
+            Tb = T if fin else T - 7
+            K = kr.hift_body(W, mel, s[:480 * (T if fin else T - 3)], Tb, "fp16")
+            res = kr.hift_unit_refs(W, K, mel, Tb, kr.hift_windows(Tb, (20,), 6), "fp16")
+            assert [sorted(w) for w in res] == [list(range(1, 21))] * 3
+            assert max(kr.hift_ratio(r, k) for w in res for r, k in w.values()) == 0.0
+            K[12] = K[12].clone()
+            K[12][40 * 21] += 1.0                          # one row of level 1, frame 21
+            res = kr.hift_unit_refs(W, K, mel, Tb, [(18, 24)], "fp16")
+            assert kr.hift_ratio(*res[0][13]) > 1e-3
+
+
+def test_hift_emulated_source_matches_oracle():
+    """the fp32-emulating source equals oracle.hift.sine_source (torch's CPU arithmetic, which the kernel follows) to 1e-6 at every
+    sample at T = 24, 500 and 1500 - no phase-ulp mismatch - while the separately rounded interpolation l0 p0 + l1 p1 (what the
+    kernel would compute without FMA contraction) misses it on a growing number of samples and the exact fp64 source differs by up
+    to the 1-ulp phase effect"""
+    sd = _hift_oracle_sd(False)
+    W = kr.hift_weights(sd, False)
+    for T, n_unfused in ((24, 10000), (500, 300000), (1500, 1000000)):
+        g = torch.Generator().manual_seed(T)
+        f0 = 80 + 320 * torch.rand(T, generator=g)
+        noise = torch.randn(480 * T, 9, generator=g)
+        o = ohift.sine_source(sd, f0[None], noise[None])[0, 0].double()
+        d = (o - kr.hift_source(W, f0, noise, emulate=True)).abs()
+        assert int((d > 1e-6).sum()) == 0, (T, d.max().item())
+        ph = kr.hift_phase(f0, emulate=True).numpy().astype(np.float32)
+        i0, i1, l0, l1 = kr._interp_index(480 * T, T)
+        sep = ((l0[:, None] * ph[i0]).astype(np.float32) + (l1[:, None] * ph[i1]).astype(np.float32)).astype(np.float32)
+        fused = kr.hift_sample_phase(torch.from_numpy(ph.astype(np.float64)), False, emulate=True).numpy()
+        n_diff = int((sep != fused).sum())
+        print(f"T={T}: {n_diff} of {sep.size} phase samples differ without contraction; exact source differs by "
+              f"{(o - kr.hift_source(W, f0, noise)).abs().max().item():.3g}")
+        assert n_diff >= n_unfused, (T, n_diff)
+        assert (o - kr.hift_source(W, f0, noise)).abs().max().item() <= kr.hift_source_ulp_bound(W, f0)
+
+
+_HIFT_MUT_UNIT = dict(lrelu_post="level_out", no_reflect="ups", reflect_back="ups", down_pad="source_branch", poly_phase="ups",
+                      snake_swap="resblock", dil1="resblock", no_div3="level_out", hann_sym="stft", no_env="istft", phase_x="source",
+                      clip_first="istft", uv_ge="source", pre_left="conv_pre", f0_look2="f0")
+
+
+def _hift_mutation_shares(mode):
+    """share of the elements that each defect of kr.HIFT_MUTATIONS, injected into the reference of its mode (exact for fp32, rounding
+    to IEEE half for f16, to bf16 for bf16), moves beyond the bound test_hift_blocks_gpu.py holds that unit to (kr.HIFT_TOL).  A
+    defect lives in one unit, so the first read-out it changes is that unit fed the unmutated inputs; it is judged there, per element
+    over the reference row's rms (istft and source: absolute; f0: in fp32 ulps, against one ulp)."""
+    rnd = {"fp32": None, "f16": "fp16", "bf16": "bf16"}[mode]
+    tol = kr.HIFT_TOL[mode]
+    shares = {}
+    g = torch.Generator().manual_seed(12)
+    T = 14
+    mel = torch.randn(T, 80, generator=g) * 2 - 5
+    s = torch.tanh(3 * torch.randn(480 * T, generator=g))
+    f0 = torch.full((T,), 10.0)
+    f0[T // 2:] = 150.0
+    noise = torch.randn(480 * T, 9, generator=g)
+    for causal in (False, True):
+        W = kr.hift_weights(kr.hift_test_state_dict(5, causal, clip=True), causal)
+        ref, wav = kr.hift_decode(W, mel, s, rounding=rnd)
+        for m in kr.HIFT_MUTATIONS:
+            unit = _HIFT_MUT_UNIT[m]
+            if (m in ("pre_left", "f0_look2")) != causal:
+                continue
+            if unit == "f0":
+                a, b = kr.hift_f0(W, mel), kr.hift_f0(W, mel, mutate=m)
+                r = a.float().abs()
+                shares[m] = (((b - a).abs() / (torch.nextafter(r, r + 1) - r).double()) > 1.0).double().mean().item()
+            elif unit == "source":
+                a, b = kr.hift_source(W, f0, noise), kr.hift_source(W, f0, noise, mutate=m)
+                shares[m] = ((b - a).abs() > kr.HIFT_TOL["source"]).double().mean().item()
+            elif unit == "istft":
+                a, b = kr.hift_istft(ref[20]), kr.hift_istft(ref[20], mutate=m)
+                shares[m] = ((b - a).abs() > tol["istft"]).double().mean().item()
+            else:
+                mut, _ = kr.hift_decode(W, mel, s, rounding=rnd, mutate=m)
+                u = next(i for i in range(21) if mut[i].shape != ref[i].shape or not torch.equal(mut[i], ref[i]))
+                # a resblock defect shows first in the source branch, whose source resblock comes first
+                assert kr.HIFT_UNIT_GROUP.get(u, "stft") in (unit, "source_branch" if unit == "resblock" else unit), (m, u)
+                unit = kr.HIFT_UNIT_GROUP.get(u, "stft")
+                a, b = ref[u], mut[u]
+                if a.shape != b.shape:
+                    n = min(a.shape[0], b.shape[0])
+                    a, b = a[:n], b[:n]
+                rms = a.pow(2).mean(-1, keepdim=True).sqrt().clamp_min(1e-30)
+                shares[("c_" if causal else "") + m] = ((b - a).abs() / rms > tol[unit]).double().mean().item()
+    return shares
+
+
+# share of the elements beyond the GPU bound that each defect must move, in every mode (fp32, f16, bf16): all of them are caught in
+# all three.  Measured on this case (fp32 / f16 / bf16): lrelu_post 0.52 / 0.50 / 0.44, reflect_back, down_pad, poly_phase, dil1,
+# no_div3 0.94 - 1.0, snake_swap 1.0 / 0.98 / 0.84, hann_sym 0.89 / 0.85 / 0.59, causal pre_left 1.0 / 0.96 / 0.75; mode-independent:
+# no_reflect 6e-4 (the one front row of 1681 it changes, changed beyond the bound), no_env 0.10 and clip_first 0.27 (most samples of
+# the clip=True waveform sit on the +-0.99 clamp, where neither defect shows), phase_x and uv_ge 0.5 (the voiced half of the crafted
+# f0; uv_ge on the frames at exactly 10 Hz), f0_look2 1.0 (in fp32 ulps of the fp64 predictor).
+HIFT_CAUGHT = dict(lrelu_post=0.25, no_reflect=5e-4, reflect_back=0.5, down_pad=0.5, poly_phase=0.5, snake_swap=0.5, dil1=0.5,
+                   no_div3=0.5, hann_sym=0.3, no_env=0.05, phase_x=0.25, clip_first=0.1, uv_ge=0.25, c_pre_left=0.3, f0_look2=0.5)
+
+
+@pytest.mark.parametrize("mode", ["fp32", "f16", "bf16"])
+def test_hift_mutations_exceed_bounds(mode):
+    """each defect of kr.HIFT_MUTATIONS moves at least the stated share of its unit's elements beyond the bound of its mode"""
+    shares = _hift_mutation_shares(mode)
+    print(mode, {k: round(v, 4) for k, v in shares.items()})
+    assert set(HIFT_CAUGHT) == set(shares)
+    for m, need in HIFT_CAUGHT.items():
+        assert shares[m] >= need, (m, shares[m], need)

@@ -28,7 +28,7 @@ def test_hift3_offline_golden(precision, golden):
     c = model(precision)
     c.hift3_set_noise(rand_ini, sine_noise[0])
     wav, f0, src = c.hift3_inference(mel[0].t().contiguous(), [mel.shape[2]], finalize=True)
-    np.testing.assert_allclose(f0.cpu().numpy(), g["f0_final"][0], rtol=1e-4, atol=1e-2)         # float64 predictor (weight-norm folded in fp32)
+    np.testing.assert_allclose(f0.cpu().numpy(), g["f0_final"][0], rtol=1e-4, atol=1e-2)         # float64 predictor (weight norm folded in float64)
     assert maxdiff(src, torch.from_numpy(g["source_final"]).reshape(-1)) < 2e-3
     d = maxdiff(wav, torch.from_numpy(g["wav_final"]).reshape(-1))
     # bf16 (IEEE-half vocoder operands): largest |d| measured on an H100 80GB HBM3 (700 W) 1.12e-2 on |wav| <= 1; the bound is about twice
